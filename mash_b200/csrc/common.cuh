@@ -57,7 +57,7 @@ struct mashgpu_ctx {
     double scan_ms = 0, dist_ms = 0;
     std::vector<mashgpu::EventPair> scan_events, dist_events;
     // sketch_stream_core scratch
-    mashgpu::Scratch sc_start, sc_t, sc_off, sc_log2, sc_flags, sc_maxhash, sc_keys, sc_cnt, sc_tmax, sc_first, sc_last, sc_qtarget, sc_qtstar;
+    mashgpu::Scratch sc_start, sc_t, sc_off, sc_log2, sc_flags, sc_maxhash, sc_keys, sc_cnt, sc_tmax, sc_tunit, sc_first, sc_last, sc_qtarget, sc_qtstar;
     // mashgpu_sketch_batch: wave stream buffers and outputs
     mashgpu::Scratch sc_wave[2], sc_inval[2], sc_runs[2], sc_out_hashes, sc_out_n, sc_out_counts;
     mashgpu::Scratch sc_sep[2], sc_codes[2];

@@ -10,40 +10,10 @@ namespace mashgpu {
 //   x * const  -> IMAD.WIDE.U32 + 2 IMAD          rotl -> 2 SHF (funnel)        add -> IADD3 + IADD3.X
 struct u64x2 { uint32_t lo, hi; };
 
-// ---- pipe balancing -----------------------------------------------------------------------------------------
-// The hot loop is bound by the ALU pipe (SHF/LOP3/IADD3/PRMT; the FMA pipe is far less busy).  Shifts,
-// rotates and 64-bit adds can also be done by the integer multiply-add unit (IMAD / IMAD.WIDE / IMAD.HI on the FMA
-// pipe) if the multiplier is a power of two -- but ptxas strength-reduces a literal power of two back into
-// SHF/LEA/IADD3.  Reading the multipliers from constant memory keeps them opaque (the IMAD takes the constant-bank
-// operand directly, no register needed).  Each MG_*_FMA switch moves one class of operations to the FMA pipe.
-// Every switch made tools/scan_microbench.cu (k=21 canonical) slower -- IMAD.WIDE/IMAD.HI cost more issue slots than the
-// SHF/IADD3 they replace -- so every switch defaults to 0.  Kept as documented dead ends.
-#ifndef MG_ROT_FMA
-#define MG_ROT_FMA 0
-#endif
-#ifndef MG_SHR_FMA
-#define MG_SHR_FMA 0
-#endif
-#ifndef MG_ADD_FMA
-#define MG_ADD_FMA 0
-#endif
-#ifndef MG_SEL_FMA
-#define MG_SEL_FMA 0
-#endif
-// g_pow2[i] = 2^i (i = 0..31)
-static __constant__ uint32_t g_pow2[32] = {
-    1u << 0, 1u << 1, 1u << 2, 1u << 3, 1u << 4, 1u << 5, 1u << 6, 1u << 7, 1u << 8, 1u << 9, 1u << 10, 1u << 11, 1u << 12, 1u << 13, 1u << 14, 1u << 15,
-    1u << 16, 1u << 17, 1u << 18, 1u << 19, 1u << 20, 1u << 21, 1u << 22, 1u << 23, 1u << 24, 1u << 25, 1u << 26, 1u << 27, 1u << 28, 1u << 29, 1u << 30, 1u << 31};
-
-// x >> S on the FMA pipe: high word of x * 2^(32-S)
-template <int S>
-__device__ __forceinline__ uint32_t shr_fma(uint32_t x)
-{
-    static_assert(S >= 1 && S <= 31, "shift");
-    uint32_t r;
-    asm("mul.hi.u32 %0, %1, %2;" : "=r"(r) : "r"(x), "r"(g_pow2[32 - S]));
-    return r;
-}
+// The hot loop is bound by the ALU pipe (SHF/LOP3/IADD3/PRMT).  Moving 64-bit adds, shifts, rotates or the PRMT selector
+// shift onto the FMA pipe through opaque power-of-two IMADs made the k=21 scan slower on B200 and on H100 (IMAD.WIDE/IMAD.HI
+// cost more issue slots than the SHF/IADD3 they replace); the scan uses the FMA pipe only where an add can ride on a
+// multiply-add that is there anyway (fmix_hi).
 
 __device__ __forceinline__ u64x2 mul_const(u64x2 a, uint64_t c)
 {
@@ -60,14 +30,6 @@ __device__ __forceinline__ u64x2 rotl(u64x2 a)
 {
     u64x2 r;
     if constexpr (R == 32) { r.lo = a.hi; r.hi = a.lo; }
-    else if constexpr (MG_ROT_FMA) {
-        // rotl by R' = R mod 32 of (h:l) [halves pre-swapped when R > 32]:  l*2^R' (wide) + {h >> (32-R'), h << R'}
-        const uint32_t l = R < 32 ? a.lo : a.hi, h = R < 32 ? a.hi : a.lo;
-        const uint32_t c = g_pow2[R & 31];
-        asm("{\n\t.reg .u64 t;\n\t.reg .u32 x, y;\n\tmul.hi.u32 x, %3, %4;\n\tmul.lo.u32 y, %3, %4;\n\tmov.b64 t, {x, y};\n\t"
-            "mad.wide.u32 t, %2, %4, t;\n\tmov.b64 {%0, %1}, t;\n\t}"
-            : "=r"(r.lo), "=r"(r.hi) : "r"(l), "r"(h), "r"(c));
-    }
     else if constexpr (R < 32) { r.hi = __funnelshift_l(a.lo, a.hi, R); r.lo = __funnelshift_l(a.hi, a.lo, R); }
     else { r.hi = __funnelshift_l(a.hi, a.lo, R - 32); r.lo = __funnelshift_l(a.lo, a.hi, R - 32); }
     return r;
@@ -76,13 +38,7 @@ __device__ __forceinline__ u64x2 rotl(u64x2 a)
 __device__ __forceinline__ u64x2 add64(u64x2 a, u64x2 b)
 {
     u64x2 r;
-#if MG_ADD_FMA
-    // a.lo * 1 + b (wide) carries into the high word; then + a.hi
-    asm("{\n\t.reg .u64 t;\n\tmov.b64 t, {%4, %5};\n\tmad.wide.u32 t, %2, %6, t;\n\tmov.b64 {%0, %1}, t;\n\tmad.lo.u32 %1, %3, %6, %1;\n\t}"
-        : "=r"(r.lo), "=&r"(r.hi) : "r"(a.lo), "r"(a.hi), "r"(b.lo), "r"(b.hi), "r"(g_pow2[0]));
-#else
     asm("add.cc.u32 %0, %2, %4;\n\taddc.u32 %1, %3, %5;" : "=r"(r.lo), "=r"(r.hi) : "r"(a.lo), "r"(a.hi), "r"(b.lo), "r"(b.hi));
-#endif
     return r;
 }
 
@@ -98,14 +54,7 @@ __device__ __forceinline__ u64x2 mul5_add(u64x2 a, uint32_t c)
     return r;
 }
 
-__device__ __forceinline__ uint32_t shr1(uint32_t x)
-{
-#if MG_SHR_FMA
-    return shr_fma<1>(x);
-#else
-    return x >> 1;
-#endif
-}
+__device__ __forceinline__ uint32_t shr1(uint32_t x) { return x >> 1; }
 
 __device__ __forceinline__ u64x2 fmix(u64x2 k)
 {
@@ -117,10 +66,22 @@ __device__ __forceinline__ u64x2 fmix(u64x2 k)
     return k;
 }
 
-// a[i] = ASCII bytes 4i..4i+3 of the k-mer (little endian, byte 0 = first base), bytes >= K zeroed.
-// NA = 2*ceil(K/8) words.  Returns h1 (the first 8 bytes of the 128-bit digest).
+// high word of fmix(k), plus `add` (the final `k ^= k >> 33` only changes the low word).  The addend enters the first
+// multiply-add (IMAD.HI), so summing two of these and a constant stays on the FMA pipe.
+__device__ __forceinline__ uint32_t fmix_hi(u64x2 k, uint32_t add)
+{
+    k.lo ^= shr1(k.hi);
+    k = mul_const(k, 0xff51afd7ed558ccdULL);
+    k.lo ^= shr1(k.hi);
+    constexpr uint64_t c = 0xc4ceb9fe1a85ec53ULL;
+    uint32_t r;
+    asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(k.lo), "n"((uint32_t)c), "r"(add));
+    return r + k.lo * (uint32_t)(c >> 32) + k.hi * (uint32_t)c;
+}
+
+// The body of MurmurHash3_x64_128 up to the finalisation: h1, h2 after the length xor and the two cross adds.
 template <int K, int NA>
-__device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t seed)
+__device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t seed, u64x2 &h1_out, u64x2 &h2_out)
 {
     constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
     constexpr int NB = K / 16, TAIL = K & 15;
@@ -143,9 +104,41 @@ __device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t se
     }
     h1.lo ^= (uint32_t)K; h2.lo ^= (uint32_t)K;
     h1 = add64(h1, h2); h2 = add64(h2, h1);
+    h1_out = h1; h2_out = h2;
+}
+
+// a[i] = ASCII bytes 4i..4i+3 of the k-mer (little endian, byte 0 = first base), bytes >= K zeroed.
+// NA = 2*ceil(K/8) words.  Returns h1 (the first 8 bytes of the 128-bit digest).
+template <int K, int NA>
+__device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t seed)
+{
+    u64x2 h1, h2;
+    murmur3_body<K, NA>(a, seed, h1, h2);
     h1 = fmix(h1); h2 = fmix(h2);
     h1 = add64(h1, h2);
     return h1;
+}
+
+// Filter word of h1 for the scan's fast path: X = hi(fmix(h1)) + hi(fmix(h2)) + 1 (mod 2^32), the high word of h1 with
+// the carry out of the low words (never computed) replaced by 1.  With H the exact high word of h1 and T < 2^32 - 1,
+//   H <= T  implies  X <= T + 1
+// (carry 0: X = H + 1 <= T + 1;  carry 1: X = H), so `X <= T + 1` (or anything, when T = 2^32 - 1) never rejects a hash
+// whose high word is <= T.  It lets through at most the one extra high word T + 1 and X = 0 (high words summing to
+// 2^32 - 1); the slow path recomputes the exact hash.  tests/test_scan_filter_model.py models this predicate.
+template <int K, int NA>
+__device__ __forceinline__ uint32_t murmur3_h1_filter(const uint32_t (&a)[NA], uint32_t seed)
+{
+    u64x2 h1, h2;
+    murmur3_body<K, NA>(a, seed, h1, h2);
+    uint32_t one;    // opaque, so that ptxas keeps the +1 as the IMAD.HI addend rather than a separate add on the ALU pipe
+    asm("mov.u32 %0, 1;" : "=r"(one));
+    return fmix_hi(h2, fmix_hi(h1, one));
+}
+
+// threshold for murmur3_h1_filter's word, from the exact high-word threshold T = tmax >> 32: T + 1, saturated at 2^32 - 1
+__host__ __device__ __forceinline__ uint32_t filter_threshold(uint32_t t_hi)
+{
+    return t_hi + (t_hi != 0xFFFFFFFFu ? 1u : 0u);
 }
 
 }  // namespace mashgpu

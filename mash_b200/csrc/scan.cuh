@@ -15,6 +15,7 @@
 // Only hashes at or below the tile's coarse threshold leave the fast path.
 #pragma once
 #include <cstdint>
+#include <utility>
 #include "murmur3.cuh"
 
 namespace mashgpu {
@@ -38,6 +39,8 @@ struct ScanArgs {
     uint64_t stream_len;          // positions >= stream_len are treated as separators
     uint64_t tile_begin, tile_end;
     const uint64_t *tile_tmax;    // per-tile coarse threshold (indexed by absolute tile id); NULL -> coarse_t
+    const uint32_t *tile_unit;    // per-tile first unit: last u with unit_start[u] <= the tile's first position (absolute
+                                  //   tile id); NULL -> the slow path binary-searches unit_start
     uint64_t coarse_t;
     uint32_t seed;
     int use64;
@@ -118,13 +121,20 @@ static __device__ __noinline__ void scan_emit(const ScanArgs &a, uint32_t hash_l
         return;
     }
     // (screen: the reference table was probed by screen_probe_lanes before the survivors were serialised)
-    // unit of this position: last u with unit_start[u] <= pos
-    uint32_t lo = 0, hi = a.n_units;
-    while (hi - lo > 1) {
-        uint32_t mid = (lo + hi) >> 1;
-        if (a.unit_start[mid] <= pos) lo = mid; else hi = mid;
+    // unit of this position: last u with unit_start[u] <= pos -- from the tile's first unit a tile rarely spans more than one
+    // or two units, so a forward scan of a load or two replaces a binary search of ~log2(n_units) dependent loads
+    uint32_t u;
+    if (a.tile_unit) {
+        u = a.tile_unit[pos / SCAN_TILE];
+        while (u + 1 < a.n_units && a.unit_start[u + 1] <= pos) u++;
+    } else {
+        uint32_t lo = 0, hi = a.n_units;
+        while (hi - lo > 1) {
+            uint32_t mid = (lo + hi) >> 1;
+            if (a.unit_start[mid] <= pos) lo = mid; else hi = mid;
+        }
+        u = lo;
     }
-    const uint32_t u = lo;
     if (a.only_unit >= 0 && (int64_t)u != a.only_unit) return;
     if (hash > a.unit_t[u]) return;
     if (a.mode == SCAN_EVENTS) {
@@ -163,10 +173,15 @@ static __device__ __noinline__ void scan_emit(const ScanArgs &a, uint32_t hash_l
 // window validity from the warp's tile: DNA kernels keep nibbles (bit 3 = outside the alphabet), byte kernels bytes (0 = outside)
 __device__ __forceinline__ bool window_valid(const uint32_t *sm_tile, uint32_t lp, int k)
 {
-    if (k > 0) {
+    if (k > 0) {   // bit 3 of the window's k nibbles, a word (8 nibbles) at a time
+        const uint32_t w = lp >> 3, sh = 4 * (lp & 7);
         uint32_t bad = 0;
-        for (int i = 0; i < k; i++) bad |= sm_tile[(lp + i) >> 3] >> (4 * ((lp + i) & 7));
-        return !(bad & 8u);
+        for (int i = 0; 8 * i < k; i++) {
+            uint32_t x = __funnelshift_r(sm_tile[w + i], sm_tile[w + i + 1], sh);
+            if (k - 8 * i < 8) x &= (1u << (4 * (k - 8 * i))) - 1u;
+            bad |= x;
+        }
+        return !(bad & 0x88888888u);
     }
     const uint8_t *bytes = reinterpret_cast<const uint8_t *>(sm_tile);
     bool ok = true;
@@ -275,48 +290,130 @@ struct KmerShape {
     static constexpr int BW = (K + 7 + 7) / 8;       // nibble words per block of 8 window starts
     static constexpr int NA = 2 * NW;                // ASCII words per k-mer
     static constexpr uint32_t LAST_MASK = (K % 8) ? ((1u << (4 * (K % 8))) - 1u) : 0xFFFFFFFFu;
+    // the nibbles of the last word past the k-mer hold code 8: PRMT's sign-replicate of byte 0 of the pool ('A' = 0x41)
+    // turns them into 0x00 bytes, which is what MurmurHash3 reads past the key.  Both strands carry the same padding in
+    // their most significant nibbles, so the canonical compare is decided by the k-mer's own nibbles as before.
+    static constexpr uint32_t LAST_PAD = 0x88888888u & ~LAST_MASK;
 };
 
-// nibble words (codes 0..3) -> ASCII words, bytes >= K zeroed
+// nibble words (codes 0..3, padded with code 8 past K) -> ASCII words, bytes >= K zeroed
 template <int K>
 __device__ __forceinline__ void expand_ascii(const uint32_t (&c)[KmerShape<K>::NW], uint32_t (&a)[KmerShape<K>::NA], uint32_t POOL)
 {
 #pragma unroll
     for (int i = 0; i < KmerShape<K>::NW; i++) {
-        uint32_t lo = prmt(POOL, 0, c[i]);
-#if MG_SEL_FMA
-        uint32_t hi = prmt(POOL, 0, shr_fma<16>(c[i]));
-#else
-        uint32_t hi = prmt(POOL, 0, c[i] >> 16);
-#endif
-        const int rem_lo = K - 8 * i;      // bases left for word 2i
-        const int rem_hi = K - 8 * i - 4;  // bases left for word 2i+1
-        if (rem_lo < 4) lo &= (1u << (8 * rem_lo)) - 1u;
-        if (rem_hi <= 0) hi = 0;
-        else if (rem_hi < 4) hi &= (1u << (8 * rem_hi)) - 1u;
-        a[2 * i] = lo;
-        a[2 * i + 1] = hi;
+        a[2 * i] = prmt(POOL, 0, c[i]);
+        a[2 * i + 1] = K - 8 * i - 4 <= 0 ? 0u : prmt(POOL, 0, c[i] >> 16);   // no base left for word 2i+1: zero
     }
 }
 
-#ifndef SCAN_RC_SMEM
-#define SCAN_RC_SMEM 1         // keep a reverse-complement image of the tile in shared memory (see scan_kernel)
-#endif
+// canonical k-mer of a window: c = rc when rc < fwd as little-endian multi-word integers  <=>  memcmp(fwd, rc, k) > 0
+// (Sketch.cpp:569-571): borrow out of rc - fwd.  m = all-ones when the reverse complement is the canonical k-mer.
+template <int K>
+__device__ __forceinline__ void canonical_words(const uint32_t (&f)[KmerShape<K>::NW], const uint32_t (&r)[KmerShape<K>::NW],
+                                                uint32_t (&c)[KmerShape<K>::NW])
+{
+    using S = KmerShape<K>;
+    uint32_t m;
+    if (S::NW == 1) {
+        asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.u32 %0, 0, 0;\n\t}" : "=r"(m) : "r"(r[0]), "r"(f[0]));
+    } else if (S::NW == 2) {
+        asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.u32 %0, 0, 0;\n\t}"
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]));
+    } else if (S::NW == 3) {
+        asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.u32 %0, 0, 0;\n\t}"
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]));
+    } else {
+        asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.cc.u32 t, %7, %8;\n\tsubc.u32 %0, 0, 0;\n\t}"
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]),
+              "r"(r[S::NW > 3 ? 3 : 0]), "r"(f[S::NW > 3 ? 3 : 0]));
+    }
+#pragma unroll
+    for (int i = 0; i < S::NW; i++) c[i] = (f[i] & ~m) | (r[i] & m);
+}
+
+__device__ __forceinline__ uint32_t lds_u32(uint32_t addr)
+{
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+
+// Exact hash of the window at nibble `lp` of a warp tile (shared-memory address sm_addr), rebuilt from the tile's nibble
+// words alone: forward words by funnel shifts, reverse complement by nibble reversal of those.  Returns false when the
+// window holds a base outside the alphabet (bit 3 of a nibble).
+template <int K, bool CANON>
+__device__ __forceinline__ bool window_hash(const ScanArgs &a, uint32_t sm_addr, uint32_t lp, uint64_t &hash)
+{
+    using S = KmerShape<K>;
+    uint32_t x[S::NW + 1], f[S::NW], c[S::NW];
+    const uint32_t w = sm_addr + 4 * (lp >> 3), sh = 4 * (lp & 7);
+#pragma unroll
+    for (int i = 0; i <= S::NW; i++) x[i] = lds_u32(w + 4 * i);     // word index <= 127 + 4 < SCAN_WARP_WORDS
+    uint32_t bad = 0;
+#pragma unroll
+    for (int i = 0; i < S::NW; i++) {
+        f[i] = __funnelshift_r(x[i], x[i + 1], sh);
+        if (i == S::NW - 1) f[i] = (f[i] & S::LAST_MASK) | S::LAST_PAD;
+        bad |= i == S::NW - 1 ? f[i] & S::LAST_MASK : f[i];
+    }
+    if (CANON) {
+        // rr = the 8 NW nibbles of f reversed and complemented; the reverse complement starts P = 8 NW - K nibbles in
+        constexpr int P = 8 * S::NW - K;
+        uint32_t rr[S::NW + 1], r[S::NW];
+#pragma unroll
+        for (int i = 0; i < S::NW; i++) rr[i] = nibble_reverse(f[S::NW - 1 - i]) ^ 0x33333333u;
+        rr[S::NW] = 0;
+#pragma unroll
+        for (int i = 0; i < S::NW; i++) {
+            r[i] = P ? __funnelshift_r(rr[i], rr[i + 1], 4 * P) : rr[i];
+            if (i == S::NW - 1) r[i] = (r[i] & S::LAST_MASK) | S::LAST_PAD;
+        }
+        canonical_words<K>(f, r, c);
+    } else {
+#pragma unroll
+        for (int i = 0; i < S::NW; i++) c[i] = f[i];
+    }
+    uint32_t pool;
+    asm("mov.u32 %0, 0x54474341;" : "=r"(pool));
+    uint32_t asc[S::NA];
+    expand_ascii<K>(c, asc, pool);
+    const u64x2 h = murmur3_h1<K, S::NA>(asc, a.seed);
+    hash = K <= 16 ? (uint64_t)h.lo : (((uint64_t)h.hi << 32) | h.lo);
+    return !(bad & 0x88888888u);
+}
+
+// Slow path of the filter-word kernels: one out-of-line call per vote group that has a survivor.  Bit j of `pm` = window
+// lp0 + j passed the fast-path filter; each lane rebuilds the exact hash of its own passing windows from the tile, and the
+// lanes whose window is valid and at or below the tile threshold do their own table work (in parallel, not serialised).
+template <int K, bool CANON>
+static __device__ __noinline__ void scan_survivors(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint32_t lp0, uint64_t tile_base,
+                                                   uint64_t tmax)
+{
+    while (pm) {
+        const uint32_t lp = lp0 + __ffs(pm) - 1;
+        pm &= pm - 1;
+        uint64_t hash;
+        if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), tile_base, lp);
+    }
+}
+
 #ifndef SCAN_VOTE_GROUP
-#define SCAN_VOTE_GROUP 4      // windows hashed back to back before one warp vote (1, 2, 4 or 8); see scan_group.
-                               // tools/scan_microbench.cu compares the settings (-DSCAN_VOTE_GROUP=n)
+#define SCAN_VOTE_GROUP 2      // windows hashed back to back before one warp vote (1, 2, 4 or 8); see scan_group_filter.
+                               // tools/scan_microbench.cu compares the settings (-DSCAN_VOTE_GROUP=n); on H100 2 beat 4 and 8
 #endif
 
+// ASCII words of the canonical k-mer of window J of the block (b = forward words, rb = reverse-complement words)
 template <int K, bool CANON, int J>
-__device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
-                                            const uint32_t (&rb)[KmerShape<K>::BW], uint64_t tmax, uint32_t pool, u64x2 &h_out)
+__device__ __forceinline__ void window_ascii(const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool,
+                                             uint32_t (&asc)[KmerShape<K>::NA])
 {
     using S = KmerShape<K>;
     uint32_t f[S::NW];
 #pragma unroll
     for (int i = 0; i < S::NW; i++) {
         f[i] = block_word<J, S::BW>(b, i);
-        if (i == S::NW - 1) f[i] &= S::LAST_MASK;
+        if (i == S::NW - 1) f[i] = (f[i] & S::LAST_MASK) | S::LAST_PAD;
     }
     uint32_t c[S::NW];
     if (CANON) {
@@ -325,32 +422,24 @@ __device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&
 #pragma unroll
         for (int i = 0; i < S::NW; i++) {
             r[i] = block_word<RO, S::BW>(rb, i);
-            if (i == S::NW - 1) r[i] &= S::LAST_MASK;
+            if (i == S::NW - 1) r[i] = (r[i] & S::LAST_MASK) | S::LAST_PAD;
         }
-        // rc < fwd as little-endian multi-word integers  <=>  memcmp(fwd, rc, k) > 0  (Sketch.cpp:569-571):
-        // borrow out of rc - fwd.  m = all-ones when the reverse complement is the canonical k-mer.
-        uint32_t m;
-        if (S::NW == 1) {
-            asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.u32 %0, 0, 0;\n\t}" : "=r"(m) : "r"(r[0]), "r"(f[0]));
-        } else if (S::NW == 2) {
-            asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.u32 %0, 0, 0;\n\t}"
-                : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]));
-        } else if (S::NW == 3) {
-            asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.u32 %0, 0, 0;\n\t}"
-                : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]));
-        } else {
-            asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.cc.u32 t, %7, %8;\n\tsubc.u32 %0, 0, 0;\n\t}"
-                : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]),
-                  "r"(r[S::NW > 3 ? 3 : 0]), "r"(f[S::NW > 3 ? 3 : 0]));
-        }
-#pragma unroll
-        for (int i = 0; i < S::NW; i++) c[i] = (f[i] & ~m) | (r[i] & m);
+        canonical_words<K>(f, r, c);
     } else {
 #pragma unroll
         for (int i = 0; i < S::NW; i++) c[i] = f[i];
     }
-    uint32_t asc[S::NA];
     expand_ascii<K>(c, asc, pool);
+}
+
+// Full-hash fast path (k <= 16, and the screen's probing kernels: every lane probes the reference table with its own hash)
+template <int K, bool CANON, int J>
+__device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
+                                            const uint32_t (&rb)[KmerShape<K>::BW], uint64_t tmax, uint32_t pool, u64x2 &h_out)
+{
+    using S = KmerShape<K>;
+    uint32_t asc[S::NA];
+    window_ascii<K, CANON, J>(b, rb, pool, asc);
     u64x2 h = murmur3_h1<K, S::NA>(asc, a.seed);
     if (K <= 16) h.hi = 0;        // 32-bit hashes: |{A,C,G,T}|^k <= 2^32 (reference Sketch.cpp:1136, hash.cpp:31-35)
     // coarse filter on one 32-bit word; validity and the exact threshold are checked in the slow path
@@ -358,8 +447,33 @@ __device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&
     return (K <= 16) ? (h.lo <= (uint32_t)tmax) : (h.hi <= (uint32_t)(tmax >> 32));
 }
 
-// G consecutive windows (J0 .. J0+G-1) are hashed without a control-flow break in between, which lets ptxas interleave
-// their independent multiply chains, then ONE warp vote decides whether anybody has a survivor.
+// Filter-word fast path (k > 16): only murmur3_h1_filter's word, to be tested against filter_threshold(tmax >> 32)
+template <int K, bool CANON, int J>
+__device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
+                                                       const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool)
+{
+    using S = KmerShape<K>;
+    uint32_t asc[S::NA];
+    window_ascii<K, CANON, J>(b, rb, pool, asc);
+    return murmur3_h1_filter<K, S::NA>(asc, a.seed);
+}
+
+// G consecutive windows J0 .. J0+G-1 hashed back to back (independent multiply chains that ptxas can interleave), ONE warp
+// vote, and one out-of-line slow-path call for the group.  The hot path only compares and votes; the per-lane bit mask of
+// passing windows is built inside the (rarely taken) branch.
+template <int K, bool CANON, int J0, int... J>
+__device__ __forceinline__ void scan_group_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
+                                                  uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t tf, uint32_t pool, uint32_t sm_addr,
+                                                  std::integer_sequence<int, J...>)
+{
+    const uint32_t x[] = {scan_window_filter<K, CANON, J0 + J>(a, b, rb, pool)...};
+    if (__any_sync(0xFFFFFFFFu, ((x[J] <= tf) || ...))) {
+        const uint32_t pm = (((x[J] <= tf ? 1u : 0u) << J) | ...);
+        scan_survivors<K, CANON>(a, pm, sm_addr, local0 + J0, tile_base, tmax);
+    }
+}
+
+// Full-hash variant of the group: G windows, one warp vote, then the survivors of each window serialised by scan_emit_warp.
 template <int K, bool CANON, int J0, int G>
 __device__ __forceinline__ void scan_group(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
                                            uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t pool, const uint32_t *sm_tile)
@@ -441,24 +555,28 @@ __device__ __forceinline__ uint4 expand32(uint64_t c, uint32_t m)
 // so the only synchronisation is __syncwarp().  The next tile's bytes are prefetched into registers before the
 // current tile is hashed (global latency hidden behind ~4000 instructions of work per lane).
 #ifndef SCAN_MIN_BLOCKS
-#define SCAN_MIN_BLOCKS 4      // resident CTAs per SM requested from ptxas (=> 64 registers);
-                               // tools/scan_microbench.cu compares the settings (-DSCAN_MIN_BLOCKS=n)
+#define SCAN_MIN_BLOCKS 3      // resident CTAs per SM requested from ptxas (=> 80 registers, no spills; 4 => 64 registers
+                               // and spills); tools/scan_microbench.cu compares the settings (-DSCAN_MIN_BLOCKS=n)
 #endif
-template <int K, bool CANON, bool PACKED>
+// FULL: the fast path computes the whole 64-bit hash (k <= 16, where the filter is on the low word, and SCAN_SCREEN, where
+// every lane probes the reference table with it); otherwise only murmur3_h1_filter's word and the slow path recomputes.
+template <int K, bool CANON, bool PACKED, bool FULL>
 __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) ? 3 : SCAN_MIN_BLOCKS) scan_kernel(const __grid_constant__ ScanArgs a)
 {
     using S = KmerShape<K>;
+    static_assert(FULL || K > 16, "the filter word is the high word of the hash");
     __shared__ __align__(16) uint32_t sm_all[SCAN_WARPS][SCAN_WARP_WORDS];
-#if SCAN_RC_SMEM
     // reverse-complement image of the tile (word i = nibble-reversed, complemented word NW-1-i), written once at staging so
     // that a block's reverse-complement words are 4 more LDS (the LSU is idle) instead of ~16 ALU instructions per block
     __shared__ __align__(16) uint32_t smr_all[CANON ? SCAN_WARPS : 1][SCAN_WARP_WORDS];
-#endif
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t *sm = sm_all[warp];
-#if SCAN_RC_SMEM
     uint32_t *smr = smr_all[CANON ? warp : 0];
-#endif
+    // the hot loop and the slow path address the tiles as 32-bit shared-memory addresses, passed through a shuffle (they are
+    // warp-uniform) so that ptxas keeps them in registers: it otherwise re-derives them (S2R SR_CgaCtaId, LEA, IMAD) on every
+    // iteration of the hot loop to save a register
+    const uint32_t sm_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(sm), 0);
+    const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(smr), 0);
     const uint32_t fold = a.preserve_case ? 0xFFFFFFFFu : 0xDFDFDFDFu;
     uint32_t pool;   // bytes 'A','C','G','T' for PRMT; opaque to the compiler so that it stays in one register
     asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
@@ -493,14 +611,12 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
             const uint4 e0 = expand32(pc0, pm0), e1 = expand32(pc1, pm1);
             *reinterpret_cast<uint4 *>(sm + 4 * lane) = e0;
             *reinterpret_cast<uint4 *>(sm + 4 * hg) = e1;
-#if SCAN_RC_SMEM
             if (CANON) {
                 *reinterpret_cast<uint4 *>(smr + (SCAN_WARP_WORDS - 4 - 4 * lane)) =
                     make_uint4(nibble_reverse(e0.w) ^ 0x33333333u, nibble_reverse(e0.z) ^ 0x33333333u, nibble_reverse(e0.y) ^ 0x33333333u, nibble_reverse(e0.x) ^ 0x33333333u);
                 *reinterpret_cast<uint4 *>(smr + (SCAN_WARP_WORDS - 4 - 4 * hg)) =
                     make_uint4(nibble_reverse(e1.w) ^ 0x33333333u, nibble_reverse(e1.z) ^ 0x33333333u, nibble_reverse(e1.y) ^ 0x33333333u, nibble_reverse(e1.x) ^ 0x33333333u);
             }
-#endif
         } else {
             const uint2 s0 = stage16(q0, base + 16ull * lane, a.stream_len, fold);
             const uint2 s1 = stage16(q1, base + 16ull * (lane + 32), a.stream_len, fold);
@@ -508,13 +624,11 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
             *reinterpret_cast<uint2 *>(sm + 2 * lane) = s0;
             *reinterpret_cast<uint2 *>(sm + 2 * (lane + 32)) = s1;
             *reinterpret_cast<uint2 *>(sm + 2 * v2) = s2;
-#if SCAN_RC_SMEM
             if (CANON) {
                 *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * lane)) = make_uint2(nibble_reverse(s0.y) ^ 0x33333333u, nibble_reverse(s0.x) ^ 0x33333333u);
                 *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * (lane + 32))) = make_uint2(nibble_reverse(s1.y) ^ 0x33333333u, nibble_reverse(s1.x) ^ 0x33333333u);
                 *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * v2)) = make_uint2(nibble_reverse(s2.y) ^ 0x33333333u, nibble_reverse(s2.x) ^ 0x33333333u);
             }
-#endif
         }
         __syncwarp();
         const uint64_t next = wt + wt_stride;
@@ -532,33 +646,45 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         }
         __syncwarp();
         const uint64_t tmax = a.tile_tmax ? a.tile_tmax[base / SCAN_TILE] : a.coarse_t;
+        const uint32_t tf = filter_threshold((uint32_t)(tmax >> 32));
 #pragma unroll 1
         for (int g = lane; g < SCAN_WARP_TILE / 8; g += 32) {
             uint32_t b[S::BW], rb[S::BW];
 #pragma unroll
-            for (int i = 0; i < S::BW; i++) b[i] = sm[g + i];
+            for (int i = 0; i < S::BW; i++) b[i] = lds_u32(sm_addr + 4u * (g + i));
             if (CANON) {
-#if SCAN_RC_SMEM
 #pragma unroll
-                for (int i = 0; i < S::BW; i++) rb[i] = smr[SCAN_WARP_WORDS - S::BW - g + i];
-#else
-#pragma unroll
-                for (int i = 0; i < S::BW; i++) rb[i] = nibble_reverse(b[S::BW - 1 - i]) ^ 0x33333333u;
-#endif
+                for (int i = 0; i < S::BW; i++) rb[i] = lds_u32(smr_addr + 4u * (SCAN_WARP_WORDS - S::BW - g + i));
             }
             const uint32_t local0 = 8u * g;
             constexpr int G = SCAN_VOTE_GROUP;
-            scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
-            if constexpr (G < 8) scan_group<K, CANON, (G < 8 ? G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-            if constexpr (G < 4) {
-                scan_group<K, CANON, (G < 4 ? 2 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, (G < 4 ? 3 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-            }
-            if constexpr (G < 2) {
-                scan_group<K, CANON, 4, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 5, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 6, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 7, 1>(a, b, rb, base, local0, tmax, pool, sm);
+            if constexpr (!FULL) {
+                const auto js = std::make_integer_sequence<int, G>();
+                scan_group_filter<K, CANON, 0>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                if constexpr (G < 8) scan_group_filter<K, CANON, (G < 8 ? G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                if constexpr (G < 4) {
+                    scan_group_filter<K, CANON, (G < 4 ? 2 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, (G < 4 ? 3 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                }
+                if constexpr (G < 2) {
+                    scan_group_filter<K, CANON, 4>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, 5>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, 6>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, 7>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                }
+            } else {
+                scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
+                if constexpr (G < 8) scan_group<K, CANON, (G < 8 ? G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
+                if constexpr (G < 4) {
+                    scan_group<K, CANON, (G < 4 ? 2 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
+                    scan_group<K, CANON, (G < 4 ? 3 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
+                }
+                if constexpr (G < 2) {
+                    scan_group<K, CANON, 4, 1>(a, b, rb, base, local0, tmax, pool, sm);
+                    scan_group<K, CANON, 5, 1>(a, b, rb, base, local0, tmax, pool, sm);
+                    scan_group<K, CANON, 6, 1>(a, b, rb, base, local0, tmax, pool, sm);
+                    scan_group<K, CANON, 7, 1>(a, b, rb, base, local0, tmax, pool, sm);
+                }
             }
         }
         __syncwarp();

@@ -1,4 +1,4 @@
-// scan_inst.cu -- explicit instantiations of scan_kernel<K, CANON> for K in [SCAN_K_LO, SCAN_K_HI].
+// scan_inst.cu -- explicit instantiations of scan_kernel<K, CANON, PACKED, FULL> for K in [SCAN_K_LO, SCAN_K_HI].
 // Compiled several times with different -DSCAN_K_LO/-DSCAN_K_HI/-DSCAN_PART so the parts build in parallel.
 #include "scan.cuh"
 
@@ -9,15 +9,15 @@
 namespace mashgpu {
 
 // grid <= 0: size the persistent grid to the resident CTAs (occupancy x SM count, queried once per kernel)
-template <int K, bool CANON, bool PACKED>
-static void launch_scan(const ScanArgs &a, int grid, cudaStream_t stream)
+template <int K, bool CANON, bool PACKED, bool FULL>
+static void launch_scan_kernel(const ScanArgs &a, int grid, cudaStream_t stream)
 {
     static int resident = 0;
     if (resident == 0) {
         int per_sm = 0, dev = 0, sms = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan_kernel<K, CANON, PACKED>, SCAN_THREADS, 0);
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, scan_kernel<K, CANON, PACKED, FULL>, SCAN_THREADS, 0);
         resident = (per_sm > 0 ? per_sm : 1) * (sms > 0 ? sms : 1);
     }
     const uint64_t warp_tiles = (a.tile_end - a.tile_begin) * (SCAN_TILE / SCAN_WARP_TILE);
@@ -25,7 +25,16 @@ static void launch_scan(const ScanArgs &a, int grid, cudaStream_t stream)
     int g = grid > 0 ? grid : resident;
     if ((uint64_t)g > need) g = (int)need;
     if (g < 1) g = 1;
-    scan_kernel<K, CANON, PACKED><<<g, SCAN_THREADS, 0, stream>>>(a);
+    scan_kernel<K, CANON, PACKED, FULL><<<g, SCAN_THREADS, 0, stream>>>(a);
+}
+
+// k > 16: the screen probes the reference table with every lane's full hash; every other mode only needs the filter word
+template <int K, bool CANON, bool PACKED>
+static void launch_scan(const ScanArgs &a, int grid, cudaStream_t stream)
+{
+    if constexpr (K <= 16) launch_scan_kernel<K, CANON, PACKED, true>(a, grid, stream);
+    else if (a.mode == SCAN_SCREEN) launch_scan_kernel<K, CANON, PACKED, true>(a, grid, stream);
+    else launch_scan_kernel<K, CANON, PACKED, false>(a, grid, stream);
 }
 
 template <int K>

@@ -58,10 +58,12 @@ constexpr uint32_t SEL_MAX_LOG2 = 14;     // select_kernel sorts up to 2^14 keys
 constexpr int SEL_THREADS = 256;
 
 // ---------------------------------------------------------------------------------------------------------
-// per-tile coarse threshold: max T over the units a tile touches
+// per-tile coarse threshold: max T over the units a tile touches; and (tile_unit != NULL) the tile's first unit, from which
+// the scan's slow path finds a survivor's unit with a short forward scan
 // ---------------------------------------------------------------------------------------------------------
 __global__ void tile_tmax_kernel(const uint64_t *unit_start, uint32_t n_units, const uint64_t *unit_t,
-                                 uint64_t stream_len, int k, uint64_t tile_begin, uint64_t tile_end, uint64_t *tile_tmax)
+                                 uint64_t stream_len, int k, uint64_t tile_begin, uint64_t tile_end, uint64_t *tile_tmax,
+                                 uint32_t *tile_unit)
 {
     uint64_t tile = tile_begin + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (tile >= tile_end) return;
@@ -73,6 +75,7 @@ __global__ void tile_tmax_kernel(const uint64_t *unit_start, uint32_t n_units, c
     uint64_t t = 0;
     for (uint32_t u = lo; u < n_units && unit_start[u] <= last; u++) t = max(t, unit_t[u]);
     tile_tmax[tile] = t;
+    if (tile_unit) tile_unit[tile] = lo;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -391,6 +394,7 @@ static int recount_hash(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const 
     c.tile_begin = lo / SCAN_TILE;
     c.tile_end = hi / SCAN_TILE + 1;
     c.tile_tmax = nullptr;
+    c.tile_unit = nullptr;      // the first pass's per-tile buffers are not kept
     c.coarse_t = target;
     c.count_target = target; c.count_lo = lo; c.count_hi = hi; c.count_out = d_count_slot;
     MG_CUDA(ctx, cudaMemsetAsync(d_count_slot, 0, 4, st));
@@ -435,6 +439,7 @@ static int rerun_unit(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const Sk
         a.tile_begin = S.unit_start[u] / SCAN_TILE;
         a.tile_end = (S.unit_start[u + 1] + SCAN_TILE - 1) / SCAN_TILE;
         a.tile_tmax = nullptr;
+        a.tile_unit = nullptr;
         a.coarse_t = t;
         a.only_unit = u;
         a.unit_t = meta.p - u;
@@ -539,7 +544,8 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
     d_start.p = ctx->sc_start.get<uint64_t>(n_units + 1); d_t.p = ctx->sc_t.get<uint64_t>(n_units); d_off.p = ctx->sc_off.get<uint64_t>(n_units);
     d_log2.p = ctx->sc_log2.get<uint32_t>(n_units); d_flags.p = ctx->sc_flags.get<uint32_t>(n_units); d_maxhash.p = ctx->sc_maxhash.get<uint32_t>(n_units);
     d_keys.p = ctx->sc_keys.get<uint64_t>(slots); d_cnt.p = ctx->sc_cnt.get<uint32_t>(slots); d_tmax.p = ctx->sc_tmax.get<uint64_t>(ntiles);
-    if (!d_start.p || !d_t.p || !d_off.p || !d_log2.p || !d_flags.p || !d_maxhash.p || !d_keys.p || !d_cnt.p || !d_tmax.p)
+    uint32_t *d_tunit = ctx->sc_tunit.get<uint32_t>(ntiles);
+    if (!d_start.p || !d_t.p || !d_off.p || !d_log2.p || !d_flags.p || !d_maxhash.p || !d_keys.p || !d_cnt.p || !d_tmax.p || !d_tunit)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu candidate slots for %u units)", (unsigned long long)slots, n_units);
     const bool want_counts = d_out_counts != nullptr;
     const uint32_t mc = probe ? 1u : std::max(1u, p->min_copies);      // the screen mixture is a plain MinHashHeap (CommandScreen.cpp:114-119)
@@ -591,10 +597,11 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
         a.ref_bitmap = probe->bitmap; a.ref_bitmap_shift = probe->bitmap_shift;
     }
     if (ntiles) {
-        tile_tmax_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, st>>>(d_start.p, n_units, d_t.p, stream_len, p->kmer_size, 0, ntiles, d_tmax.p);
+        tile_tmax_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, st>>>(d_start.p, n_units, d_t.p, stream_len, p->kmer_size, 0, ntiles, d_tmax.p, d_tunit);
         ctx->kernel_launches++;
     }
     a.tile_tmax = d_tmax.p;
+    a.tile_unit = d_tunit;
     if (probe) {
         // coarse filter must also let reference-hash candidates through
         a.tile_tmax = nullptr;
@@ -1489,7 +1496,7 @@ extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_param
     MG_CUDA(ctx, cudaMemcpyAsync(d_bstart.p, band_start.data(), (n_bands + 1) * 8ull, cudaMemcpyHostToDevice, st));
     MG_CUDA(ctx, cudaMemcpyAsync(d_bt.p, band_t.data(), n_bands * 8ull, cudaMemcpyHostToDevice, st));
     MG_CUDA(ctx, cudaMemsetAsync(ev_count.p, 0, 8, st));
-    tile_tmax_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, st>>>(d_bstart.p, n_bands, d_bt.p, total, params->kmer_size, 0, ntiles, d_tmax.p);
+    tile_tmax_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, st>>>(d_bstart.p, n_bands, d_bt.p, total, params->kmer_size, 0, ntiles, d_tmax.p, nullptr);
     ScanArgs a;
     memset(&a, 0, sizeof a);
     a.stream = d_stream.p; a.stream_len = total;

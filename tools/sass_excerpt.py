@@ -12,8 +12,9 @@ import subprocess
 import sys
 
 KERNELS = {
-    "scan_kernel_k21_canonical_ascii": "_ZN7mashgpu11scan_kernelILi21ELb1ELb0EEEvNS_8ScanArgsE",
-    "scan_kernel_k21_canonical_packed": "_ZN7mashgpu11scan_kernelILi21ELb1ELb1EEEvNS_8ScanArgsE",
+    "scan_kernel_k21_canonical_ascii": "_ZN7mashgpu11scan_kernelILi21ELb1ELb0ELb0EEEvNS_8ScanArgsE",
+    "scan_kernel_k21_canonical_packed": "_ZN7mashgpu11scan_kernelILi21ELb1ELb1ELb0EEEvNS_8ScanArgsE",
+    "scan_kernel_k21_canonical_ascii_screen": "_ZN7mashgpu11scan_kernelILi21ELb1ELb0ELb1EEEvNS_8ScanArgsE",
     "dist_kernel": "_ZN7mashgpu11dist_kernelILb0EEEvNS_8DistArgsE",
     "dist_kernel_bulk_copy_variant": "_ZN7mashgpu11dist_kernelILb1EEEvNS_8DistArgsE",
     "dist_probe_kernel": "_ZN7mashgpu17dist_probe_kernelILb0EEEvNS_8DistArgsE",
@@ -28,6 +29,28 @@ PIPES = {
     "TMA / bulk copy (UTMALDG/UBLKCP)": ("UTMALDG", "UBLKCP", "UTMASTG"),
     "tensor (HMMA/UTCMMA/...)": ("HMMA", "IMMA", "UTCHMMA", "UTCIMMA", "UTCQMMA"),
 }
+
+
+def opcode(t):
+    return re.sub(r"^@!?U?P\w+\s+", "", t).split()[0].split(".")[0]
+
+
+def hot_path_line(body):
+    """The scan kernel's hot path: its longest innermost loop minus the blocks that the branch after each warp vote
+    (VOTE.ANY) skips when no lane has a survivor -- i.e. what a warp issues per 8 windows when nobody passes the filter."""
+    skip = []
+    for i, (_, t) in enumerate(body):
+        if t.startswith("VOTE.ANY"):
+            for j in range(i + 1, min(i + 6, len(body))):
+                m = re.search(r"@!?P\d BRA.*?0x([0-9a-f]+)", body[j][1])
+                if m:
+                    skip.append((body[j][0] + 1, int(m.group(1), 16)))
+                    break
+    hot = [(a, t) for a, t in body if not any(x <= a < y for x, y in skip)]
+    c = collections.Counter(opcode(t) for _, t in hot)
+    alu = sum(n for o, n in c.items() if o in PIPES["ALU (SHF/LOP3/IADD3/PRMT/ISETP/SEL/...)"] + ("VIADD",))
+    return (f"hot path (longest innermost loop without the {len(skip)} survivor blocks behind the warp votes): {len(hot)} "
+            f"instructions per lane per 8 windows; ALU pipe {alu}, IMAD {c['IMAD']}, STL {c['STL']}, LDL {c['LDL']}, S2R {c['S2R']}")
 
 
 def main():
@@ -83,6 +106,9 @@ def main():
             if inner:
                 loops.append(body)
         loops.sort(key=len, reverse=True)
+        if name.startswith("scan_kernel") and loops:
+            summary.append("")
+            summary.append(hot_path_line(loops[0]))
         for body in loops[:8]:
             lo = collections.Counter(re.sub(r"^@!?U?P\d+\s+", "", t).split()[0].split(".")[0] for _, t in body)
             summary.append("")
