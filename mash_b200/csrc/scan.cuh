@@ -383,21 +383,75 @@ __device__ __forceinline__ bool window_hash(const ScanArgs &a, uint32_t sm_addr,
     return !(bad & 0x88888888u);
 }
 
+// Survivor queue of the filter-word kernels: per warp, up to SCAN_SQ exact survivors {hash, stream position} waiting for
+// their table work.  scan_emit's work is a chain of dependent global loads and atomics (unit lookup, threshold, table
+// insert) of a few thousand cycles; done where the survivor is found, the whole warp waits for it once per survivor (about
+// one vote group in 25 at the sketch's thresholds), which was 12.7 % of the k=21 kernel's time (DESIGN.md §2.4).  Queued,
+// it is done by scan_sq_flush between tiles, 32 survivors at a time, one per lane, so the warp waits once per 32.  Every
+// effect of scan_emit is an order-independent atomic or a write to the survivor's own position (SCAN_EVENTS' events are
+// sorted by position before they are replayed), so the results do not depend on when it runs.
+constexpr int SCAN_SQ = 64;          // queue capacity per warp; a survivor that finds it full does its table work at once
+constexpr int SCAN_SQ_FLUSH = 32;    // scan_kernel flushes the queue after a tile that leaves at least this many entries
+__shared__ uint64_t scan_sq_hash[SCAN_WARPS][SCAN_SQ];
+__shared__ uint64_t scan_sq_pos[SCAN_WARPS][SCAN_SQ];
+__shared__ uint32_t scan_sq_n[SCAN_WARPS];   // entries appended since the last flush (may exceed SCAN_SQ: those went direct)
+
 // Slow path of the filter-word kernels: one out-of-line call per vote group that has a survivor.  Bit j of `pm` = window
 // lp0 + j passed the fast-path filter; each lane rebuilds the exact hash of its own passing windows from the tile, and the
-// lanes whose window is valid and at or below the tile threshold do their own table work (in parallel, not serialised).
+// lanes whose window is valid and at or below the tile threshold queue it for its table work.
 template <int K, bool CANON>
 static __device__ __noinline__ void scan_survivors(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint32_t lp0, uint64_t tile_base,
                                                    uint64_t tmax)
 {
+    const uint32_t warp = threadIdx.x >> 5;
     while (pm) {
         const uint32_t lp = lp0 + __ffs(pm) - 1;
         pm &= pm - 1;
         uint64_t hash;
-        if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), tile_base, lp);
+        if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) {
+            const uint32_t at = atomicAdd(&scan_sq_n[warp], 1u);
+            if (at < SCAN_SQ) {
+                scan_sq_hash[warp][at] = hash;
+                scan_sq_pos[warp][at] = tile_base + lp;
+            } else {
+                scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), tile_base, lp);
+            }
+        }
     }
 }
 
+// Table work of the queued survivors of this warp, one per lane; warp-uniform call, leaves the queue empty
+static __device__ __noinline__ void scan_sq_flush(const ScanArgs &a)
+{
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    __syncwarp();
+    const uint32_t n = min(scan_sq_n[warp], (uint32_t)SCAN_SQ);
+    for (uint32_t i = lane; i < n; i += 32) {
+        const uint64_t hash = scan_sq_hash[warp][i];
+        scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), scan_sq_pos[warp][i], 0);
+    }
+    __syncwarp();
+    if (lane == 0) scan_sq_n[warp] = 0;
+    __syncwarp();
+}
+
+// Cost-accounting switches for tools/scan_microbench.cu (0 in the library; see DESIGN.md §2.4).  Each takes one part of
+// the kernel out or measures it; the kernel's results are not what the library needs when one of them is set.
+//   SCAN_MB_NO_SURVIVORS: no warp vote and no survivor call; the filter words are xor-ed into a per-lane accumulator
+//                         that is stored once at the end (a.out_hash[global thread]), so the hash stays live.
+//   SCAN_MB_STAGE_ONCE:   each warp stages its first tile only and hashes it again in place of every later tile: no
+//                         staging and no global prefetch after the first.
+//   SCAN_MB_CLOCK:        clock64() around each tile's hot loop; lane 0 stores the warp's total cycles at
+//                         a.out_hash[gridDim.x * SCAN_THREADS + global warp].
+#ifndef SCAN_MB_NO_SURVIVORS
+#define SCAN_MB_NO_SURVIVORS 0
+#endif
+#ifndef SCAN_MB_STAGE_ONCE
+#define SCAN_MB_STAGE_ONCE 0
+#endif
+#ifndef SCAN_MB_CLOCK
+#define SCAN_MB_CLOCK 0
+#endif
 #ifndef SCAN_VOTE_GROUP
 #define SCAN_VOTE_GROUP 2      // windows hashed back to back before one warp vote (1, 2, 4 or 8); see scan_group_filter.
                                // tools/scan_microbench.cu compares the settings (-DSCAN_VOTE_GROUP=n); on H100 2 beat 4 and 8
@@ -464,10 +518,11 @@ __device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const 
 template <int K, bool CANON, int J0, int... J>
 __device__ __forceinline__ void scan_group_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
                                                   uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t tf, uint32_t pool, uint32_t sm_addr,
-                                                  std::integer_sequence<int, J...>)
+                                                  uint32_t &mb_acc, std::integer_sequence<int, J...>)
 {
     const uint32_t x[] = {scan_window_filter<K, CANON, J0 + J>(a, b, rb, pool)...};
-    if (__any_sync(0xFFFFFFFFu, ((x[J] <= tf) || ...))) {
+    mb_acc ^= (x[J] ^ ...);
+    if (!SCAN_MB_NO_SURVIVORS && __any_sync(0xFFFFFFFFu, ((x[J] <= tf) || ...))) {
         const uint32_t pm = (((x[J] <= tf ? 1u : 0u) << J) | ...);
         scan_survivors<K, CANON>(a, pm, sm_addr, local0 + J0, tile_base, tmax);
     }
@@ -605,9 +660,18 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         q1 = load16(a.stream, base + 16ull * (lane + 32), a.stream_len);
         q2 = load16(a.stream, base + 16ull * v2, a.stream_len);
     }
+    if (!FULL) {
+        if (lane == 0) scan_sq_n[warp] = 0;
+        __syncwarp();
+    }
+    uint32_t mb_acc = 0;
+    long long mb_cycles = 0;
+    const uint64_t wt_first = wt;
     for (; wt < wt_end; wt += wt_stride) {
         const uint64_t base = wt * (uint64_t)SCAN_WARP_TILE;
-        if (PACKED) {
+        if (SCAN_MB_STAGE_ONCE && wt != wt_first) {
+            // microbenchmark only: hash the first tile again
+        } else if (PACKED) {
             const uint4 e0 = expand32(pc0, pm0), e1 = expand32(pc1, pm1);
             *reinterpret_cast<uint4 *>(sm + 4 * lane) = e0;
             *reinterpret_cast<uint4 *>(sm + 4 * hg) = e1;
@@ -632,7 +696,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         }
         __syncwarp();
         const uint64_t next = wt + wt_stride;
-        if (next < wt_end) {   // prefetch
+        if (!SCAN_MB_STAGE_ONCE && next < wt_end) {   // prefetch
             if (PACKED) {
                 const uint64_t g0 = next * (uint64_t)(SCAN_WARP_TILE / 32);
                 pc0 = __ldg(a.codes + g0 + lane); pm0 = __ldg(a.inval + g0 + lane);
@@ -647,6 +711,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         __syncwarp();
         const uint64_t tmax = a.tile_tmax ? a.tile_tmax[base / SCAN_TILE] : a.coarse_t;
         const uint32_t tf = filter_threshold((uint32_t)(tmax >> 32));
+        const long long c0 = SCAN_MB_CLOCK ? clock64() : 0;
 #pragma unroll 1
         for (int g = lane; g < SCAN_WARP_TILE / 8; g += 32) {
             uint32_t b[S::BW], rb[S::BW];
@@ -660,17 +725,17 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
             constexpr int G = SCAN_VOTE_GROUP;
             if constexpr (!FULL) {
                 const auto js = std::make_integer_sequence<int, G>();
-                scan_group_filter<K, CANON, 0>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
-                if constexpr (G < 8) scan_group_filter<K, CANON, (G < 8 ? G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                scan_group_filter<K, CANON, 0>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
+                if constexpr (G < 8) scan_group_filter<K, CANON, (G < 8 ? G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
                 if constexpr (G < 4) {
-                    scan_group_filter<K, CANON, (G < 4 ? 2 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
-                    scan_group_filter<K, CANON, (G < 4 ? 3 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, (G < 4 ? 2 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
+                    scan_group_filter<K, CANON, (G < 4 ? 3 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
                 }
                 if constexpr (G < 2) {
-                    scan_group_filter<K, CANON, 4>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
-                    scan_group_filter<K, CANON, 5>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
-                    scan_group_filter<K, CANON, 6>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
-                    scan_group_filter<K, CANON, 7>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, js);
+                    scan_group_filter<K, CANON, 4>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
+                    scan_group_filter<K, CANON, 5>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
+                    scan_group_filter<K, CANON, 6>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
+                    scan_group_filter<K, CANON, 7>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
                 }
             } else {
                 scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
@@ -687,8 +752,13 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
                 }
             }
         }
+        if (SCAN_MB_CLOCK) mb_cycles += clock64() - c0;
         __syncwarp();
+        if (!FULL && scan_sq_n[warp] >= SCAN_SQ_FLUSH) scan_sq_flush(a);
     }
+    if (!FULL && scan_sq_n[warp] > 0) scan_sq_flush(a);
+    if (SCAN_MB_NO_SURVIVORS) a.out_hash[(uint64_t)blockIdx.x * SCAN_THREADS + threadIdx.x] = mb_acc;
+    if (SCAN_MB_CLOCK && lane == 0) a.out_hash[(uint64_t)gridDim.x * SCAN_THREADS + (uint64_t)blockIdx.x * SCAN_WARPS + warp] = (uint64_t)mb_cycles;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -7,6 +7,12 @@
 // order-independent checksum of the candidate tables (key, count and unit of every occupied slot, plus the overflow and
 // 2^64-1 counters), so two variants can be shown to produce the same candidates.
 //
+// Cost accounting (DESIGN.md §2.4): scan.cuh's SCAN_MB_* switches build variants without the survivor path
+// (-DSCAN_MB_NO_SURVIVORS=1), with each warp's tile staged once and hashed again (-DSCAN_MB_STAGE_ONCE=1), or with clock64()
+// around each tile's hot loop (-DSCAN_MB_CLOCK=1: reports the loop's cycles per warp per 256 windows, i.e. per 8 windows per
+// lane; the hot-path instruction count of tools/sass_excerpt.py over it is a warp's issue rate inside the loop).  Their
+// checksums differ from the kernel's by design.
+//
 // Build one binary per variant and run them alternately, e.g.
 //   nvcc -std=c++17 -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -DSCAN_MIN_BLOCKS=3 -I mash_b200/csrc \
 //        tools/scan_microbench.cu -o tools/mb_mb3
@@ -98,6 +104,10 @@ int main(int argc, char **argv)
     cudaFuncAttributes fa; CK(cudaFuncGetAttributes(&fa, kern));
     const uint64_t need = (ntiles * (SCAN_TILE / SCAN_WARP_TILE) + SCAN_WARPS - 1) / SCAN_WARPS;   // as scan_inst.cu's launcher
     const int grid = (int)std::min<uint64_t>((uint64_t)per_sm * sms, need);
+    // sink of the SCAN_MB_* variants: one word per thread, then one per warp
+    const uint64_t sink_n = (uint64_t)grid * SCAN_THREADS + (uint64_t)grid * SCAN_WARPS;
+    uint64_t *sink; CK(cudaMalloc(&sink, sink_n * 8)); CK(cudaMemset(sink, 0, sink_n * 8));
+    a.out_hash = sink;
     auto reset = [&] {
         CK(cudaMemset(keys, 0xFF, slots * 8)); CK(cudaMemset(cnt, 0, slots * 4));
         CK(cudaMemset(flags, 0, n_units * 4ull)); CK(cudaMemset(maxh, 0, n_units * 4ull));
@@ -119,17 +129,25 @@ int main(int argc, char **argv)
     CK(cudaMemcpy(hf.data(), flags, n_units * 4ull, cudaMemcpyDeviceToHost)); CK(cudaMemcpy(hm.data(), maxh, n_units * 4ull, cudaMemcpyDeviceToHost));
     uint64_t nflag = 0, nmax = 0;
     for (uint32_t u = 0; u < n_units; u++) { nflag += hf[u] != 0; nmax += hm[u]; }
+    // SCAN_MB_CLOCK: the warps' in-loop cycles (of the last repetition) per 256 windows
+    std::vector<uint64_t> wcyc((size_t)grid * SCAN_WARPS);
+    CK(cudaMemcpy(wcyc.data(), sink + (uint64_t)grid * SCAN_THREADS, wcyc.size() * 8, cudaMemcpyDeviceToHost));
+    double cyc = 0;
+    for (uint64_t c : wcyc) cyc += (double)c;
+    const double loop_cycles_256 = cyc / ((double)ntiles * (SCAN_TILE / SCAN_WARP_TILE) * (SCAN_WARP_TILE / 256));
     std::vector<float> sorted = ms; std::sort(sorted.begin(), sorted.end());
     const float med = sorted[reps / 2];
     printf("{\"variant\": \"%s\", \"min_blocks\": %d, \"vote_group\": %d, \"regs\": %d, \"local_bytes\": %zu, \"occupancy\": %d, "
            "\"units\": %u, \"bases\": %llu, \"ms_median\": %.3f, \"ms_min\": %.3f, \"ms_max\": %.3f, \"gbps_median\": %.1f, "
-           "\"checksum\": \"%016llx\", \"candidates\": %llu, \"overflowed_units\": %llu, \"maxhash\": %llu}\n",
+           "\"checksum\": \"%016llx\", \"candidates\": %llu, \"overflowed_units\": %llu, \"maxhash\": %llu, \"warps_per_scheduler\": %d, "
+           "\"loop_cycles_per_256_windows_per_warp\": %.1f, \"gbps_min\": %.1f, \"gbps_max\": %.1f}\n",
 #ifdef VARIANT
            VARIANT,
 #else
            "default",
 #endif
            SCAN_MIN_BLOCKS, SCAN_VOTE_GROUP, fa.numRegs, (size_t)fa.localSizeBytes, per_sm, n_units, (unsigned long long)n, med,
-           sorted[0], sorted[reps - 1], n / med / 1e6, h_sum[0], h_sum[1], (unsigned long long)nflag, (unsigned long long)nmax);
+           sorted[0], sorted[reps - 1], n / med / 1e6, h_sum[0], h_sum[1], (unsigned long long)nflag, (unsigned long long)nmax,
+           per_sm * SCAN_WARPS / 4, SCAN_MB_CLOCK ? loop_cycles_256 : 0.0, n / sorted[reps - 1] / 1e6, n / sorted[0] / 1e6);
     return 0;
 }
