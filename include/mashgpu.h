@@ -263,7 +263,15 @@ int mashgpu_dist(mashgpu_ctx *ctx, const mashgpu_sketch_set *ref, const mashgpu_
  * ------------------------------------------------------------------------------------------------------- */
 typedef struct mashgpu_screen_job mashgpu_screen_job;
 
-/* Builds the distinct-hash table of the reference sketches with zeroed counters (CommandScreen.cpp:93-114). */
+/* Builds the distinct-hash table of the reference sketches with zeroed counters (CommandScreen.cpp:93-114).
+ * The alphabet picks the mode, as in the reference (CommandScreen.cpp:120):
+ *   {A,C,G,T}                        nucleotide k-mers of the reads (canonical unless noncanonical);
+ *   exactly ACDEFGHIKLMNPQRSTVWY     translated screen: every chunk is translated in all six frames (standard genetic code;
+ *                                    a stop codon or a codon with a byte outside {A,C,G,T} ends the peptide; 'U' counts as
+ *                                    'A' on the reverse strand only, as the reference's complement table has it) and its
+ *                                    non-canonical amino-acid k-mers are screened; kmer space 20^k;
+ *   any other alphabet (-z)          byte k-mers of the reads as they stand.
+ * Non-nucleotide jobs always upload ASCII (MASHGPU_SCREEN_HOST_PACK is ignored). */
 int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, const mashgpu_sketch_set *refs,
                         mashgpu_screen_job **job);
 /* One HashInput (CommandScreen.h:104-133): a '*'-joined chunk of reads (CommandScreen.cpp:224-262; any byte
@@ -311,6 +319,8 @@ typedef struct mashgpu_stats {
     double dist_kernel_ms;         /* accumulated device time of the merge kernel */
     uint64_t dist_kernel_launches;
     uint64_t exact_reruns;         /* units that needed the exact re-run path */
+    double translate_kernel_ms;    /* accumulated device time of the six-frame translation kernel (translated screen) */
+    uint64_t translate_kernel_launches;
 } mashgpu_stats;
 /* timing != 0 brackets the dominant kernels with CUDA events (adds a sync at mashgpu_get_stats). */
 int mashgpu_set_timing(mashgpu_ctx *ctx, int timing);

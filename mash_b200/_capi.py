@@ -51,7 +51,8 @@ class SketchSet(C.Structure):
 
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("scan_kernel_ms", C.c_double), ("scan_kernel_launches", C.c_uint64),
-                ("dist_kernel_ms", C.c_double), ("dist_kernel_launches", C.c_uint64), ("exact_reruns", C.c_uint64)]
+                ("dist_kernel_ms", C.c_double), ("dist_kernel_launches", C.c_uint64), ("exact_reruns", C.c_uint64),
+                ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64)]
 
 
 def lib_path():

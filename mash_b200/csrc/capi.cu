@@ -100,15 +100,18 @@ extern "C" int mashgpu_get_stats(mashgpu_ctx *ctx, mashgpu_stats *out, int reset
     cudaSetDevice(ctx->device);
     drain(ctx->scan_events, ctx->scan_ms);
     drain(ctx->dist_events, ctx->dist_ms);
+    drain(ctx->translate_events, ctx->translate_ms);
     out->kernel_launches = ctx->kernel_launches;
     out->scan_kernel_ms = ctx->scan_ms;
     out->scan_kernel_launches = ctx->scan_launches;
     out->dist_kernel_ms = ctx->dist_ms;
     out->dist_kernel_launches = ctx->dist_launches;
     out->exact_reruns = ctx->exact_reruns;
+    out->translate_kernel_ms = ctx->translate_ms;
+    out->translate_kernel_launches = ctx->translate_launches;
     if (reset) {
-        ctx->kernel_launches = ctx->scan_launches = ctx->dist_launches = ctx->exact_reruns = 0;
-        ctx->scan_ms = ctx->dist_ms = 0;
+        ctx->kernel_launches = ctx->scan_launches = ctx->dist_launches = ctx->exact_reruns = ctx->translate_launches = 0;
+        ctx->scan_ms = ctx->dist_ms = ctx->translate_ms = 0;
     }
     return MASHGPU_OK;
 }

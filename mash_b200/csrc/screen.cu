@@ -7,6 +7,12 @@
 // SCAN_SCREEN mode: k-mer hashes <= the largest reference hash probe the table and bump the counter on a hit,
 // and the chunk's bottom-s candidates are merged into the running bottom-s of the whole mixture (the
 // reference merges per-thread MinHashHeaps the same way, :288-302; bottom-s of a union is order independent).
+//
+// Protein sketches switch the job to the translated screen (:120, 516-530): every fed chunk is first translated in six
+// frames by translate.cu into a peptide stream (stops and invalid codons as 0 bytes) and the byte scan kernel runs over
+// that stream.  The result does not depend on how the reads are cut into chunks (DESIGN.md 4.1), so chunk joining, the
+// two-buffer pipeline and the exact re-run work unchanged.  Other non-nucleotide alphabets (-z) are screened as byte
+// k-mers, untranslated (:541).
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -237,7 +243,27 @@ struct mashgpu_screen_job {
     bool winner = false;     // -w
     std::vector<uint64_t> h_len;      // Reference::length per sketch (tie break of -w), zeros when the caller gave none
     std::vector<uint32_t> h_n;        // hashes per sketch
+    // translated screen (protein sketches): each chunk is translated in six frames into pep[slot] and the peptide stream is
+    // scanned; a slot's buffer stays untouched until its chunk is collected (the exact re-run reads it again)
+    bool translate = false;
+    DevBuf<uint8_t> pep[2];
 };
+
+namespace {
+
+// The reference switches `mash screen` to translated mode exactly when the sketch alphabet is alphabetProtein
+// (CommandScreen.cpp:120); setAlphabetFromString sorts the letters, so this is equality of the letter sets.
+bool is_protein_alphabet(const mashgpu_sketch_params *p)
+{
+    static const char prot[] = "ACDEFGHIKLMNPQRSTVWY";
+    uint8_t want[256] = {0};
+    for (const char *c = prot; *c; c++) want[(unsigned char)*c] = 1;
+    for (int i = 0; i < 256; i++)
+        if ((p->alphabet[i] != 0) != (want[i] != 0)) return false;
+    return true;
+}
+
+}  // namespace
 
 extern "C" int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, const mashgpu_sketch_set *refs,
                                    mashgpu_screen_job **job_out)
@@ -247,13 +273,14 @@ extern "C" int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params
     if (!refs || !job_out) return fail(ctx, MASHGPU_ERR_INVALID, "NULL argument");
     if (refs->n && (!refs->hashes || !refs->n_hashes)) return fail(ctx, MASHGPU_ERR_INVALID, "reference set has NULL arrays");
     if (params->sketch_size > (1u << 13)) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "screen supports sketch_size <= 8192");
-    if (!is_dna_alphabet(params))
-        return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "screen is only provided for nucleotide sketches (the reference 6-frame-translates "
-                                                  "the mixture for amino-acid sketches, CommandScreen.cpp:516-530: out of scope)");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     mashgpu_screen_job *job = new mashgpu_screen_job();
     job->ctx = ctx; job->params = *params; job->n_ref = refs->n; job->stride = refs->stride;
+    // protein sketch: translated screen; any other non-nucleotide alphabet (-z): byte k-mers, untranslated (CommandScreen.cpp:541).
+    // Both take ASCII copies: the 2-bit packer only carries {A,C,G,T} and cannot tell 'U' (a base on the reverse strand) from 'N'
+    job->translate = is_protein_alphabet(params);
+    if (!is_dna_alphabet(params)) job->host_pack = 0;
     auto bail = [&](int rc) { delete job; return rc; };
     const uint64_t total = refs->n * refs->stride;
     if (refs->on_device) { job->ref_hashes = refs->hashes; job->ref_n = refs->n_hashes; }
@@ -347,12 +374,22 @@ constexpr uint64_t SCREEN_SMALL_CHUNK = 4ull << 20;     // host chunks below thi
 constexpr uint64_t SCREEN_FLUSH_BYTES = 32ull << 20;    // ... until this much has accumulated (the reference feeds 1 MiB HashInputs)
 
 // kernels of one chunk: scan (+ table probe) -> chunk bottom-s -> merge into the running mixture -> {n, top} read-back.  No sync.
-int screen_enqueue(mashgpu_screen_job *job, const void *d_chunk, uint64_t len, const uint64_t *d_codes = nullptr, const uint32_t *d_inval = nullptr,
+// Translated jobs first turn the chunk into its six-frame peptide stream in pep[slot] and scan that instead.
+int screen_enqueue(mashgpu_screen_job *job, int slot, const void *d_chunk, uint64_t len, const uint64_t *d_codes = nullptr, const uint32_t *d_inval = nullptr,
                    cudaEvent_t data_ready = nullptr)
 {
     mashgpu_ctx *ctx = job->ctx;
     cudaStream_t st = ctx->stream;
     const uint32_t s = job->params.sketch_size;
+    if (job->translate) {
+        const uint64_t pep_len = translated_length(len);
+        if (job->pep[slot].reserve(pep_len + 16) != cudaSuccess)
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (peptide stream of %llu B)", (unsigned long long)pep_len);
+        if (data_ready) { MG_CUDA(ctx, cudaStreamWaitEvent(st, data_ready, 0)); data_ready = nullptr; }
+        MG_TRY(translate_enqueue(ctx, d_chunk, len, job->params.preserve_case, job->pep[slot].p, st));
+        d_chunk = job->pep[slot].p;
+        len = pep_len;
+    }
     uint64_t unit_start[2] = {0, len};
     SketchStream S;
     S.d_stream = d_chunk; S.d_codes = d_codes; S.d_inval = d_inval; S.unit_start = unit_start; S.n_units = 1; S.data_ready = data_ready;
@@ -453,7 +490,7 @@ int screen_feed_host_packed(mashgpu_screen_job *job, const void *chunk, uint64_t
     MG_CUDA(ctx, cudaEventRecord(job->copied[b], ctx->copy_stream));
     MG_TRY(screen_collect(job));                                    // the chunk before this one: its kernels overlapped the packing
     const double t3 = now();
-    const int rc = screen_enqueue(job, nullptr, len, d_codes, d_inval, job->copied[b]);      // the scan kernel waits for the upload, this thread does not
+    const int rc = screen_enqueue(job, b, nullptr, len, d_codes, d_inval, job->copied[b]);      // the scan kernel waits for the upload, this thread does not
     if (trace) fprintf(stderr, "[mashgpu] screen packed feed %llu B: wait %.2f, alloc + pack %.2f (%d threads), collect previous %.2f, enqueue %.2f ms\n",
                        (unsigned long long)len, t1 - t0, t2 - t1, job->pack_threads, t3 - t2, now() - t3);
     return rc;
@@ -490,7 +527,7 @@ int screen_feed_host(mashgpu_screen_job *job, const void *chunk, uint64_t len)
     MG_CUDA(ctx, cudaEventRecord(job->copied[b], ctx->copy_stream));
     MG_TRY(screen_collect(job));                                    // the chunk before this one: its kernels overlapped the copy above
     MG_CUDA(ctx, cudaEventSynchronize(job->copied[b]));
-    return screen_enqueue(job, stage, len);
+    return screen_enqueue(job, b, stage, len);
 }
 
 int screen_flush_acc(mashgpu_screen_job *job)
@@ -511,7 +548,7 @@ extern "C" int mashgpu_screen_feed_dev(mashgpu_screen_job *job, const void *d_ch
     if (!d_chunk) return fail(ctx, MASHGPU_ERR_INVALID, "chunk is NULL");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     MG_TRY(screen_collect(job));
-    MG_TRY(screen_enqueue(job, d_chunk, len));
+    MG_TRY(screen_enqueue(job, 0, d_chunk, len));
     return screen_collect(job);          // the caller's device buffer is free again when this returns
 }
 

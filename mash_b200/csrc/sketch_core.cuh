@@ -54,4 +54,9 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
                           const ScreenProbe *probe, SketchTicket &t);
 int sketch_stream_finalize(mashgpu_ctx *ctx, SketchTicket &t);
 
+// translate.cu: six-frame translation of a nucleotide chunk (translated screen).  d_pep receives translated_length(len) bytes
+// and must be allocated to that length rounded up to 16 (the scan kernel reads whole 16-byte vectors).
+uint64_t translated_length(uint64_t len);
+int translate_enqueue(mashgpu_ctx *ctx, const void *d_chunk, uint64_t len, int preserve_case, uint8_t *d_pep, cudaStream_t st);
+
 }  // namespace mashgpu

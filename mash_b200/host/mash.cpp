@@ -3,7 +3,7 @@
 // CommandTriangle.cpp:45-214, CommandScreen.cpp:54-461, CommandInfo.cpp:222-299): same option identifiers and
 // defaults (Command.cpp:165-200), same stdout formats (iostream default precision), same ordering contracts.
 // It exists so that the reference's `make test` flow can be replayed against the GPU engine; help text, `paste`,
-// `bounds`, `taxscreen`, `within`, `find`, winner-take-all and translated screening are out of scope.
+// `bounds`, `taxscreen`, `within` and `find` are out of scope.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -490,7 +490,7 @@ int runScreen(int argc, const char **argv)
     parameters = sketch.getParameters();
     string alphabet;
     sketch.getAlphabetAsString(alphabet);
-    if (alphabet == alphabetProtein) { cerr << "ERROR: translated (amino acid) screening is not available in the GPU engine." << endl; return 1; }
+    const bool trans = alphabet == alphabetProtein;          // CommandScreen.cpp:120: the library translates the mixture in six frames
     cerr << "Loading " << c.arguments[0] << "..." << endl;
     mashgpu_sketch_params p;
     fillGpuParams(p, parameters);
@@ -501,7 +501,7 @@ int runScreen(int argc, const char **argv)
     if (mashgpu_screen_open(gpuContext(), &p, &set, &job) != MASHGPU_OK) gpuFail();
     if (c.opt("winning!").active && mashgpu_screen_set_winner(job, 1) != MASHGPU_OK) gpuFail();     // -w, CommandScreen.cpp:357-407
     int queryCount = (int)c.arguments.size() - 1;
-    cerr << "Streaming from ";
+    cerr << (trans ? "Translating from " : "Streaming from ");
     if (queryCount == 1) cerr << c.arguments[1]; else cerr << queryCount << " inputs";
     cerr << "..." << endl;
     // round robin over the mixture files, '*'-joined chunks (reference CommandScreen.cpp:156-270; chunks of 64 MiB
@@ -555,7 +555,7 @@ int runScreen(int argc, const char **argv)
     uint64_t setSize = 0;
     if (mashgpu_screen_finish(job, shared.data(), median.data(), identity.data(), pValue.data(), &setSize, 0, 0) != MASHGPU_OK) gpuFail();
     mashgpu_screen_close(job);
-    cerr << "   Estimated distinct k-mers in mixture: " << setSize << endl;
+    cerr << "   Estimated distinct" << (trans ? " (translated)" : "") << " k-mers in mixture: " << setSize << endl;
     if (setSize == 0) cerr << "WARNING: no valid k-mers in input." << endl;
     cerr << "Summing shared..." << endl << "Computing coverage medians..." << endl << "Writing output..." << endl;
     for (uint64_t i = 0; i < n; i++) {                       // reference CommandScreen.cpp:418-455
