@@ -310,6 +310,48 @@ int mashgpu_screen_merge_mixtures_dev(mashgpu_screen_job *job, const uint64_t *d
 int mashgpu_screen_close(mashgpu_screen_job *job);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * `mash taxscreen`: lowest-common-ancestor taxon of every distinct reference hash of a screen job, counted per taxon and
+ * rolled up the tree (CommandTaxScreen.cpp:415-471, TaxDB::getLowestCommonAncestor taxdb.hpp:158-190).
+ * ------------------------------------------------------------------------------------------------------- */
+typedef struct mashgpu_taxonomy mashgpu_taxonomy;
+
+/* A taxonomy of n_nodes dense nodes: parent[i] is the index of node i's parent, parent[i] == i marks a root, taxid[i] is its
+ * taxID (distinct).  Nodes with taxID 0 or 1 end the LCA walks as roots do (the reference's walks stop there); the roll-up
+ * still goes through them to their parent.  A parent cycle is refused (MASHGPU_ERR_INVALID).  The tree stays in device
+ * memory until mashgpu_taxonomy_close. */
+int mashgpu_taxonomy_open(mashgpu_ctx *ctx, uint64_t n_nodes, const uint32_t *parent, const uint64_t *taxid, mashgpu_taxonomy **tax);
+int mashgpu_taxonomy_close(mashgpu_taxonomy *tax);
+
+#define MASHGPU_TAX_NONE 0xFFFFFFFFu   /* ref_code of a sketch without a taxID (taxID 0) */
+
+/* One key of the reference's `counts` map (TaxCounts, taxdb.hpp:40-46). */
+typedef struct mashgpu_tax_row {
+    uint64_t taxid;
+    uint64_t tax_count;          /* hashes assigned to this taxon and seen in the reads at least once */
+    uint64_t tax_hash_count;     /* hashes assigned to this taxon */
+    uint64_t clade_count;        /* tax_count summed over the clade; 0 for taxIDs outside the taxonomy */
+    uint64_t clade_hash_count;   /* tax_hash_count summed over the clade; 0 for taxIDs outside the taxonomy */
+} mashgpu_tax_row;
+
+/* After the last chunk was fed (and, across GPUs, after the counters were all-reduced): ref_code[r] for each of the job's
+ * reference sketches is a node index, n_nodes + u for the unknown taxID unknown_taxid[u] (distinct, none of them 0 or in
+ * the taxonomy), or MASHGPU_TAX_NONE.  Each distinct hash h gets the reference's fold of getLowestCommonAncestor over the
+ * sketches holding it:
+ *   no sketch with a taxID -> 0; one -> its taxID, known or not; two or more -> 1 if any is unknown, if the known taxa share no
+ *   ancestor or if their LCA is a root (or has taxID 0 or 1); otherwise the LCA.
+ * Rows: one per taxon with a nonzero clade hash count, plus taxIDs outside the taxonomy (0 and unknown ones included) that got
+ * hashes; ascending node index, then unknown slots, then 0 and 1.  *n_rows is their number; they are copied only when it is at
+ * most `capacity` (n_nodes + n_unknown + 2 is always enough).  total_count / total_hash_count (nullable): sums of tax_count
+ * and tax_hash_count over the rows.  hash_taxid (nullable, one entry per distinct hash in ascending hash order): the taxID
+ * assigned to it.  unknown_in_lca (nullable, n_unknown bytes): 1 when unknown taxID u took part in a fold of two or more
+ * sketches (the reference prints "TaxID u not in database" then).  Host buffers. */
+int mashgpu_screen_taxonomy(mashgpu_screen_job *job, const mashgpu_taxonomy *tax, const uint32_t *ref_code,
+                            uint32_t n_unknown, const uint64_t *unknown_taxid,
+                            mashgpu_tax_row *rows, uint64_t capacity, uint64_t *n_rows,
+                            uint64_t *total_count, uint64_t *total_hash_count,
+                            uint64_t *hash_taxid, uint8_t *unknown_in_lca);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Instrumentation (bench.py): kernel launch counter and device time of the dominant kernels.
  * ------------------------------------------------------------------------------------------------------- */
 typedef struct mashgpu_stats {
@@ -321,6 +363,7 @@ typedef struct mashgpu_stats {
     uint64_t exact_reruns;         /* units that needed the exact re-run path */
     double translate_kernel_ms;    /* accumulated device time of the six-frame translation kernel (translated screen) */
     uint64_t translate_kernel_launches;
+    double taxonomy_ms;            /* accumulated device time of mashgpu_screen_taxonomy's kernels, copies and scans */
 } mashgpu_stats;
 /* timing != 0 brackets the dominant kernels with CUDA events (adds a sync at mashgpu_get_stats). */
 int mashgpu_set_timing(mashgpu_ctx *ctx, int timing);

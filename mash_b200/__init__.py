@@ -6,7 +6,7 @@ libmashgpu.so has not been built (`python -c "import __graft_entry__ as g; g.bui
 Engine() fails if no CUDA device is present.
 """
 from ._capi import (Engine, MashGpuError, SketchParams, DistParams, lib_path, load_library,
-                    ALPHABET_NUCLEOTIDE, ALPHABET_PROTEIN)
+                    ALPHABET_NUCLEOTIDE, ALPHABET_PROTEIN, TAX_NONE)
 
 __all__ = ["Engine", "MashGpuError", "SketchParams", "DistParams", "lib_path", "load_library",
-           "ALPHABET_NUCLEOTIDE", "ALPHABET_PROTEIN"]
+           "ALPHABET_NUCLEOTIDE", "ALPHABET_PROTEIN", "TAX_NONE"]

@@ -52,7 +52,16 @@ class SketchSet(C.Structure):
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("scan_kernel_ms", C.c_double), ("scan_kernel_launches", C.c_uint64),
                 ("dist_kernel_ms", C.c_double), ("dist_kernel_launches", C.c_uint64), ("exact_reruns", C.c_uint64),
-                ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64)]
+                ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64), ("taxonomy_ms", C.c_double)]
+
+
+class TaxRow(C.Structure):
+    """mashgpu_tax_row (one key of the reference's counts map, TaxCounts taxdb.hpp:40-46)."""
+    _fields_ = [("taxid", C.c_uint64), ("tax_count", C.c_uint64), ("tax_hash_count", C.c_uint64),
+                ("clade_count", C.c_uint64), ("clade_hash_count", C.c_uint64)]
+
+
+TAX_NONE = 0xFFFFFFFF          # MASHGPU_TAX_NONE: a sketch without a taxID
 
 
 def lib_path():
@@ -115,6 +124,9 @@ def load_library():
     L.mashgpu_dist_open_encoded.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64,
                                             C.POINTER(DistParams), C.POINTER(C.c_void_p)]
     L.mashgpu_screen_set_winner.argtypes = [C.c_void_p, C.c_int]
+    L.mashgpu_taxonomy_open.argtypes = [C.c_void_p, C.c_uint64, u32p, u64p, C.POINTER(C.c_void_p)]
+    L.mashgpu_taxonomy_close.argtypes = [C.c_void_p]
+    L.mashgpu_screen_taxonomy.argtypes = [C.c_void_p, C.c_void_p, u32p, C.c_uint32, u64p, C.c_void_p, C.c_uint64, u64p, u64p, u64p, u64p, u8p]
     L.mashgpu_set_timing.argtypes = [C.c_void_p, C.c_int]
     L.mashgpu_get_stats.argtypes = [C.c_void_p, C.POINTER(Stats), C.c_int]
     _lib = L
@@ -315,6 +327,10 @@ class Engine:
     def screen_open(self, ref, ref_n, p, ref_len=None):
         return ScreenJob(self, ref, ref_n, p, ref_len)
 
+    def taxonomy_open(self, parent, taxid):
+        """Dense taxonomy in device memory: parent[i] = index of node i's parent (i for a root), taxid[i] its taxID."""
+        return Taxonomy(self, parent, taxid)
+
     # ---- instrumentation -----------------------------------------------------------------------------------
     def set_timing(self, on=True):
         self._check(self.lib.mashgpu_set_timing(self.h, int(on)))
@@ -457,7 +473,43 @@ class ScreenJob:
                                                            C.byref(set_size), _p(mix, u64p), C.byref(mix_n)))
         return dict(shared=shared, median=median, identity=ident, pvalue=pv, set_size=set_size.value, mixture=mix[:mix_n.value].copy())
 
+    def taxonomy(self, tax, ref_code, unknown_taxid=(), hash_taxid=False):
+        """`mash taxscreen` after the last feed: LCA taxon of every distinct hash, per-taxon counts and their roll-up.
+        ref_code[r]: node index, n_nodes + u for unknown_taxid[u], or TAX_NONE.  Returns dict(rows (structured array of
+        taxid, tax_count, tax_hash_count, clade_count, clade_hash_count), total_count, total_hash_count,
+        hash_taxid (ascending hash order, or None), unknown_in_lca)."""
+        code = np.ascontiguousarray(ref_code, np.uint32)
+        unk = np.ascontiguousarray(unknown_taxid, np.uint64)
+        cap = tax.n_nodes + unk.size + 2
+        rows = (TaxRow * cap)()
+        n_rows = C.c_uint64(0); tc = C.c_uint64(0); thc = C.c_uint64(0)
+        _, n_distinct = self.counters()
+        ht = np.zeros(max(1, n_distinct), np.uint64) if hash_taxid else None
+        flags = np.zeros(max(1, unk.size), np.uint8)
+        self.eng._check(self.eng.lib.mashgpu_screen_taxonomy(self.h, tax.h, _p(code, u32p) if code.size else None, unk.size,
+                                                             _p(unk, u64p) if unk.size else None, C.cast(rows, C.c_void_p), cap,
+                                                             C.byref(n_rows), C.byref(tc), C.byref(thc), _p(ht, u64p), _p(flags, u8p)))
+        out = np.frombuffer(rows, dtype=np.dtype([(f, "<u8") for f, _ in TaxRow._fields_]))[:n_rows.value].copy()
+        return dict(rows=out, total_count=tc.value, total_hash_count=thc.value,
+                    hash_taxid=ht[:n_distinct].copy() if hash_taxid else None, unknown_in_lca=flags[:unk.size].astype(bool))
+
     def close(self):
         if self.h:
             self.eng.lib.mashgpu_screen_close(self.h)
+            self.h = None
+
+
+class Taxonomy:
+    def __init__(self, eng, parent, taxid):
+        self.eng = eng
+        self.parent = np.ascontiguousarray(parent, np.uint32)
+        self.taxid = np.ascontiguousarray(taxid, np.uint64)
+        self.n_nodes = int(self.taxid.size)
+        h = C.c_void_p()
+        eng._check(eng.lib.mashgpu_taxonomy_open(eng.h, self.n_nodes, _p(self.parent, u32p), _p(self.taxid, u64p), C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if self.h:
+            self.eng.lib.mashgpu_taxonomy_close(self.h)
             self.h = None

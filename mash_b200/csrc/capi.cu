@@ -51,7 +51,7 @@ extern "C" void mashgpu_destroy(mashgpu_ctx *ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    for (auto *list : {&ctx->scan_events, &ctx->dist_events})
+    for (auto *list : {&ctx->scan_events, &ctx->dist_events, &ctx->tax_events})
         for (auto &ev : *list) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     for (int b = 0; b < 2; b++) {
         if (ctx->pinned[b]) cudaFreeHost(ctx->pinned[b]);
@@ -101,6 +101,7 @@ extern "C" int mashgpu_get_stats(mashgpu_ctx *ctx, mashgpu_stats *out, int reset
     drain(ctx->scan_events, ctx->scan_ms);
     drain(ctx->dist_events, ctx->dist_ms);
     drain(ctx->translate_events, ctx->translate_ms);
+    drain(ctx->tax_events, ctx->tax_ms);
     out->kernel_launches = ctx->kernel_launches;
     out->scan_kernel_ms = ctx->scan_ms;
     out->scan_kernel_launches = ctx->scan_launches;
@@ -109,9 +110,10 @@ extern "C" int mashgpu_get_stats(mashgpu_ctx *ctx, mashgpu_stats *out, int reset
     out->exact_reruns = ctx->exact_reruns;
     out->translate_kernel_ms = ctx->translate_ms;
     out->translate_kernel_launches = ctx->translate_launches;
+    out->taxonomy_ms = ctx->tax_ms;
     if (reset) {
         ctx->kernel_launches = ctx->scan_launches = ctx->dist_launches = ctx->exact_reruns = ctx->translate_launches = 0;
-        ctx->scan_ms = ctx->dist_ms = ctx->translate_ms = 0;
+        ctx->scan_ms = ctx->dist_ms = ctx->translate_ms = ctx->tax_ms = 0;
     }
     return MASHGPU_OK;
 }

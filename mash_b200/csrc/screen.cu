@@ -27,6 +27,7 @@
 #include "pack.h"
 #include "sketch_core.cuh"
 #include "binom.cuh"
+#include "screen_view.cuh"
 
 namespace mashgpu {
 
@@ -744,6 +745,18 @@ extern "C" int mashgpu_screen_merge_mixtures_dev(mashgpu_screen_job *job, const 
         MG_CUDA(ctx, cudaMemcpyAsync(&job->h_mix_top, job->mix.p + (job->h_mix_n - 1), 8, cudaMemcpyDeviceToHost, st));
         MG_CUDA(ctx, cudaStreamSynchronize(st));
     }
+    return MASHGPU_OK;
+}
+
+int mashgpu::screen_table_view(mashgpu_screen_job *job, ScreenTableView *v)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    MG_TRY(screen_flush_acc(job));
+    MG_TRY(screen_collect(job));
+    MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    *v = ScreenTableView{ctx, job->n_ref, job->stride, job->ref_hashes, job->ref_n, job->h_n.data(), job->keys.p, job->slot_idx.p, job->cnt.p,
+                         job->log2cap, job->n_distinct};
     return MASHGPU_OK;
 }
 

@@ -1,9 +1,9 @@
-// mash.cpp -- thin command-line front end over the host shim: `mash sketch | dist | triangle | screen | info`.
+// mash.cpp -- thin command-line front end over the host shim: `mash sketch | dist | triangle | screen | taxscreen | info | paste`.
 // Mirrors the reference's command drivers (CommandSketch.cpp:36-169, CommandDistance.cpp:44-304,
-// CommandTriangle.cpp:45-214, CommandScreen.cpp:54-461, CommandInfo.cpp:222-299): same option identifiers and
-// defaults (Command.cpp:165-200), same stdout formats (iostream default precision), same ordering contracts.
-// It exists so that the reference's `make test` flow can be replayed against the GPU engine; help text, `paste`,
-// `bounds`, `taxscreen`, `within` and `find` are out of scope.
+// CommandTriangle.cpp:45-214, CommandScreen.cpp:54-461, CommandTaxScreen.cpp:57-480, CommandInfo.cpp:222-299): same option
+// identifiers and defaults (Command.cpp:165-200), same stdout formats (iostream default precision), same ordering contracts.
+// It exists so that the reference's `make test` flow can be replayed against the GPU engine; help text, `bounds`,
+// `within` and `find` are out of scope.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -21,6 +21,7 @@
 
 #include "fastout.hpp"
 #include "fastx.hpp"
+#include "taxdb.hpp"
 
 using namespace std;
 using namespace mash;
@@ -468,6 +469,60 @@ int runTriangle(int argc, const char **argv)
 }
 
 // ---------------------------------------------------------------------------------------------------- screen
+// The stream of `mash screen` and `mash taxscreen` (CommandScreen.cpp:156-270, CommandTaxScreen.cpp:212-384): round robin over
+// the input files arguments[1..], '*'-joined chunks of 64 MiB instead of 1 MiB (any split gives the same counts) fed to the
+// job.  Exits with the reference's messages on a bad input.
+void streamInputs(mashgpu_screen_job *job, const vector<string> &arguments, int kmerSize, bool trans)
+{
+    int queryCount = (int)arguments.size() - 1;
+    cerr << (trans ? "Translating from " : "Streaming from ");
+    if (queryCount == 1) cerr << arguments[1]; else cerr << queryCount << " inputs";
+    cerr << "..." << endl;
+    vector<gzFile> fps;
+    std::vector<mashhost::FastxReader *> readers;
+    for (size_t f = 1; f < arguments.size(); f++) {
+        if (arguments[f] == "-" && f > 1) { cerr << "ERROR: '-' for stdin must be first query" << endl; exit(1); }
+        gzFile fp = mashhost::FastxReader::openPath(arguments[f]);
+        if (fp == 0) { cerr << "ERROR: could not open " << arguments[f] << endl; exit(1); }
+        fps.push_back(fp);
+        readers.push_back(new mashhost::FastxReader(fp));
+    }
+    const size_t chunkSize = 64u << 20;
+    string input;
+    input.reserve(chunkSize + (1 << 20));
+    uint64_t count = 0;
+    int lstate = 0;
+    size_t it = 0;
+    auto flush = [&]() {
+        if (input.empty()) return;
+        if (mashgpu_screen_feed(job, input.data(), input.size()) != MASHGPU_OK) gpuFail();
+        input.clear();
+    };
+    while (!readers.empty()) {
+        int len = readers[it]->read();
+        lstate = len;
+        if (len < -1) break;
+        if (len == -1) {
+            delete readers[it];
+            readers.erase(readers.begin() + it);
+            if (it >= readers.size()) it = 0;
+            continue;
+        }
+        if (input.length() + (len >= kmerSize ? len + 1 : 0) > chunkSize) flush();
+        count++;
+        if (len >= kmerSize) {
+            input.append(1, '*');
+            input.append(readers[it]->seq.data(), readers[it]->seq.size());
+        }
+        it++;
+        if (it >= readers.size()) it = 0;
+    }
+    flush();
+    if (lstate != -1) { cerr << "\nERROR: reading inputs" << endl; exit(1); }
+    for (gzFile fp : fps) gzclose(fp);
+    if (count == 0) { cerr << "\nERROR: Did not find sequence records in inputs" << endl; exit(1); }
+}
+
 int runScreen(int argc, const char **argv)
 {
     Command c;
@@ -500,56 +555,7 @@ int runScreen(int argc, const char **argv)
     mashgpu_screen_job *job = 0;
     if (mashgpu_screen_open(gpuContext(), &p, &set, &job) != MASHGPU_OK) gpuFail();
     if (c.opt("winning!").active && mashgpu_screen_set_winner(job, 1) != MASHGPU_OK) gpuFail();     // -w, CommandScreen.cpp:357-407
-    int queryCount = (int)c.arguments.size() - 1;
-    cerr << (trans ? "Translating from " : "Streaming from ");
-    if (queryCount == 1) cerr << c.arguments[1]; else cerr << queryCount << " inputs";
-    cerr << "..." << endl;
-    // round robin over the mixture files, '*'-joined chunks (reference CommandScreen.cpp:156-270; chunks of 64 MiB
-    // instead of 1 MiB -- any split gives the same counts)
-    vector<gzFile> fps;
-    std::vector<mashhost::FastxReader *> readers;
-    for (size_t f = 1; f < c.arguments.size(); f++) {
-        if (c.arguments[f] == "-" && f > 1) { cerr << "ERROR: '-' for stdin must be first query" << endl; exit(1); }
-        gzFile fp = mashhost::FastxReader::openPath(c.arguments[f]);
-        if (fp == 0) { cerr << "ERROR: could not open " << c.arguments[f] << endl; exit(1); }
-        fps.push_back(fp);
-        readers.push_back(new mashhost::FastxReader(fp));
-    }
-    const size_t chunkSize = 64u << 20;
-    string input;
-    input.reserve(chunkSize + (1 << 20));
-    uint64_t count = 0;
-    int lstate = 0;
-    size_t it = 0;
-    const int kmerSize = parameters.kmerSize;
-    auto flush = [&]() {
-        if (input.empty()) return;
-        if (mashgpu_screen_feed(job, input.data(), input.size()) != MASHGPU_OK) gpuFail();
-        input.clear();
-    };
-    while (!readers.empty()) {
-        int len = readers[it]->read();
-        lstate = len;
-        if (len < -1) break;
-        if (len == -1) {
-            delete readers[it];
-            readers.erase(readers.begin() + it);
-            if (it >= readers.size()) it = 0;
-            continue;
-        }
-        if (input.length() + (len >= kmerSize ? len + 1 : 0) > chunkSize) flush();
-        count++;
-        if (len >= kmerSize) {
-            input.append(1, '*');
-            input.append(readers[it]->seq.data(), readers[it]->seq.size());
-        }
-        it++;
-        if (it >= readers.size()) it = 0;
-    }
-    flush();
-    if (lstate != -1) { cerr << "\nERROR: reading inputs" << endl; exit(1); }
-    for (gzFile fp : fps) gzclose(fp);
-    if (count == 0) { cerr << "\nERROR: Did not find sequence records in inputs" << endl; exit(1); }
+    streamInputs(job, c.arguments, parameters.kmerSize, trans);
     const uint64_t n = sketch.getReferenceCount();
     vector<uint64_t> shared(n), median(n); vector<double> identity(n), pValue(n);
     uint64_t setSize = 0;
@@ -566,6 +572,165 @@ int runScreen(int argc, const char **argv)
                  << '\t' << sketch.getReference(i).name << '\t' << sketch.getReference(i).comment << endl;
         }
     }
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- taxscreen
+// reference CommandTaxScreen.cpp:57-480: the screen stream, then the LCA taxon of every distinct reference hash, per-taxon
+// counts and their roll-up on the GPU (mashgpu_screen_taxonomy), and the Kraken-style report (taxdb.hpp)
+int runTaxScreen(int argc, const char **argv)
+{
+    Command c;
+    c.add("help", Option(Option::Boolean, "h", ""));
+    c.add("threads", Option(Option::Integer, "p", "1"));
+    c.add("identity", Option(Option::Number, "i", "0", -1., 1.));      // parsed and unused, as in the reference
+    c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
+    c.add("mapping-file", Option(Option::String, "m", ""));
+    c.add("taxonomy-dir", Option(Option::String, "t", "."));
+    if (c.parse(argc, argv)) return 1;
+    if (c.arguments.size() < 2 || c.opt("help").active) { cerr << "usage: mash taxscreen [options] <queries>.msh <pool> [<pool>] ..." << endl; return 0; }
+    if (!hasSuffix(c.arguments[0], suffixSketch)) {
+        cerr << "ERROR: " << c.arguments[0] << " does not look like a sketch (.msh)" << endl;
+        exit(1);
+    }
+    const string taxonomyDir = c.opt("taxonomy-dir").argument, mappingFileName = c.opt("mapping-file").argument;
+    Sketch sketch;
+    Sketch::Parameters parameters;
+    vector<string> refArgVector(1, c.arguments[0]);
+    sketch.initFromFiles(refArgVector, parameters);
+    parameters = sketch.getParameters();
+    string alphabet;
+    sketch.getAlphabetAsString(alphabet);
+    const bool trans = alphabet == alphabetProtein;
+    const string namesDumpFile = taxonomyDir + "/names.dmp", nodesDumpFile = taxonomyDir + "/nodes.dmp";
+    if (!ifstream(namesDumpFile).good() || !ifstream(nodesDumpFile).good()) {
+        cerr << "Could not find a file names.dmp or nodes.dmp in directory " << taxonomyDir << "\n"
+             << " To download the required taxonomy files into the current directory, use the following commands:\n"
+             << "   wget ftp://ftp.ncbi.nih.gov/pub/taxonomy/taxdump.tar.gz\n"
+             << "   tar xvvf taxdump.tar.gz\n"
+             << endl;
+        exit(1);
+    }
+    cerr << "Loading taxonomy files ..." << endl;
+    mashhost::TaxTree tax;
+    tax.load(namesDumpFile, nodesDumpFile, cerr);
+    cerr << "Reading mapping file ..." << endl;
+    const uint64_t n = sketch.getReferenceCount();
+    vector<uint64_t> referenceTaxIDs(n, 0);
+    if (mappingFileName != "") {                 // lines "taxID<one byte>reference name"; the first line of a name wins
+        string text;
+        if (!mashhost::readFile(mappingFileName, text)) throw std::runtime_error("unable to open mapping file");
+        mashhost::IStream in(text.data(), text.data() + text.size());
+        unordered_map<string, uint64_t> refTaxMap;
+        uint64_t taxID = 0;
+        string referenceID;
+        while (in.num(taxID)) {
+            in.ignore(1);
+            in.getline(referenceID, '\n');
+            refTaxMap.emplace(referenceID, taxID);
+        }
+        for (uint64_t i = 0; i < n; i++) {
+            auto it = refTaxMap.find(sketch.getReference(i).name);
+            if (it != refTaxMap.end()) referenceTaxIDs[i] = it->second;
+        }
+    }
+    for (uint64_t i = 0; i < n; i++) {          // otherwise the number after the word "taxid" in the comment (the last one)
+        uint64_t taxID = referenceTaxIDs[i];
+        if (taxID == 0) {
+            const string &comment = sketch.getReference(i).comment;
+            mashhost::IStream in(comment.data(), comment.data() + comment.size());
+            string word;
+            while (in.word(word))
+                if (word == "taxid") in.num(taxID);
+        }
+        if (taxID == 0) cerr << "Could not find taxID for reference " << sketch.getReference(i).name << " in comment field or mapping file!" << endl;
+        else referenceTaxIDs[i] = taxID;
+    }
+    cerr << "Loading " << c.arguments[0] << "..." << endl;
+    mashgpu_sketch_params p;
+    fillGpuParams(p, parameters);
+    mashgpu_sketch_set set;
+    vector<uint64_t> h, l; vector<uint32_t> nn;
+    sketch.toSketchSet(set, h, nn, l);
+    mashgpu_screen_job *job = 0;
+    if (mashgpu_screen_open(gpuContext(), &p, &set, &job) != MASHGPU_OK) gpuFail();
+    uint32_t *dCounters = 0;
+    uint64_t nDistinct = 0;
+    if (mashgpu_screen_counters(job, &dCounters, &nDistinct) != MASHGPU_OK) gpuFail();
+    cerr << "   " << nDistinct << " distinct hashes." << endl;
+    streamInputs(job, c.arguments, parameters.kmerSize, trans);
+    uint64_t setSize = 0;
+    if (mashgpu_screen_finish(job, 0, 0, 0, 0, &setSize, 0, 0) != MASHGPU_OK) gpuFail();
+    cerr << "   Estimated distinct" << (trans ? " (translated)" : "") << " k-mers in pool: " << setSize << endl;
+    if (setSize == 0) cerr << "WARNING: no valid k-mers in input." << endl;
+    cerr << "Assigning LCA taxIDs to hashes ..." << endl;
+    // sketch codes: taxonomy node, or a slot per distinct taxID outside the taxonomy (ascending), or none for taxID 0
+    vector<uint64_t> unknown;
+    for (uint64_t t : referenceTaxIDs)
+        if (t != 0 && tax.find(t) < 0) unknown.push_back(t);
+    sort(unknown.begin(), unknown.end());
+    unknown.erase(unique(unknown.begin(), unknown.end()), unknown.end());
+    vector<uint32_t> code(n);
+    for (uint64_t i = 0; i < n; i++) {
+        const uint64_t t = referenceTaxIDs[i];
+        const int64_t node = tax.find(t);
+        if (t == 0) code[i] = MASHGPU_TAX_NONE;
+        else if (node >= 0) code[i] = (uint32_t)node;
+        else code[i] = (uint32_t)(tax.taxid.size() + (lower_bound(unknown.begin(), unknown.end(), t) - unknown.begin()));
+    }
+    mashgpu_taxonomy *gtax = 0;
+    if (mashgpu_taxonomy_open(gpuContext(), tax.taxid.size(), tax.parent.data(), tax.taxid.data(), &gtax) != MASHGPU_OK) gpuFail();
+    vector<mashgpu_tax_row> rows(tax.taxid.size() + unknown.size() + 2);
+    vector<uint8_t> unknownInLca(unknown.size());
+    uint64_t nRows = 0, totalCount = 0, totalHashCount = 0;
+    if (mashgpu_screen_taxonomy(job, gtax, code.data(), (uint32_t)unknown.size(), unknown.data(), rows.data(), rows.size(), &nRows,
+                                &totalCount, &totalHashCount, 0, unknownInLca.data()) != MASHGPU_OK) gpuFail();
+    rows.resize(nRows);
+    mashgpu_taxonomy_close(gtax);
+    mashgpu_screen_close(job);
+    // the reference prints this once per LCA call that meets the taxID (taxdb.hpp:166, 172), a number that depends on hash-set
+    // order; here once per taxID that met another sketch's taxID in a fold
+    for (size_t u = 0; u < unknown.size(); u++)
+        if (unknownInLca[u]) cerr << "TaxID " << unknown[u] << " not in database - ignoring it.\n";
+    vector<uint64_t> outside;                    // the roll-up's getEntry of a taxon outside the taxonomy (taxdb.hpp:74-82), ascending
+    for (const auto &r : rows)
+        if (tax.find(r.taxid) < 0) outside.push_back(r.taxid);
+    sort(outside.begin(), outside.end());
+    for (uint64_t t : outside) cerr << "Couldn't find tax entry with taxID " << t << endl;
+    cerr << "Writing output..." << endl;
+    mashhost::writeTaxReport(stdout, tax, rows, totalCount);
+    return 0;
+}
+
+// test helpers of the taxonomy reader and the report writer (no GPU):
+//   mash tax-dump <dir>              every node: taxid, parent taxid (itself for a root), rank, name, tab-separated, ascending taxid
+//   mash tax-report <dir> <rows>     the report of the rows "taxid taxCount taxHashCount cladeCount cladeHashCount" (one per
+//                                    line, first line "totalCount totalHashCount")
+int runTaxDump(int argc, const char **argv)
+{
+    if (argc < 1) { cerr << "usage: mash tax-dump <taxonomy dir>" << endl; return 1; }
+    mashhost::TaxTree tax;
+    tax.load(string(argv[0]) + "/names.dmp", string(argv[0]) + "/nodes.dmp", cerr);
+    vector<uint32_t> order(tax.taxid.size());
+    for (uint32_t i = 0; i < order.size(); i++) order[i] = i;
+    sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return tax.taxid[a] < tax.taxid[b]; });
+    for (uint32_t i : order)
+        cout << tax.taxid[i] << '\t' << tax.taxid[tax.parent[i]] << '\t' << tax.rank[i] << '\t' << tax.name[i] << '\n';
+    return 0;
+}
+
+int runTaxReport(int argc, const char **argv)
+{
+    if (argc < 2) { cerr << "usage: mash tax-report <taxonomy dir> <rows>" << endl; return 1; }
+    mashhost::TaxTree tax;
+    tax.load(string(argv[0]) + "/names.dmp", string(argv[0]) + "/nodes.dmp", cerr);
+    ifstream in(argv[1]);
+    uint64_t totalCount = 0, totalHashCount = 0;
+    in >> totalCount >> totalHashCount;
+    vector<mashgpu_tax_row> rows;
+    mashgpu_tax_row r;
+    while (in >> r.taxid >> r.tax_count >> r.tax_hash_count >> r.clade_count >> r.clade_hash_count) rows.push_back(r);
+    mashhost::writeTaxReport(stdout, tax, rows, totalCount);
     return 0;
 }
 
@@ -739,6 +904,9 @@ static int runCommand(int argc, const char **argv)
     if (cmd == "dist") return runDist(argc - 2, argv + 2);
     if (cmd == "triangle") return runTriangle(argc - 2, argv + 2);
     if (cmd == "screen") return runScreen(argc - 2, argv + 2);
+    if (cmd == "taxscreen") return runTaxScreen(argc - 2, argv + 2);
+    if (cmd == "tax-dump") return runTaxDump(argc - 2, argv + 2);
+    if (cmd == "tax-report") return runTaxReport(argc - 2, argv + 2);
     if (cmd == "info") return runInfo(argc - 2, argv + 2);
     if (cmd == "paste") return runPaste(argc - 2, argv + 2);
     if (cmd == "import-json") return runImportJson(argc - 2, argv + 2);
@@ -749,7 +917,7 @@ static int runCommand(int argc, const char **argv)
 int main(int argc, const char **argv)
 {
     if (argc < 2) {
-        cerr << "usage: mash <sketch|dist|triangle|screen|info> ...   (H100 engine; see INTEGRATION.md)" << endl;
+        cerr << "usage: mash <sketch|dist|triangle|screen|taxscreen|info|paste> ...   (H100 engine; see INTEGRATION.md)" << endl;
         return 0;
     }
     const int rc = runCommand(argc, argv);
