@@ -396,28 +396,45 @@ __shared__ uint64_t scan_sq_hash[SCAN_WARPS][SCAN_SQ];
 __shared__ uint64_t scan_sq_pos[SCAN_WARPS][SCAN_SQ];
 __shared__ uint32_t scan_sq_n[SCAN_WARPS];   // entries appended since the last flush (may exceed SCAN_SQ: those went direct)
 
-// Slow path of the filter-word kernels: one out-of-line call per vote group that has a survivor.  Bit j of `pm` = window
-// lp0 + j passed the fast-path filter; each lane rebuilds the exact hash of its own passing windows from the tile, and the
-// lanes whose window is valid and at or below the tile threshold queue it for its table work.
+// Slow path of the filter-word kernels, once per warp tile that has a survivor.  A lane's pass mask covers its 32 windows of
+// the tile: bit 8 i + j = window j of the lane's block i (window start 8 (lane + 32 i) + j) passed the fast-path filter.  The
+// lanes walk their set bits together (a lane with none left idles), rebuild the exact hash of each passing window from the
+// tile, and queue the valid ones at or below the tile threshold for their table work.
+#ifndef SCAN_RESOLVE_INLINE
+#define SCAN_RESOLVE_INLINE 0   // 1: inline the per-tile resolution into scan_kernel (tools/scan_microbench.cu compares both)
+#endif
 template <int K, bool CANON>
-static __device__ __noinline__ void scan_survivors(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint32_t lp0, uint64_t tile_base,
-                                                   uint64_t tmax)
+static __device__ __forceinline__ void scan_resolve_body(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
 {
-    const uint32_t warp = threadIdx.x >> 5;
-    while (pm) {
-        const uint32_t lp = lp0 + __ffs(pm) - 1;
-        pm &= pm - 1;
-        uint64_t hash;
-        if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) {
-            const uint32_t at = atomicAdd(&scan_sq_n[warp], 1u);
-            if (at < SCAN_SQ) {
-                scan_sq_hash[warp][at] = hash;
-                scan_sq_pos[warp][at] = tile_base + lp;
-            } else {
-                scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), tile_base, lp);
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    while (__any_sync(0xFFFFFFFFu, pm != 0)) {
+        if (pm) {
+            const uint32_t bit = __ffs(pm) - 1;
+            pm &= pm - 1;
+            const uint32_t lp = 8 * (lane + 32 * (bit >> 3)) + (bit & 7);
+            uint64_t hash;
+            if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) {
+                const uint32_t at = atomicAdd(&scan_sq_n[warp], 1u);
+                if (at < SCAN_SQ) {
+                    scan_sq_hash[warp][at] = hash;
+                    scan_sq_pos[warp][at] = tile_base + lp;
+                } else {
+                    scan_emit(a, (uint32_t)hash, (uint32_t)(hash >> 32), tile_base, lp);
+                }
             }
         }
     }
+}
+template <int K, bool CANON>
+static __device__ __noinline__ void scan_resolve_call(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
+{
+    scan_resolve_body<K, CANON>(a, pm, sm_addr, tile_base, tmax);
+}
+template <int K, bool CANON>
+__device__ __forceinline__ void scan_resolve(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
+{
+    if (SCAN_RESOLVE_INLINE) scan_resolve_body<K, CANON>(a, pm, sm_addr, tile_base, tmax);
+    else scan_resolve_call<K, CANON>(a, pm, sm_addr, tile_base, tmax);
 }
 
 // Table work of the queued survivors of this warp, one per lane; warp-uniform call, leaves the queue empty
@@ -437,8 +454,9 @@ static __device__ __noinline__ void scan_sq_flush(const ScanArgs &a)
 
 // Cost-accounting switches for tools/scan_microbench.cu (0 in the library; see DESIGN.md §2.4).  Each takes one part of
 // the kernel out or measures it; the kernel's results are not what the library needs when one of them is set.
-//   SCAN_MB_NO_SURVIVORS: no warp vote and no survivor call; the filter words are xor-ed into a per-lane accumulator
-//                         that is stored once at the end (a.out_hash[global thread]), so the hash stays live.
+//   SCAN_MB_NO_SURVIVORS: (filter-word kernels) no per-tile resolution of the pass masks; each tile's mask is xor-ed into a
+//                         per-lane accumulator that is stored once at the end (a.out_hash[global thread]), so the hash and
+//                         the compare stay live.
 //   SCAN_MB_STAGE_ONCE:   each warp stages its first tile only and hashes it again in place of every later tile: no
 //                         staging and no global prefetch after the first.
 //   SCAN_MB_CLOCK:        clock64() around each tile's hot loop; lane 0 stores the warp's total cycles at
@@ -453,8 +471,13 @@ static __device__ __noinline__ void scan_sq_flush(const ScanArgs &a)
 #define SCAN_MB_CLOCK 0
 #endif
 #ifndef SCAN_VOTE_GROUP
-#define SCAN_VOTE_GROUP 2      // windows hashed back to back before one warp vote (1, 2, 4 or 8); see scan_group_filter.
-                               // tools/scan_microbench.cu compares the settings (-DSCAN_VOTE_GROUP=n); on H100 2 beat 4 and 8
+#define SCAN_VOTE_GROUP 2      // FULL kernels only: windows hashed back to back before one warp vote (1, 2, 4 or 8); see
+                               // scan_group.  The filter-word kernels do not vote in the hot loop (per-lane pass masks,
+                               // resolved once per tile).  On H100 2 beat 4 and 8 (filter-word kernel, before the masks)
+#endif
+#ifndef SCAN_PREFETCH_SMEM
+#define SCAN_PREFETCH_SMEM 1   // filter-word kernels: 1 = the next tile is prefetched by cp.async into a per-warp shared landing
+                               // buffer, 0 = into registers (as the FULL kernels do); tools/scan_microbench.cu compares them
 #endif
 
 // ASCII words of the canonical k-mer of window J of the block (b = forward words, rb = reverse-complement words)
@@ -512,20 +535,14 @@ __device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const 
     return murmur3_h1_filter<K, S::NA>(asc, a.seed);
 }
 
-// G consecutive windows J0 .. J0+G-1 hashed back to back (independent multiply chains that ptxas can interleave), ONE warp
-// vote, and one out-of-line slow-path call for the group.  The hot path only compares and votes; the per-lane bit mask of
-// passing windows is built inside the (rarely taken) branch.
-template <int K, bool CANON, int J0, int... J>
-__device__ __forceinline__ void scan_group_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
-                                                  uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t tf, uint32_t pool, uint32_t sm_addr,
-                                                  uint32_t &mb_acc, std::integer_sequence<int, J...>)
+// The 8 windows of a block hashed back to back (independent multiply chains that ptxas can interleave), their pass flags
+// at bits 24..31 of the result (bit 24 + j = window j).  No vote and no branch: the hot loop shifts the block's flags into
+// the lane's pass mask, and the mask is resolved once per tile (scan_resolve).
+template <int K, bool CANON, int... J>
+__device__ __forceinline__ uint32_t scan_block_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
+                                                      uint32_t tf, uint32_t pool, std::integer_sequence<int, J...>)
 {
-    const uint32_t x[] = {scan_window_filter<K, CANON, J0 + J>(a, b, rb, pool)...};
-    mb_acc ^= (x[J] ^ ...);
-    if (!SCAN_MB_NO_SURVIVORS && __any_sync(0xFFFFFFFFu, ((x[J] <= tf) || ...))) {
-        const uint32_t pm = (((x[J] <= tf ? 1u : 0u) << J) | ...);
-        scan_survivors<K, CANON>(a, pm, sm_addr, local0 + J0, tile_base, tmax);
-    }
+    return (((scan_window_filter<K, CANON, J>(a, b, rb, pool) <= tf ? 1u : 0u) << (24 + J)) | ...);
 }
 
 // Full-hash variant of the group: G windows, one warp vote, then the survivors of each window serialised by scan_emit_warp.
@@ -580,6 +597,67 @@ __device__ __forceinline__ uint4 load16(const uint8_t *stream, uint64_t off, uin
     return make_uint4(0, 0, 0, 0);
 }
 
+// asynchronous global -> shared copies (cp.async, completed by cp_async_wait_all) of 16, 8 or 4 bytes
+template <int N>
+__device__ __forceinline__ void cp_async(uint32_t dst, const void *src)
+{
+    if (N == 16) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(dst), "l"(src) : "memory");
+    else asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" :: "r"(dst), "l"(src), "n"(N) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all()
+{
+    asm volatile("cp.async.wait_all;" ::: "memory");
+}
+
+__device__ __forceinline__ uint64_t lds_u64(uint32_t addr)
+{
+    uint64_t v;
+    asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint4 lds_u128(uint32_t addr)
+{
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ void sts_u128(uint32_t addr, uint4 v)
+{
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" :: "r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+
+// Prefetch of warp tile `wt` into the warp's landing buffer (shared address `land`), filter-word kernels.  ASCII source: the
+// tile's 68 16-byte vectors, lanes taking vectors lane, lane + 32 and (lanes 0-3) 64 + lane.  A tile that lies wholly
+// before stream_len goes by cp.async; one that reaches past it (the last tile of a launch) is loaded with load16 and stored
+// by the lanes themselves, so no copy touches memory past the caller's buffer.  Packed source: groups lane and (lanes
+// 0, 1) 32 + lane, the 64-bit codes at byte 8 g and the invalid bits at byte 8 * 34 + 4 g -- the words the register
+// prefetch reads.
+constexpr int SCAN_LAND_INVAL = 8 * 34;
+template <bool PACKED>
+__device__ __forceinline__ void scan_prefetch_land(const ScanArgs &a, uint64_t wt, uint32_t land, int lane)
+{
+    if (PACKED) {
+        const uint64_t g0 = wt * (uint64_t)(SCAN_WARP_TILE / 32);
+        cp_async<8>(land + 8 * lane, a.codes + g0 + lane);
+        cp_async<4>(land + SCAN_LAND_INVAL + 4 * lane, a.inval + g0 + lane);
+        if (lane < 2) {
+            cp_async<8>(land + 8 * (32 + lane), a.codes + g0 + 32 + lane);
+            cp_async<4>(land + SCAN_LAND_INVAL + 4 * (32 + lane), a.inval + g0 + 32 + lane);
+        }
+        return;
+    }
+    const uint64_t base = wt * (uint64_t)SCAN_WARP_TILE;
+    if (base + 16ull * SCAN_WARP_VECS <= a.stream_len) {
+        cp_async<16>(land + 16 * lane, a.stream + base + 16ull * lane);
+        cp_async<16>(land + 16 * (lane + 32), a.stream + base + 16ull * (lane + 32));
+        if (lane < 4) cp_async<16>(land + 16 * (64 + lane), a.stream + base + 16ull * (64 + lane));
+    } else {
+        sts_u128(land + 16 * lane, load16(a.stream, base + 16ull * lane, a.stream_len));
+        sts_u128(land + 16 * (lane + 32), load16(a.stream, base + 16ull * (lane + 32), a.stream_len));
+        if (lane < 4) sts_u128(land + 16 * (64 + lane), load16(a.stream, base + 16ull * (64 + lane), a.stream_len));
+    }
+}
+
 // 32 packed positions (2-bit codes + invalid bits) -> 4 nibble words
 __device__ __forceinline__ uint32_t spread_codes8(uint32_t x)   // 8 two-bit codes (16 bits) -> 8 nibbles
 {
@@ -607,16 +685,23 @@ __device__ __forceinline__ uint4 expand32(uint64_t c, uint32_t m)
 }
 
 // Warp-private tiles: every warp owns WARP_TILE window starts at a time, staged in its own slice of shared memory,
-// so the only synchronisation is __syncwarp().  The next tile's bytes are prefetched into registers before the
-// current tile is hashed (global latency hidden behind ~4000 instructions of work per lane).
+// so the only synchronisation is __syncwarp().  The next tile's bytes are prefetched before the current tile is hashed
+// (global latency hidden behind ~4000 instructions of work per lane): by the FULL kernels into registers, by the
+// filter-word kernels into a per-warp shared landing buffer (SCAN_PREFETCH_SMEM), which keeps those registers free
+// through the hot loop.
 #ifndef SCAN_MIN_BLOCKS
-#define SCAN_MIN_BLOCKS 3      // resident CTAs per SM requested from ptxas (=> 80 registers, no spills; 4 => 64 registers
-                               // and spills); tools/scan_microbench.cu compares the settings (-DSCAN_MIN_BLOCKS=n)
+#define SCAN_MIN_BLOCKS 4      // filter-word kernels: resident CTAs per SM requested from ptxas (4 => 64 registers, no spills
+                               // since the hot loop holds neither a survivor call nor prefetch registers; 3 => 80 registers, 1 %
+                               // slower); tools/scan_microbench.cu compares the settings (-DSCAN_MIN_BLOCKS=n)
+#endif
+#ifndef SCAN_MIN_BLOCKS_FULL
+#define SCAN_MIN_BLOCKS_FULL 3 // FULL kernels (=> 80 registers, no spills; 4 => 64 registers and spills)
 #endif
 // FULL: the fast path computes the whole 64-bit hash (k <= 16, where the filter is on the low word, and SCAN_SCREEN, where
 // every lane probes the reference table with it); otherwise only murmur3_h1_filter's word and the slow path recomputes.
 template <int K, bool CANON, bool PACKED, bool FULL>
-__global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) ? 3 : SCAN_MIN_BLOCKS) scan_kernel(const __grid_constant__ ScanArgs a)
+__global__ void __launch_bounds__(SCAN_THREADS, FULL ? ((K > 24 && SCAN_MIN_BLOCKS_FULL > 3) ? 3 : SCAN_MIN_BLOCKS_FULL) : SCAN_MIN_BLOCKS)
+scan_kernel(const __grid_constant__ ScanArgs a)
 {
     using S = KmerShape<K>;
     static_assert(FULL || K > 16, "the filter word is the high word of the hash");
@@ -624,6 +709,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
     // reverse-complement image of the tile (word i = nibble-reversed, complemented word NW-1-i), written once at staging so
     // that a block's reverse-complement words are 4 more LDS (the LSU is idle) instead of ~16 ALU instructions per block
     __shared__ __align__(16) uint32_t smr_all[CANON ? SCAN_WARPS : 1][SCAN_WARP_WORDS];
+    constexpr bool LAND = !FULL && SCAN_PREFETCH_SMEM;
+    __shared__ __align__(16) uint4 land_all[LAND ? SCAN_WARPS : 1][LAND ? SCAN_WARP_VECS : 1];   // next tile's raw bytes
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t *sm = sm_all[warp];
     uint32_t *smr = smr_all[CANON ? warp : 0];
@@ -632,6 +719,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
     // iteration of the hot loop to save a register
     const uint32_t sm_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(sm), 0);
     const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(smr), 0);
+    const uint32_t land = (uint32_t)__cvta_generic_to_shared(land_all[LAND ? warp : 0]);
     const uint32_t fold = a.preserve_case ? 0xFFFFFFFFu : 0xDFDFDFDFu;
     uint32_t pool;   // bytes 'A','C','G','T' for PRMT; opaque to the compiler so that it stays in one register
     asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
@@ -650,7 +738,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
     uint64_t pc0 = 0, pc1 = 0;             // packed source: group (lane) and one of the 2 halo groups (32 + lane%2)
     uint32_t pm0 = 0, pm1 = 0;
     const int hg = 32 + (lane & 1);
-    if (PACKED) {
+    if (LAND) {
+        scan_prefetch_land<PACKED>(a, wt, land, lane);
+    } else if (PACKED) {
         const uint64_t g0 = wt * (uint64_t)(SCAN_WARP_TILE / 32);
         pc0 = __ldg(a.codes + g0 + lane); pm0 = __ldg(a.inval + g0 + lane);
         pc1 = __ldg(a.codes + g0 + hg);   pm1 = __ldg(a.inval + g0 + hg);
@@ -669,6 +759,18 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
     const uint64_t wt_first = wt;
     for (; wt < wt_end; wt += wt_stride) {
         const uint64_t base = wt * (uint64_t)SCAN_WARP_TILE;
+        if (LAND && !(SCAN_MB_STAGE_ONCE && wt != wt_first)) {   // this tile's bytes, copied in during the previous tile
+            cp_async_wait_all();
+            __syncwarp();
+            if (PACKED) {
+                pc0 = lds_u64(land + 8 * lane); pm0 = lds_u32(land + SCAN_LAND_INVAL + 4 * lane);
+                pc1 = lds_u64(land + 8 * hg);   pm1 = lds_u32(land + SCAN_LAND_INVAL + 4 * hg);
+            } else {
+                q0 = lds_u128(land + 16 * lane);
+                q1 = lds_u128(land + 16 * (lane + 32));
+                q2 = lds_u128(land + 16 * v2);
+            }
+        }
         if (SCAN_MB_STAGE_ONCE && wt != wt_first) {
             // microbenchmark only: hash the first tile again
         } else if (PACKED) {
@@ -697,7 +799,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         __syncwarp();
         const uint64_t next = wt + wt_stride;
         if (!SCAN_MB_STAGE_ONCE && next < wt_end) {   // prefetch
-            if (PACKED) {
+            if (LAND) {
+                scan_prefetch_land<PACKED>(a, next, land, lane);
+            } else if (PACKED) {
                 const uint64_t g0 = next * (uint64_t)(SCAN_WARP_TILE / 32);
                 pc0 = __ldg(a.codes + g0 + lane); pm0 = __ldg(a.inval + g0 + lane);
                 pc1 = __ldg(a.codes + g0 + hg);   pm1 = __ldg(a.inval + g0 + hg);
@@ -712,6 +816,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
         const uint64_t tmax = a.tile_tmax ? a.tile_tmax[base / SCAN_TILE] : a.coarse_t;
         const uint32_t tf = filter_threshold((uint32_t)(tmax >> 32));
         const long long c0 = SCAN_MB_CLOCK ? clock64() : 0;
+        static_assert(SCAN_WARP_TILE / 8 == 4 * 32, "a lane's pass mask holds 4 blocks of 8 windows");
+        uint32_t pmask = 0;   // filter-word kernels: the lane's pass flags of this tile, see scan_resolve
 #pragma unroll 1
         for (int g = lane; g < SCAN_WARP_TILE / 8; g += 32) {
             uint32_t b[S::BW], rb[S::BW];
@@ -724,19 +830,8 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
             const uint32_t local0 = 8u * g;
             constexpr int G = SCAN_VOTE_GROUP;
             if constexpr (!FULL) {
-                const auto js = std::make_integer_sequence<int, G>();
-                scan_group_filter<K, CANON, 0>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                if constexpr (G < 8) scan_group_filter<K, CANON, (G < 8 ? G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                if constexpr (G < 4) {
-                    scan_group_filter<K, CANON, (G < 4 ? 2 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                    scan_group_filter<K, CANON, (G < 4 ? 3 * G : 0)>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                }
-                if constexpr (G < 2) {
-                    scan_group_filter<K, CANON, 4>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                    scan_group_filter<K, CANON, 5>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                    scan_group_filter<K, CANON, 6>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                    scan_group_filter<K, CANON, 7>(a, b, rb, base, local0, tmax, tf, pool, sm_addr, mb_acc, js);
-                }
+                // block i = (g - lane) / 32 ends at bits 8 i .. 8 i + 7 after the tile's 4 trips
+                pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, pool, std::make_integer_sequence<int, 8>());
             } else {
                 scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
                 if constexpr (G < 8) scan_group<K, CANON, (G < 8 ? G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
@@ -753,6 +848,10 @@ __global__ void __launch_bounds__(SCAN_THREADS, (K > 24 && SCAN_MIN_BLOCKS > 3) 
             }
         }
         if (SCAN_MB_CLOCK) mb_cycles += clock64() - c0;
+        if (!FULL) {
+            if (SCAN_MB_NO_SURVIVORS) mb_acc ^= pmask;
+            else if (__any_sync(0xFFFFFFFFu, pmask != 0)) scan_resolve<K, CANON>(a, pmask, sm_addr, base, tmax);
+        }
         __syncwarp();
         if (!FULL && scan_sq_n[warp] >= SCAN_SQ_FLUSH) scan_sq_flush(a);
     }

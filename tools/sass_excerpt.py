@@ -39,7 +39,9 @@ def opcode(t):
 
 def hot_path_line(body):
     """The scan kernel's hot path: its longest innermost loop minus the blocks that the branch after each warp vote
-    (VOTE.ANY) skips when no lane has a survivor -- i.e. what a warp issues per 8 windows when nobody passes the filter."""
+    (VOTE.ANY) skips when no lane has a survivor -- i.e. what a warp issues per 8 windows when nobody passes the filter.
+    The filter-word kernels have no vote in the loop (pass masks are resolved after it), so there it is the whole loop; the
+    control instructions it holds are listed."""
     skip = []
     for i, (_, t) in enumerate(body):
         if t.startswith("VOTE.ANY"):
@@ -51,8 +53,11 @@ def hot_path_line(body):
     hot = [(a, t) for a, t in body if not any(x <= a < y for x, y in skip)]
     c = collections.Counter(opcode(t) for _, t in hot)
     alu = sum(n for o, n in c.items() if o in PIPES["ALU (SHF/LOP3/IADD3/PRMT/ISETP/SEL/...)"] + ("VIADD",))
-    return (f"hot path (longest innermost loop without the {len(skip)} survivor blocks behind the warp votes): {len(hot)} "
-            f"instructions per lane per 8 windows; ALU pipe {alu}, IMAD {c['IMAD']}, STL {c['STL']}, LDL {c['LDL']}, S2R {c['S2R']}")
+    ctl = ", ".join(f"{o} {c[o]}" for o in ("VOTE", "CALL", "BSSY", "BSYNC", "BRA") if c[o]) or "none"
+    what = f"without the {len(skip)} survivor blocks behind the warp votes" if skip else "no warp vote in it: the whole loop"
+    return (f"hot path (longest innermost loop, {what}): {len(hot)} "
+            f"instructions per lane per 8 windows; ALU pipe {alu}, IMAD {c['IMAD']}, STL {c['STL']}, LDL {c['LDL']}, S2R {c['S2R']}; "
+            f"control: {ctl}")
 
 
 def main():
@@ -115,11 +120,13 @@ def main():
             lo = collections.Counter(re.sub(r"^@!?U?P\d+\s+", "", t).split()[0].split(".")[0] for _, t in body)
             summary.append("")
             summary.append(f"innermost loop, {len(body)} instructions at {body[0][0]:#x}..{body[-1][0]:#x}: " + ", ".join(f"{o} {c}" for o, c in lo.most_common(12)))
-        for body in loops[:4]:
+        for i, body in enumerate(loops[:4]):
+            # the scan kernels' hot loop in full, so that its control flow can be read off the listing
+            keep = 1200 if i == 0 and name.startswith("scan_kernel") else 400
             excerpt.append(f"\n// ---- loop {body[0][0]:#x}..{body[-1][0]:#x} ({len(body)} instructions)")
-            excerpt += [f"/*{addr:05x}*/  {t}" for addr, t in body[:400]]
-            if len(body) > 400:
-                excerpt.append(f"// ... {len(body) - 400} more")
+            excerpt += [f"/*{addr:05x}*/  {t}" for addr, t in body[:keep]]
+            if len(body) > keep:
+                excerpt.append(f"// ... {len(body) - keep} more")
         tma = [f"/*{addr:05x}*/  {t}" for addr, t in ins if re.search(r"UBLKCP|UTMALDG|SYNCS|UTMASTG", t)]
         if tma:
             excerpt.append("\n// ---- TMA / mbarrier instructions in this kernel")
