@@ -79,9 +79,21 @@ __device__ __forceinline__ uint32_t fmix_hi(u64x2 k, uint32_t add)
     return r + k.lo * (uint32_t)(c >> 32) + k.hi * (uint32_t)c;
 }
 
+// k1 of the tail block, rotl31(t * c1) * c2, where t holds the tail's (at most 8) bytes; when the tail has 8 bytes or fewer,
+// h1 ^= this is all the tail does
+__host__ __device__ __forceinline__ uint64_t murmur3_tail_k1(uint64_t t)
+{
+    t *= 0x87c37b91114253d5ULL;
+    t = (t << 31) | (t >> 33);
+    return t * 0x4cf5ad432745937fULL;
+}
+
 // The body of MurmurHash3_x64_128 up to the finalisation: h1, h2 after the length xor and the two cross adds.
-template <int K, int NA>
-__device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t seed, u64x2 &h1_out, u64x2 &h2_out)
+// K1_GIVEN (tails of 1..8 bytes only): the tail's k1 is `k1_tail` (murmur3_tail_k1, e.g. from a table) and the tail words of
+// `a` are not read.
+template <int K, int NA, bool K1_GIVEN = false>
+__device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t seed, u64x2 &h1_out, u64x2 &h2_out,
+                                             u64x2 k1_tail = u64x2{0u, 0u})
 {
     constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
     constexpr int NB = K / 16, TAIL = K & 15;
@@ -98,7 +110,10 @@ __device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t s
         u64x2 k2{a[4 * NB + 2], a[4 * NB + 3]};
         k2 = mul_const(k2, c2); k2 = rotl<33>(k2); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
     }
-    if constexpr (TAIL > 0) {
+    static_assert(!K1_GIVEN || (TAIL > 0 && TAIL <= 8), "a given k1 replaces the whole tail");
+    if constexpr (K1_GIVEN) {
+        h1 = xor64(h1, k1_tail);
+    } else if constexpr (TAIL > 0) {
         u64x2 k1{a[4 * NB], a[4 * NB + 1]};
         k1 = mul_const(k1, c1); k1 = rotl<31>(k1); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
     }
@@ -125,11 +140,11 @@ __device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t se
 // (carry 0: X = H + 1 <= T + 1;  carry 1: X = H), so `X <= T + 1` (or anything, when T = 2^32 - 1) never rejects a hash
 // whose high word is <= T.  It lets through at most the one extra high word T + 1 and X = 0 (high words summing to
 // 2^32 - 1); the slow path recomputes the exact hash.  tests/test_scan_filter_model.py models this predicate.
-template <int K, int NA>
-__device__ __forceinline__ uint32_t murmur3_h1_filter(const uint32_t (&a)[NA], uint32_t seed)
+template <int K, int NA, bool K1_GIVEN = false>
+__device__ __forceinline__ uint32_t murmur3_h1_filter(const uint32_t (&a)[NA], uint32_t seed, u64x2 k1_tail = u64x2{0u, 0u})
 {
     u64x2 h1, h2;
-    murmur3_body<K, NA>(a, seed, h1, h2);
+    murmur3_body<K, NA, K1_GIVEN>(a, seed, h1, h2, k1_tail);
     uint32_t one;    // opaque, so that ptxas keeps the +1 as the IMAD.HI addend rather than a separate add on the ALU pipe
     asm("mov.u32 %0, 1;" : "=r"(one));
     return fmix_hi(h2, fmix_hi(h1, one));

@@ -290,13 +290,28 @@ struct KmerShape {
     static constexpr int BW = (K + 7 + 7) / 8;       // nibble words per block of 8 window starts
     static constexpr int NA = 2 * NW;                // ASCII words per k-mer
     static constexpr uint32_t LAST_MASK = (K % 8) ? ((1u << (4 * (K % 8))) - 1u) : 0xFFFFFFFFu;
-    // the nibbles of the last word past the k-mer hold code 8: PRMT's sign-replicate of byte 0 of the pool ('A' = 0x41)
-    // turns them into 0x00 bytes, which is what MurmurHash3 reads past the key.  Both strands carry the same padding in
-    // their most significant nibbles, so the canonical compare is decided by the k-mer's own nibbles as before.
-    static constexpr uint32_t LAST_PAD = 0x88888888u & ~LAST_MASK;
+    // the nibbles of the last word past the k-mer hold 0xF: as a PRMT selector that is the sign-replicate of byte 7 of
+    // {0, pool}, a 0x00 byte, which is what MurmurHash3 reads past the key.  The pad is the complement of the mask, so
+    // masking and padding are one OR.  Both strands carry the same padding in their most significant nibbles, so the
+    // canonical compare is decided by the k-mer's own nibbles.
+    static constexpr uint32_t LAST_PAD = ~LAST_MASK;
+    // 17 <= K <= 21 (a tail block of 1..5 bases): the filter-word kernels take the tail's k1 from a table (TailTable)
+    static constexpr bool TAIL_TABLE = K >= 17 && K <= 21;
 };
 
-// nibble words (codes 0..3, padded with code 8 past K) -> ASCII words, bytes >= K zeroed
+// Tail block by table.  For 17 <= K <= 21 the tail block of MurmurHash3 is bases 16..K-1 of the canonical k-mer, and its k1
+// (murmur3_tail_k1 of their ASCII bytes) takes at most 4^5 values and does not depend on the seed.  The filter-word kernels
+// keep the 1024 values in shared memory and replace the tail's two PRMT, two multiplies and rotate by one IMAD, one shift
+// and one 8-byte LDS.  The index is computed from the canonical k-mer's last nibble word with bit 3 and bit 2 of every
+// nibble cleared (codes c0..c4 at bits 0, 4, 8, 12, 16): w * (2^10 + 1) puts c0, c3, c1, c4, c2 side by side at bits
+// 10..19 without overlap and without a carry, and the shift keeps those ten bits.  Windows with a base outside the
+// alphabet read some entry and are rejected by the exact rebuild, as before.
+constexpr uint32_t TAIL_IDX_MUL = 0x401000u;   // (2^10 + 1) << 12
+constexpr int TAIL_IDX_SHIFT = 22;
+constexpr int TAIL_TAB_SIZE = 1024;
+__host__ __device__ __forceinline__ uint32_t tail_index(uint32_t w) { return (w * TAIL_IDX_MUL) >> TAIL_IDX_SHIFT; }
+
+// nibble words (codes 0..3, padded with 0xF past K) -> ASCII words, bytes >= K zeroed
 template <int K>
 __device__ __forceinline__ void expand_ascii(const uint32_t (&c)[KmerShape<K>::NW], uint32_t (&a)[KmerShape<K>::NA], uint32_t POOL)
 {
@@ -336,6 +351,12 @@ __device__ __forceinline__ uint32_t lds_u32(uint32_t addr)
 {
     uint32_t v;
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint64_t lds_u64(uint32_t addr)
+{
+    uint64_t v;
+    asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(addr));
     return v;
 }
 
@@ -480,33 +501,65 @@ static __device__ __noinline__ void scan_sq_flush(const ScanArgs &a)
                                // buffer, 0 = into registers (as the FULL kernels do); tools/scan_microbench.cu compares them
 #endif
 
-// ASCII words of the canonical k-mer of window J of the block (b = forward words, rb = reverse-complement words)
-template <int K, bool CANON, int J>
-__device__ __forceinline__ void window_ascii(const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool,
-                                             uint32_t (&asc)[KmerShape<K>::NA])
+// Nibble words of the canonical k-mer of window J of the block (b = forward words, rb = reverse-complement words); the last
+// word of each strand becomes (w & LM) | LP before the compare
+template <int K, bool CANON, int J, uint32_t LM, uint32_t LP>
+__device__ __forceinline__ void window_words(const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
+                                             uint32_t (&c)[KmerShape<K>::NW])
 {
     using S = KmerShape<K>;
     uint32_t f[S::NW];
 #pragma unroll
     for (int i = 0; i < S::NW; i++) {
         f[i] = block_word<J, S::BW>(b, i);
-        if (i == S::NW - 1) f[i] = (f[i] & S::LAST_MASK) | S::LAST_PAD;
+        if (i == S::NW - 1) f[i] = (f[i] & LM) | LP;
     }
-    uint32_t c[S::NW];
     if (CANON) {
         constexpr int RO = 8 * S::BW - K - J;   // nibble offset of the reverse-complement window
         uint32_t r[S::NW];
 #pragma unroll
         for (int i = 0; i < S::NW; i++) {
             r[i] = block_word<RO, S::BW>(rb, i);
-            if (i == S::NW - 1) r[i] = (r[i] & S::LAST_MASK) | S::LAST_PAD;
+            if (i == S::NW - 1) r[i] = (r[i] & LM) | LP;
         }
         canonical_words<K>(f, r, c);
     } else {
 #pragma unroll
         for (int i = 0; i < S::NW; i++) c[i] = f[i];
     }
+}
+
+// ASCII words of the canonical k-mer of window J of the block
+template <int K, bool CANON, int J>
+__device__ __forceinline__ void window_ascii(const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool,
+                                             uint32_t (&asc)[KmerShape<K>::NA])
+{
+    using S = KmerShape<K>;
+    uint32_t c[S::NW];
+    window_words<K, CANON, J, S::LAST_MASK, S::LAST_PAD>(b, rb, c);
     expand_ascii<K>(c, asc, pool);
+}
+
+// Cost accounting (tools/scan_microbench.cu, DESIGN.md §2.4): SCAN_MB_EXTRA_FMA = n adds a chain of n dependent IMADs to
+// every window's filter word, SCAN_MB_EXTRA_ALU = n a chain of n dependent ALU instructions (LOP3 and IADD3 in turn: a
+// chain of LOP3 alone over fewer than four inputs would fold into one).  Their operands are kernel parameters, which ptxas
+// cannot fold, and the chain enters the word as `x | (y & preserve_case)`, which the microbenchmark leaves 0, so its
+// results do not change.  The slope of the kernel's time over n tells which pipe binds the hot loop.
+#ifndef SCAN_MB_EXTRA_FMA
+#define SCAN_MB_EXTRA_FMA 0
+#endif
+#ifndef SCAN_MB_EXTRA_ALU
+#define SCAN_MB_EXTRA_ALU 0
+#endif
+__device__ __forceinline__ uint32_t scan_mb_extra(const ScanArgs &a, uint32_t x)
+{
+    if (SCAN_MB_EXTRA_FMA == 0 && SCAN_MB_EXTRA_ALU == 0) return x;
+    uint32_t y = x;
+#pragma unroll
+    for (int i = 0; i < SCAN_MB_EXTRA_FMA; i++) y = y * (uint32_t)a.coarse_t + a.seed;
+#pragma unroll
+    for (int i = 0; i < SCAN_MB_EXTRA_ALU; i++) y = (i & 1) ? y + a.seed : y ^ (uint32_t)a.coarse_t;
+    return x | (y & (uint32_t)a.preserve_case);
 }
 
 // Full-hash fast path (k <= 16, and the screen's probing kernels: every lane probes the reference table with its own hash)
@@ -525,14 +578,33 @@ __device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&
 }
 
 // Filter-word fast path (k > 16): only murmur3_h1_filter's word, to be tested against filter_threshold(tmax >> 32)
+// (tail_tab: the CTA's tail table in shared memory, used when KmerShape<K>::TAIL_TABLE)
 template <int K, bool CANON, int J>
 __device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
-                                                       const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool)
+                                                       const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool, const uint64_t *tail_tab)
 {
     using S = KmerShape<K>;
-    uint32_t asc[S::NA];
-    window_ascii<K, CANON, J>(b, rb, pool, asc);
-    return murmur3_h1_filter<K, S::NA>(asc, a.seed);
+    uint32_t x;
+    if constexpr (S::TAIL_TABLE) {
+        // the last word keeps the two code bits of the tail's nibbles (both strands alike, so the compare is unchanged for
+        // windows in the alphabet); it becomes the table index instead of ASCII words
+        uint32_t c[S::NW], asc[S::NA - 2];
+        window_words<K, CANON, J, S::LAST_MASK & 0x33333333u, 0u>(b, rb, c);
+#pragma unroll
+        for (int i = 0; i < S::NW - 1; i++) {
+            asc[2 * i] = prmt(pool, 0, c[i]);
+            asc[2 * i + 1] = prmt(pool, 0, c[i] >> 16);
+        }
+        uint32_t at;   // base + 8 index as one IMAD: written in C, ptxas makes it a shift, a mask and an add
+        asm("mad.lo.u32 %0, %1, 8, %2;" : "=r"(at) : "r"(tail_index(c[S::NW - 1])), "r"((uint32_t)__cvta_generic_to_shared(tail_tab)));
+        const uint64_t k1 = lds_u64(at);
+        x = murmur3_h1_filter<K, S::NA - 2, true>(asc, a.seed, u64x2{(uint32_t)k1, (uint32_t)(k1 >> 32)});
+    } else {
+        uint32_t asc[S::NA];
+        window_ascii<K, CANON, J>(b, rb, pool, asc);
+        x = murmur3_h1_filter<K, S::NA>(asc, a.seed);
+    }
+    return scan_mb_extra(a, x);
 }
 
 // The 8 windows of a block hashed back to back (independent multiply chains that ptxas can interleave), their pass flags
@@ -540,9 +612,27 @@ __device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const 
 // the lane's pass mask, and the mask is resolved once per tile (scan_resolve).
 template <int K, bool CANON, int... J>
 __device__ __forceinline__ uint32_t scan_block_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
-                                                      uint32_t tf, uint32_t pool, std::integer_sequence<int, J...>)
+                                                      uint32_t tf, uint32_t pool, const uint64_t *tail_tab, std::integer_sequence<int, J...>)
 {
-    return (((scan_window_filter<K, CANON, J>(a, b, rb, pool) <= tf ? 1u : 0u) << (24 + J)) | ...);
+    return (((scan_window_filter<K, CANON, J>(a, b, rb, pool, tail_tab) <= tf ? 1u : 0u) << (24 + J)) | ...);
+}
+
+// Fill the CTA's tail table (KmerShape<K>::TAIL_TABLE): entry tail_index(w) = murmur3_tail_k1 of the ASCII bytes of bases
+// 16..K-1 whose codes w holds at bits 0, 4, .. (all 4^5 code words, the codes past K ignored).
+template <int K>
+__device__ __forceinline__ void fill_tail_table(uint64_t *tab)
+{
+    for (uint32_t v = threadIdx.x; v < TAIL_TAB_SIZE; v += blockDim.x) {
+        uint32_t w = 0;
+        uint64_t t = 0;
+#pragma unroll
+        for (int i = 0; i < 5; i++) {
+            const uint32_t code = (v >> (2 * i)) & 3u;
+            w |= code << (4 * i);
+            if (i < K - 16) t |= (uint64_t)((0x54474341u >> (8 * code)) & 0xFFu) << (8 * i);   // 'A' 'C' 'G' 'T'
+        }
+        tab[tail_index(w)] = murmur3_tail_k1(t);
+    }
 }
 
 // Full-hash variant of the group: G windows, one warp vote, then the survivors of each window serialised by scan_emit_warp.
@@ -609,12 +699,6 @@ __device__ __forceinline__ void cp_async_wait_all()
     asm volatile("cp.async.wait_all;" ::: "memory");
 }
 
-__device__ __forceinline__ uint64_t lds_u64(uint32_t addr)
-{
-    uint64_t v;
-    asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(addr));
-    return v;
-}
 __device__ __forceinline__ uint4 lds_u128(uint32_t addr)
 {
     uint4 v;
@@ -711,6 +795,12 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     __shared__ __align__(16) uint32_t smr_all[CANON ? SCAN_WARPS : 1][SCAN_WARP_WORDS];
     constexpr bool LAND = !FULL && SCAN_PREFETCH_SMEM;
     __shared__ __align__(16) uint4 land_all[LAND ? SCAN_WARPS : 1][LAND ? SCAN_WARP_VECS : 1];   // next tile's raw bytes
+    constexpr bool TAB = !FULL && S::TAIL_TABLE;
+    __shared__ __align__(16) uint64_t tail_tab[TAB ? TAIL_TAB_SIZE : 1];
+    if (TAB) {
+        fill_tail_table<K>(tail_tab);
+        __syncthreads();
+    }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t *sm = sm_all[warp];
     uint32_t *smr = smr_all[CANON ? warp : 0];
@@ -831,7 +921,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
             constexpr int G = SCAN_VOTE_GROUP;
             if constexpr (!FULL) {
                 // block i = (g - lane) / 32 ends at bits 8 i .. 8 i + 7 after the tile's 4 trips
-                pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, pool, std::make_integer_sequence<int, 8>());
+                pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, pool, tail_tab, std::make_integer_sequence<int, 8>());
             } else {
                 scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
                 if constexpr (G < 8) scan_group<K, CANON, (G < 8 ? G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
