@@ -173,7 +173,7 @@ int mashgpu_dist_open(mashgpu_ctx *ctx, const mashgpu_sketch_set *ref, const mas
 /* Compares queries [q_begin, q_begin+q_count) with every reference: pair (q, r) is written at index
  * (q - q_begin) * n_ref + r, the reference's query-major order (CommandDistance.cpp:213-232, 306-334).
  * Per pair (PairOutput, CommandDistance.h:63-70): numer (shared hashes), denom, distance, pvalue, pass.
- * Sketch sizes up to 1035 run the tiled lockstep merge (32 references per shared-memory tile); larger ones (`-s 10000`) a
+ * Sketch sizes up to 1034 run the tiled lockstep merge (32 references per shared-memory tile); larger ones (`-s 10000`) a
  * warp-per-pair merge; beyond ~28 000 hashes per sketch one thread per pair from global memory.
  * Where the reference leaves numer/denom/distance/pValue unset (distance > max_distance, :409-412) this
  * engine still writes the computed numer/denom/distance and pvalue = 0, with pass = 0.

@@ -63,10 +63,9 @@ struct DistArgs {
     unsigned long long *list_count; uint64_t list_capacity;
     // prefilter work lists (dist_probe_kernel -> dist_kernel): per reference tile the queries that share a hash with it
     uint32_t *qlist; uint32_t *qcount; uint64_t qlist_stride; unsigned long long *flag_total;
-    int use_qlist;              // dist_kernel: take the queries of a tile from qlist instead of the dense range
-    int probe_prefetch;         // dist_probe_kernel: request the query lines two groups ahead into L1
     int triangle;               // lower triangle only: pairs with tri_r0 + r >= q are neither computed nor written
     uint32_t tri_r0;            // row of reference 0 in the query numbering (0 for a self comparison; the shard offset of an encoded job)
+    int use_qlist;              // dist_kernel: take the queries of a tile from qlist instead of the dense range
     // sparse related pairs (dist_probe_kernel -> dist_pair_kernel): when a query may share hashes with at most pair_max references
     // of a tile, only those (query, reference) pairs are merged, one warp per pair, instead of all 32 in lockstep
     uint2 *pair_list; unsigned long long *pair_count; uint64_t pair_capacity; unsigned long long *pair_total;
@@ -160,20 +159,25 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
     }
 }
 
-// BULK: the query rows are staged by the TMA engine (cp.async.bulk global -> shared, completion on a per-warp mbarrier) instead
-// of a coalesced LDG/STS loop.  A row of P ranks starts at a 4-byte aligned address (pitch P words), the bulk copy needs 16:
-// the copy covers the 16-byte aligned span around the row and the merge starts `skew` bytes into the warp's buffer.
-// MASHGPU_DIST_BULK=0 selects the load loop for an A/B; the staging is ~2.5 % of the kernel's instructions.
-__device__ __forceinline__ uint32_t dist_qpitch(uint32_t P, bool bulk) { return bulk ? ((P + 4u + 3u) & ~3u) : P; }
+// The query rows are staged by the TMA engine (cp.async.bulk global -> shared, completion on a per-warp mbarrier).  A row of
+// P ranks starts at a 4-byte aligned address (pitch P words), the bulk copy needs 16: the copy covers the 16-byte aligned
+// span around the row and the merge starts `skew` bytes into the warp's buffer.
+__host__ __device__ __forceinline__ uint32_t dist_qpitch(uint32_t P) { return (P + 4u + 3u) & ~3u; }
 
-template <bool BULK>
+// Dynamic shared memory of dist_kernel for rows of P ranks: the reference tile, the query buffers and the mbarriers.  Sketch
+// sizes for which it exceeds 227 KB are not tiled.
+inline size_t dist_smem_bytes(uint32_t P)
+{
+    return ((((size_t)P * DIST_TILE_R + 3) & ~(size_t)3) + (size_t)DIST_WARPS * DIST_ILP * dist_qpitch(P)) * 4 + DIST_WARPS * 8;
+}
+
 __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
 {
     extern __shared__ __align__(16) uint32_t smem[];
-    const uint32_t qpitch = dist_qpitch(a.P, BULK);
+    const uint32_t qpitch = dist_qpitch(a.P);
     uint32_t *s_ref = smem;                                  // [P][32]
     uint32_t *s_qry = smem + (((size_t)a.P * DIST_TILE_R + 3) & ~(size_t)3);      // [DIST_WARPS][DIST_ILP][qpitch]
-    uint64_t *s_bar = reinterpret_cast<uint64_t *>(s_qry + (size_t)DIST_WARPS * DIST_ILP * qpitch);     // BULK: one mbarrier per warp
+    uint64_t *s_bar = reinterpret_cast<uint64_t *>(s_qry + (size_t)DIST_WARPS * DIST_ILP * qpitch);     // one mbarrier per warp
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t r0 = blockIdx.x * DIST_TILE_R;
     const uint32_t r = r0 + lane;
@@ -197,11 +201,9 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
     uint32_t *my_q = s_qry + (size_t)warp * DIST_ILP * qpitch;
     const uint32_t bar = (uint32_t)__cvta_generic_to_shared(s_bar + warp);
     uint32_t phase = 0;
-    if (BULK) {
-        if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        __syncwarp();
-    }
+    if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    __syncwarp();
 
     for (uint64_t it_lo = (uint64_t)blockIdx.y * a.q_per_cta; it_lo < n_items; it_lo += (uint64_t)gridDim.y * a.q_per_cta) {
     const uint32_t it_hi = (uint32_t)min((uint64_t)n_items, it_lo + a.q_per_cta);
@@ -216,54 +218,38 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
             all_skipped &= qs[c] == 0xFFFFFFFFu;
         }
         if (all_skipped) continue;                      // warp-uniform
-        // load DIST_ILP query rows into this warp's buffers: coalesced LDG/STS, or (BULK) one bulk copy per row
-        uint32_t skew[DIST_ILP];
+        // load DIST_ILP query rows into this warp's buffers, one bulk copy per row
+        uint32_t skew[DIST_ILP], bytes[DIST_ILP], total = 0;
+        const uint32_t *src[DIST_ILP];
 #pragma unroll
-        for (int c = 0; c < DIST_ILP; c++) skew[c] = 0;
-        if (BULK) {
-            uint32_t bytes[DIST_ILP], total = 0;
-            const uint32_t *src[DIST_ILP];
-#pragma unroll
-            for (int c = 0; c < DIST_ILP; c++) {
-                bytes[c] = 0; src[c] = nullptr;
-                if (qs[c] != 0xFFFFFFFFu) {
-                    const uintptr_t row = (uintptr_t)(a.ranks + (a.qry_row0 + qs[c]) * (uint64_t)a.P);
-                    const uintptr_t lo = row & ~(uintptr_t)15, hi = (row + (uintptr_t)a.P * 4 + 15) & ~(uintptr_t)15;
-                    skew[c] = (uint32_t)(row - lo);
-                    src[c] = reinterpret_cast<const uint32_t *>(lo);
-                    bytes[c] = (uint32_t)(hi - lo);
-                    total += bytes[c];
-                } else {
-                    uint32_t *dst = my_q + (size_t)c * qpitch;
-                    for (uint32_t i = lane; i < a.P; i += 32) dst[i] = RANK_PAD;
-                }
-            }
-            __syncwarp();
-            if (lane == 0 && total) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // the lanes' reads of the previous rows precede the async writes
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(total) : "memory");
-#pragma unroll
-                for (int c = 0; c < DIST_ILP; c++)
-                    if (bytes[c])
-                        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                     :: "r"((uint32_t)__cvta_generic_to_shared(my_q + (size_t)c * qpitch)), "l"(src[c]), "r"(bytes[c]), "r"(bar) : "memory");
-            }
-            if (total) {
-                asm volatile("{\n\t.reg .pred p;\n\tDIST_BULK_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra DIST_BULK_WAIT;\n\t}"
-                             :: "r"(bar), "r"(phase) : "memory");
-                phase ^= 1;
-            }
-        } else {
-#pragma unroll
-            for (int c = 0; c < DIST_ILP; c++) {
+        for (int c = 0; c < DIST_ILP; c++) {
+            skew[c] = 0; bytes[c] = 0; src[c] = nullptr;
+            if (qs[c] != 0xFFFFFFFFu) {
+                const uintptr_t row = (uintptr_t)(a.ranks + (a.qry_row0 + qs[c]) * (uint64_t)a.P);
+                const uintptr_t lo = row & ~(uintptr_t)15, hi = (row + (uintptr_t)a.P * 4 + 15) & ~(uintptr_t)15;
+                skew[c] = (uint32_t)(row - lo);
+                src[c] = reinterpret_cast<const uint32_t *>(lo);
+                bytes[c] = (uint32_t)(hi - lo);
+                total += bytes[c];
+            } else {
                 uint32_t *dst = my_q + (size_t)c * qpitch;
-                if (qs[c] != 0xFFFFFFFFu) {
-                    const uint32_t *row = a.ranks + (a.qry_row0 + qs[c]) * (uint64_t)a.P;
-                    for (uint32_t i = lane; i < a.P; i += 32) dst[i] = row[i];
-                } else {
-                    for (uint32_t i = lane; i < a.P; i += 32) dst[i] = RANK_PAD;
-                }
+                for (uint32_t i = lane; i < a.P; i += 32) dst[i] = RANK_PAD;
             }
+        }
+        __syncwarp();
+        if (lane == 0 && total) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // the lanes' reads of the previous rows precede the async writes
+            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(total) : "memory");
+#pragma unroll
+            for (int c = 0; c < DIST_ILP; c++)
+                if (bytes[c])
+                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                                 :: "r"((uint32_t)__cvta_generic_to_shared(my_q + (size_t)c * qpitch)), "l"(src[c]), "r"(bytes[c]), "r"(bar) : "memory");
+        }
+        if (total) {
+            asm volatile("{\n\t.reg .pred p;\n\tDIST_BULK_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra DIST_BULK_WAIT;\n\t}"
+                         :: "r"(bar), "r"(phase) : "memory");
+            phase ^= 1;
         }
         __syncwarp();
         uint32_t pa[DIST_ILP], pb[DIST_ILP], va[DIST_ILP], vb[DIST_ILP], pb0[DIST_ILP];
@@ -374,7 +360,7 @@ __device__ __noinline__ uint2 probe_resolve(uint32_t b0, uint32_t b1, uint32_t b
 
 // One group of PROBE_DEPTH x 32 ranks of a query against the filter.  FULL: the whole group lies inside the query's list.
 // Returns true when some lane has a fingerprint match.
-template <bool FULL, bool LAZY>
+template <bool FULL>
 __device__ __forceinline__ bool probe_group(uint32_t tab_s, const uint32_t (&b)[PROBE_DEPTH], uint32_t base, uint32_t nB, int lane)
 {
     // b[c] = rank base + 32 c + lane of the query (RANK_PAD past the end of its list)
@@ -382,13 +368,12 @@ __device__ __forceinline__ bool probe_group(uint32_t tab_s, const uint32_t (&b)[
     CfProbe pr[PROBE_DEPTH];
 #pragma unroll
     for (int c = 0; c < PROBE_DEPTH; c++) {
-        pr[c] = cf_fetch_s<LAZY>(tab_s, b[c]);
+        pr[c] = cf_fetch_s(tab_s, b[c]);
         if (!FULL && base + 32 * c + lane >= nB) pr[c].f2 = 0x7E007E00u;       // past the end of the list: never matches
     }
     return cf_group_any(pr[0], pr[1], pr[2], pr[3]);
 }
 
-template <bool LAZY>
 __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const DistArgs a)
 {
     extern __shared__ uint32_t s_tab[];                      // CF_BUCKETS words, then 2 * CF_BUCKETS id bytes
@@ -469,12 +454,12 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
         uint32_t cur[PROBE_DEPTH];
         // (two groups per iteration -- 8 lookups in flight per lane, one vote per 256 ranks -- was slower: the loop is bound by
         // ALU-pipe and shared-memory throughput, not by latency)
-        if (a.probe_prefetch && 2 * GROUP <= nB) asm volatile("prefetch.global.L1 [%0];" :: "l"(rowB + GROUP + 32 * (lane & 3)));
+        if (2 * GROUP <= nB) asm volatile("prefetch.global.L1 [%0];" :: "l"(rowB + GROUP + 32 * (lane & 3)));
         while (base + GROUP <= nB && !dense) {
-            if (a.probe_prefetch && base + 3 * GROUP <= nB) asm volatile("prefetch.global.L1 [%0];" :: "l"(rowB + base + 2 * GROUP + 32 * (lane & 3)));
+            if (base + 3 * GROUP <= nB) asm volatile("prefetch.global.L1 [%0];" :: "l"(rowB + base + 2 * GROUP + 32 * (lane & 3)));
 #pragma unroll
             for (int c = 0; c < PROBE_DEPTH; c++) cur[c] = __ldg(pB + 32 * c);
-            if (probe_group<true, LAZY>(tab_s, cur, base, nB, lane)) {
+            if (probe_group<true>(tab_s, cur, base, nB, lane)) {
                 const uint2 st = probe_resolve<true>(cur[0], cur[1], cur[2], cur[3], base, nB, rowA, nA_lim, mask, a.pair_max, confirms);
                 mask = st.x; confirms = (int)st.y;
                 if (__popc(mask) > a.pair_max) { dense = true; break; }
@@ -487,7 +472,7 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
         if (base < nB && !dense) {      // ragged last group
 #pragma unroll
             for (int c = 0; c < PROBE_DEPTH; c++) cur[c] = (base + 32 * c + lane < nB) ? __ldg(pB + 32 * c) : RANK_PAD;
-            if (probe_group<false, LAZY>(tab_s, cur, base, nB, lane)) {
+            if (probe_group<false>(tab_s, cur, base, nB, lane)) {
                 const uint2 st = probe_resolve<false>(cur[0], cur[1], cur[2], cur[3], base, nB, rowA, nA_lim, mask, pair_max, confirms);
                 mask = st.x;
                 dense = __popc(mask) > pair_max;
@@ -828,12 +813,7 @@ struct mashgpu_dist_job {
     // prefilter (dist_probe_kernel): -1 = auto (on; switched off when most combinations turn out to share hashes), 0 = off, 1 = on
     int prefilter_mode = -1;
     bool triangle = false;
-    bool probe_prefetch = true;         // MASHGPU_PROBE_PREFETCH=0 to compare
-    bool lazy_second = false;           // probe kernel: load the second bucket only where the first one is full (MASHGPU_CF_LAZY=1).
-                                        // Off by default: the predicate logic costs more than the LDS wavefronts it saves
     bool auto_off = false;
-    bool bulk_rows = true;              // dist_kernel: stage the query rows with cp.async.bulk (TMA engine) so that the row load does not sit
-                                        // in front of every merge; MASHGPU_DIST_BULK=0 = coalesced load loop
     DevBuf<uint32_t> qlist, qcount;
     DevBuf<uint2> pair_list;            // sparse related pairs of the run in flight (dist_probe_kernel -> dist_pair_kernel)
     DevBuf<unsigned long long> pair_count;      // [0] pairs listed by the run in flight, [1] pairs merged from lists since the job was opened
@@ -971,22 +951,16 @@ int dist_job_tables(mashgpu_ctx *ctx, mashgpu_dist_job *job, cudaStream_t st)
     MG_CUDA(ctx, cudaMemcpyAsync(job->binom_e.p, be.data(), (S + 1) * 4, cudaMemcpyHostToDevice, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));      // the host vectors go out of scope
     if (!ctx->attr_dist) {   // per context: function attributes are per device
-        cudaError_t e = cudaFuncSetAttribute(dist_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(dist_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-        if (e != cudaSuccess) return fail(ctx, MASHGPU_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-        e = cudaFuncSetAttribute(dist_probe_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROBE_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(dist_probe_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROBE_SMEM);
+        cudaError_t e = cudaFuncSetAttribute(dist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(dist_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROBE_SMEM);
         if (e == cudaSuccess) e = cudaFuncSetAttribute(dist_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
         if (e != cudaSuccess) return fail(ctx, MASHGPU_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
         ctx->attr_dist = true;
     }
     if (const char *env = getenv("MASHGPU_DIST_PAIR_MAX")) job->pair_max = std::max(0, std::min(31, atoi(env)));
-    if (const char *env = getenv("MASHGPU_CF_LAZY")) job->lazy_second = atoi(env) != 0;
-    if (const char *env = getenv("MASHGPU_PROBE_PREFETCH")) job->probe_prefetch = atoi(env) != 0;
     if (const char *env = getenv("MASHGPU_DIST_PREFILTER")) job->prefilter_mode = atoi(env) > 0 ? 1 : (atoi(env) == 0 ? 0 : -1);
-    // shared memory needed by the merge kernel; larger sketches run dist_kernel_general
-    job->tiled = ((((size_t)job->P * DIST_TILE_R + 3) & ~(size_t)3) + (size_t)DIST_WARPS * DIST_ILP * job->P) * 4 + DIST_WARPS * 8 <= 227 * 1024;
-    if (const char *env = getenv("MASHGPU_DIST_BULK")) job->bulk_rows = atoi(env) != 0;
+    // s <= 1034: the tiled merge (dist_kernel); larger sketches run the warp-per-pair merge or dist_kernel_general
+    job->tiled = dist_smem_bytes(job->P) <= 227 * 1024;
     return MASHGPU_OK;
 }
 
@@ -1279,7 +1253,6 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     a.triangle = job->triangle ? 1 : 0;
     a.tri_r0 = job->self ? 0u : (uint32_t)job->ref_row0;
     a.pair_list = nullptr; a.pair_count = nullptr; a.pair_capacity = 0; a.pair_total = nullptr; a.pair_max = 0; a.pair_dense = 0;
-    a.probe_prefetch = job->probe_prefetch ? 1 : 0;
     {   // queue for the deferred p-values: 1/16 of the pairs (at least 2^20); beyond that dist_emit evaluates in place
         const uint64_t pairs = q_count * job->n_ref;
         const uint64_t cap = std::min<uint64_t>(pairs, std::max<uint64_t>(1ull << 20, pairs / 16));
@@ -1305,7 +1278,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
         return cudaGetLastError();
     };
     if (!job->tiled && pair_warps >= 1) {
-        // sketch sizes whose 32-reference tile does not fit shared memory (s > 1035, e.g. `-s 10000`): every pair by the warp-per-pair merge
+        // sketch sizes whose 32-reference tile does not fit shared memory (s >= 1035, e.g. `-s 10000`): every pair by the warp-per-pair merge
         a.pair_dense = 1;
         time_begin(ctx, ctx->dist_events, st);
         MG_CUDA(ctx, launch_pairs());
@@ -1327,10 +1300,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     }
     const uint32_t r_tiles = (uint32_t)((job->n_ref + DIST_TILE_R - 1) / DIST_TILE_R);
     const uint32_t round = DIST_WARPS * DIST_ILP;
-    // query rows by TMA bulk copy (MASHGPU_DIST_BULK=1) when the padded buffers still fit; default: coalesced loads
-    const size_t smem_bulk = ((((size_t)a.P * DIST_TILE_R + 3) & ~(size_t)3) + (size_t)DIST_WARPS * DIST_ILP * (((size_t)a.P + 7) & ~(size_t)3)) * 4 + DIST_WARPS * 8;
-    const bool bulk = job->bulk_rows && smem_bulk <= 227 * 1024;
-    const size_t smem = bulk ? smem_bulk : ((((size_t)a.P * DIST_TILE_R + 3) & ~(size_t)3) + (size_t)DIST_WARPS * DIST_ILP * a.P) * 4 + DIST_WARPS * 8;
+    const size_t smem = dist_smem_bytes(a.P);
     a.qlist = nullptr; a.qcount = nullptr; a.qlist_stride = 0; a.flag_total = nullptr; a.use_qlist = 0;
     dist_collect_flags(job);
     const bool prefilter = job->prefilter_mode > 0 || (job->prefilter_mode < 0 && !job->auto_off);
@@ -1368,8 +1338,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
         time_begin(ctx, ctx->dist_events, st);
         // without the pair path the kernel keeps 128 KB of shared memory and twice the L1 (query rows stream through L1)
         const size_t probe_smem = a.pair_max > 0 ? PROBE_SMEM : CF_BUCKETS * sizeof(uint32_t);
-        if (job->lazy_second) dist_probe_kernel<true><<<dim3(r_tiles, p_slices), PROBE_THREADS, probe_smem, st>>>(a);
-        else dist_probe_kernel<false><<<dim3(r_tiles, p_slices), PROBE_THREADS, probe_smem, st>>>(a);
+        dist_probe_kernel<<<dim3(r_tiles, p_slices), PROBE_THREADS, probe_smem, st>>>(a);
         time_end(ctx, ctx->dist_events, st);
         MG_CUDA(ctx, cudaGetLastError());
         // merge the listed combinations: a few CTAs per tile walk its list (CTAs of tiles with short lists exit at once)
@@ -1377,8 +1346,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
         a.q_per_cta = 2 * round;
         const uint32_t m_slices = (uint32_t)std::min<uint64_t>(8, (q_count + a.q_per_cta - 1) / a.q_per_cta);
         time_begin(ctx, ctx->dist_events, st);
-        if (bulk) dist_kernel<true><<<dim3(r_tiles, m_slices), DIST_THREADS, smem, st>>>(a);
-        else dist_kernel<false><<<dim3(r_tiles, m_slices), DIST_THREADS, smem, st>>>(a);
+        dist_kernel<<<dim3(r_tiles, m_slices), DIST_THREADS, smem, st>>>(a);
         MG_CUDA(ctx, cudaGetLastError());
         if (a.pair_list) MG_CUDA(ctx, launch_pairs());
         MG_CUDA(ctx, launch_fix());
@@ -1402,8 +1370,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     a.q_per_cta = q_per_cta;
     dim3 grid(r_tiles, slices);
     time_begin(ctx, ctx->dist_events, st);
-    if (bulk) dist_kernel<true><<<grid, DIST_THREADS, smem, st>>>(a);
-    else dist_kernel<false><<<grid, DIST_THREADS, smem, st>>>(a);
+    dist_kernel<<<grid, DIST_THREADS, smem, st>>>(a);
     MG_CUDA(ctx, cudaGetLastError());
     MG_CUDA(ctx, launch_fix());
     time_end(ctx, ctx->dist_events, st);

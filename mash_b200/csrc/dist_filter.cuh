@@ -206,32 +206,16 @@ MG_HD CfProbe cf_fetch(const uint32_t *tab, uint32_t code)
 
 #if defined(__CUDACC__)
 
-// Device form of the probe: `tab_s` is the 32-bit shared-memory address of the table.  The second bucket is loaded only by
-// the lanes that need it: buckets fill up monotonically and an insert takes the first bucket whenever it has a free slot
-// (cf_insert tries it first; evictions only ever happen out of full buckets and leave them full), so a rank whose first
-// bucket still has a free slot is either in that bucket or not in the table.  About a quarter of the buckets are full at
-// the tile's load, so the second LDS runs with a quarter of the lanes -- 1.3 instead of 3.5 bank-conflict wavefronts
-// LAZY = false loads both buckets unconditionally; that was faster (the extra predicate logic sits on the ALU pipe), so it
-// is the default.
-template <bool LAZY>
+// Device form of the probe: `tab_s` is the 32-bit shared-memory address of the table.  Both buckets are loaded by every lane,
+// because loading the second only where the first is full costs more ALU-pipe predicate logic than the shared-memory
+// wavefronts it saves.
 __device__ __forceinline__ CfProbe cf_fetch_s(uint32_t tab_s, uint32_t code)
 {
     uint32_t o1, o2;
     CfProbe r;
     cf_offsets(code, o1, o2, r.f2);
-    if (!LAZY) {
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.w1) : "r"(tab_s + o1));
-        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.w2) : "r"(tab_s + o2));
-        return r;
-    }
-    asm volatile("{\n\t.reg .pred a, b, c, d;\n\t"
-                 "ld.shared.u32 %0, [%2];\n\t"
-                 "mov.u32 %1, 0;\n\t"
-                 "setp.eq.f16x2 a|b, %0, %4;\n\t"          // fingerprint already found in bucket 1
-                 "setp.eq.f16x2 c|d, %0, %5;\n\t"          // a free slot (+0.0) in bucket 1
-                 "or.pred a, a, b;\n\tor.pred c, c, d;\n\tor.pred a, a, c;\n\t"
-                 "@!a ld.shared.u32 %1, [%3];\n\t}"
-                 : "=&r"(r.w1), "=&r"(r.w2) : "r"(tab_s + o1), "r"(tab_s + o2), "r"(r.f2), "r"(0u));
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.w1) : "r"(tab_s + o1));
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r.w2) : "r"(tab_s + o2));
     return r;
 }
 

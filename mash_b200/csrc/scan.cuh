@@ -420,12 +420,10 @@ __shared__ uint32_t scan_sq_n[SCAN_WARPS];   // entries appended since the last 
 // Slow path of the filter-word kernels, once per warp tile that has a survivor.  A lane's pass mask covers its 32 windows of
 // the tile: bit 8 i + j = window j of the lane's block i (window start 8 (lane + 32 i) + j) passed the fast-path filter.  The
 // lanes walk their set bits together (a lane with none left idles), rebuild the exact hash of each passing window from the
-// tile, and queue the valid ones at or below the tile threshold for their table work.
-#ifndef SCAN_RESOLVE_INLINE
-#define SCAN_RESOLVE_INLINE 0   // 1: inline the per-tile resolution into scan_kernel (tools/scan_microbench.cu compares both)
-#endif
+// tile, and queue the valid ones at or below the tile threshold for their table work.  Out of line: inlined into scan_kernel
+// it measured slower (DESIGN.md §2.4).
 template <int K, bool CANON>
-static __device__ __forceinline__ void scan_resolve_body(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
+static __device__ __noinline__ void scan_resolve(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
 {
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     while (__any_sync(0xFFFFFFFFu, pm != 0)) {
@@ -445,17 +443,6 @@ static __device__ __forceinline__ void scan_resolve_body(const ScanArgs &a, uint
             }
         }
     }
-}
-template <int K, bool CANON>
-static __device__ __noinline__ void scan_resolve_call(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
-{
-    scan_resolve_body<K, CANON>(a, pm, sm_addr, tile_base, tmax);
-}
-template <int K, bool CANON>
-__device__ __forceinline__ void scan_resolve(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
-{
-    if (SCAN_RESOLVE_INLINE) scan_resolve_body<K, CANON>(a, pm, sm_addr, tile_base, tmax);
-    else scan_resolve_call<K, CANON>(a, pm, sm_addr, tile_base, tmax);
 }
 
 // Table work of the queued survivors of this warp, one per lane; warp-uniform call, leaves the queue empty
@@ -490,15 +477,6 @@ static __device__ __noinline__ void scan_sq_flush(const ScanArgs &a)
 #endif
 #ifndef SCAN_MB_CLOCK
 #define SCAN_MB_CLOCK 0
-#endif
-#ifndef SCAN_VOTE_GROUP
-#define SCAN_VOTE_GROUP 2      // FULL kernels only: windows hashed back to back before one warp vote (1, 2, 4 or 8); see
-                               // scan_group.  The filter-word kernels do not vote in the hot loop (per-lane pass masks,
-                               // resolved once per tile).  On H100 2 beat 4 and 8 (filter-word kernel, before the masks)
-#endif
-#ifndef SCAN_PREFETCH_SMEM
-#define SCAN_PREFETCH_SMEM 1   // filter-word kernels: 1 = the next tile is prefetched by cp.async into a per-warp shared landing
-                               // buffer, 0 = into registers (as the FULL kernels do); tools/scan_microbench.cu compares them
 #endif
 
 // Nibble words of the canonical k-mer of window J of the block (b = forward words, rb = reverse-complement words); the last
@@ -635,32 +613,19 @@ __device__ __forceinline__ void fill_tail_table(uint64_t *tab)
     }
 }
 
-// Full-hash variant of the group: G windows, one warp vote, then the survivors of each window serialised by scan_emit_warp.
-template <int K, bool CANON, int J0, int G>
+// Full-hash variant: windows J0 and J0 + 1 hashed back to back, one warp vote, then the survivors of each window serialised by
+// scan_emit_warp.  Two windows per vote beat four and eight on H100 (measured on the filter-word kernel before its pass masks,
+// DESIGN.md §2.4).
+template <int K, bool CANON, int J0>
 __device__ __forceinline__ void scan_group(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
                                            uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t pool, const uint32_t *sm_tile)
 {
-    u64x2 h[G];
-    bool pass[G];
-    bool any = false;
-    pass[0] = scan_window<K, CANON, J0>(a, b, rb, tmax, pool, h[0]);
-    if constexpr (G > 1) pass[1] = scan_window<K, CANON, J0 + (G > 1 ? 1 : 0)>(a, b, rb, tmax, pool, h[G > 1 ? 1 : 0]);
-    if constexpr (G > 2) {
-        pass[2] = scan_window<K, CANON, J0 + (G > 2 ? 2 : 0)>(a, b, rb, tmax, pool, h[G > 2 ? 2 : 0]);
-        pass[3] = scan_window<K, CANON, J0 + (G > 2 ? 3 : 0)>(a, b, rb, tmax, pool, h[G > 2 ? 3 : 0]);
-    }
-    if constexpr (G > 4) {
-        pass[4] = scan_window<K, CANON, J0 + (G > 4 ? 4 : 0)>(a, b, rb, tmax, pool, h[G > 4 ? 4 : 0]);
-        pass[5] = scan_window<K, CANON, J0 + (G > 4 ? 5 : 0)>(a, b, rb, tmax, pool, h[G > 4 ? 5 : 0]);
-        pass[6] = scan_window<K, CANON, J0 + (G > 4 ? 6 : 0)>(a, b, rb, tmax, pool, h[G > 4 ? 6 : 0]);
-        pass[7] = scan_window<K, CANON, J0 + (G > 4 ? 7 : 0)>(a, b, rb, tmax, pool, h[G > 4 ? 7 : 0]);
-    }
-#pragma unroll
-    for (int j = 0; j < G; j++) any |= pass[j];
-    if (__any_sync(0xFFFFFFFFu, any)) {
-#pragma unroll
-        for (int j = 0; j < G; j++)
-            if (__any_sync(0xFFFFFFFFu, pass[j])) scan_emit_warp(a, pass[j], h[j].lo, h[j].hi, tile_base, local0 + J0 + j, sm_tile, K, tmax);
+    u64x2 h0, h1;
+    const bool p0 = scan_window<K, CANON, J0>(a, b, rb, tmax, pool, h0);
+    const bool p1 = scan_window<K, CANON, J0 + 1>(a, b, rb, tmax, pool, h1);
+    if (__any_sync(0xFFFFFFFFu, p0 | p1)) {
+        if (__any_sync(0xFFFFFFFFu, p0)) scan_emit_warp(a, p0, h0.lo, h0.hi, tile_base, local0 + J0, sm_tile, K, tmax);
+        if (__any_sync(0xFFFFFFFFu, p1)) scan_emit_warp(a, p1, h1.lo, h1.hi, tile_base, local0 + J0 + 1, sm_tile, K, tmax);
     }
 }
 
@@ -771,8 +736,7 @@ __device__ __forceinline__ uint4 expand32(uint64_t c, uint32_t m)
 // Warp-private tiles: every warp owns WARP_TILE window starts at a time, staged in its own slice of shared memory,
 // so the only synchronisation is __syncwarp().  The next tile's bytes are prefetched before the current tile is hashed
 // (global latency hidden behind ~4000 instructions of work per lane): by the FULL kernels into registers, by the
-// filter-word kernels into a per-warp shared landing buffer (SCAN_PREFETCH_SMEM), which keeps those registers free
-// through the hot loop.
+// filter-word kernels into a per-warp shared landing buffer, which keeps those registers free through the hot loop.
 #ifndef SCAN_MIN_BLOCKS
 #define SCAN_MIN_BLOCKS 4      // filter-word kernels: resident CTAs per SM requested from ptxas (4 => 64 registers, no spills
                                // since the hot loop holds neither a survivor call nor prefetch registers; 3 => 80 registers, 1 %
@@ -793,8 +757,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     // reverse-complement image of the tile (word i = nibble-reversed, complemented word NW-1-i), written once at staging so
     // that a block's reverse-complement words are 4 more LDS (the LSU is idle) instead of ~16 ALU instructions per block
     __shared__ __align__(16) uint32_t smr_all[CANON ? SCAN_WARPS : 1][SCAN_WARP_WORDS];
-    constexpr bool LAND = !FULL && SCAN_PREFETCH_SMEM;
-    __shared__ __align__(16) uint4 land_all[LAND ? SCAN_WARPS : 1][LAND ? SCAN_WARP_VECS : 1];   // next tile's raw bytes
+    __shared__ __align__(16) uint4 land_all[FULL ? 1 : SCAN_WARPS][FULL ? 1 : SCAN_WARP_VECS];   // next tile's raw bytes
     constexpr bool TAB = !FULL && S::TAIL_TABLE;
     __shared__ __align__(16) uint64_t tail_tab[TAB ? TAIL_TAB_SIZE : 1];
     if (TAB) {
@@ -809,7 +772,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     // iteration of the hot loop to save a register
     const uint32_t sm_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(sm), 0);
     const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(smr), 0);
-    const uint32_t land = (uint32_t)__cvta_generic_to_shared(land_all[LAND ? warp : 0]);
+    const uint32_t land = (uint32_t)__cvta_generic_to_shared(land_all[FULL ? 0 : warp]);
     const uint32_t fold = a.preserve_case ? 0xFFFFFFFFu : 0xDFDFDFDFu;
     uint32_t pool;   // bytes 'A','C','G','T' for PRMT; opaque to the compiler so that it stays in one register
     asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
@@ -828,7 +791,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     uint64_t pc0 = 0, pc1 = 0;             // packed source: group (lane) and one of the 2 halo groups (32 + lane%2)
     uint32_t pm0 = 0, pm1 = 0;
     const int hg = 32 + (lane & 1);
-    if (LAND) {
+    if constexpr (!FULL) {
         scan_prefetch_land<PACKED>(a, wt, land, lane);
     } else if (PACKED) {
         const uint64_t g0 = wt * (uint64_t)(SCAN_WARP_TILE / 32);
@@ -849,7 +812,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     const uint64_t wt_first = wt;
     for (; wt < wt_end; wt += wt_stride) {
         const uint64_t base = wt * (uint64_t)SCAN_WARP_TILE;
-        if (LAND && !(SCAN_MB_STAGE_ONCE && wt != wt_first)) {   // this tile's bytes, copied in during the previous tile
+        if (!FULL && !(SCAN_MB_STAGE_ONCE && wt != wt_first)) {   // this tile's bytes, copied in during the previous tile
             cp_async_wait_all();
             __syncwarp();
             if (PACKED) {
@@ -889,7 +852,7 @@ scan_kernel(const __grid_constant__ ScanArgs a)
         __syncwarp();
         const uint64_t next = wt + wt_stride;
         if (!SCAN_MB_STAGE_ONCE && next < wt_end) {   // prefetch
-            if (LAND) {
+            if constexpr (!FULL) {
                 scan_prefetch_land<PACKED>(a, next, land, lane);
             } else if (PACKED) {
                 const uint64_t g0 = next * (uint64_t)(SCAN_WARP_TILE / 32);
@@ -918,23 +881,14 @@ scan_kernel(const __grid_constant__ ScanArgs a)
                 for (int i = 0; i < S::BW; i++) rb[i] = lds_u32(smr_addr + 4u * (SCAN_WARP_WORDS - S::BW - g + i));
             }
             const uint32_t local0 = 8u * g;
-            constexpr int G = SCAN_VOTE_GROUP;
             if constexpr (!FULL) {
                 // block i = (g - lane) / 32 ends at bits 8 i .. 8 i + 7 after the tile's 4 trips
                 pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, pool, tail_tab, std::make_integer_sequence<int, 8>());
             } else {
-                scan_group<K, CANON, 0, G>(a, b, rb, base, local0, tmax, pool, sm);
-                if constexpr (G < 8) scan_group<K, CANON, (G < 8 ? G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-                if constexpr (G < 4) {
-                    scan_group<K, CANON, (G < 4 ? 2 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-                    scan_group<K, CANON, (G < 4 ? 3 * G : 0), G>(a, b, rb, base, local0, tmax, pool, sm);
-                }
-                if constexpr (G < 2) {
-                    scan_group<K, CANON, 4, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                    scan_group<K, CANON, 5, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                    scan_group<K, CANON, 6, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                    scan_group<K, CANON, 7, 1>(a, b, rb, base, local0, tmax, pool, sm);
-                }
+                scan_group<K, CANON, 0>(a, b, rb, base, local0, tmax, pool, sm);
+                scan_group<K, CANON, 2>(a, b, rb, base, local0, tmax, pool, sm);
+                scan_group<K, CANON, 4>(a, b, rb, base, local0, tmax, pool, sm);
+                scan_group<K, CANON, 6>(a, b, rb, base, local0, tmax, pool, sm);
             }
         }
         if (SCAN_MB_CLOCK) mb_cycles += clock64() - c0;

@@ -216,12 +216,11 @@ def test_pass_list_equals_dense_filter(gpu, oracle):
         assert np.array_equal(np.flatnonzero(want["pass"].ravel()), flat)
 
 
-def test_bulk_copy_staging_variant(gpu, oracle, monkeypatch):
-    # MASHGPU_DIST_BULK=1: dist_kernel stages the query rows with cp.async.bulk (TMA engine, mbarrier completion) instead of the
-    # coalesced load loop -- rows start at 4-byte aligned addresses, so the copy covers the 16-byte aligned span and the merge
-    # starts `skew` bytes in.  Same results for every row alignment (P odd and even, ragged rows, query ranges).
-    monkeypatch.setenv("MASHGPU_DIST_BULK", "1")
-    for s, nq in ((1000, 61), (999, 40), (37, 70), (1020, 33)):
+def test_query_row_staging_at_every_row_alignment(gpu, oracle):
+    # dist_kernel stages the query rows with cp.async.bulk (TMA engine, mbarrier completion): rows start at 4-byte aligned
+    # addresses, so the copy covers the 16-byte aligned span and the merge starts `skew` bytes in.  Same results for every row
+    # alignment (P odd and even, ragged rows, query ranges), up to s = 1034, the largest sketch size of the tiled merge.
+    for s, nq in ((1000, 61), (999, 40), (37, 70), (1020, 33), (1034, 45)):
         H, N, L = synth_sketches(70, s, seed=300 + s, n_families=3, ragged=True)
         Hq, Nq, Lq = synth_sketches(nq, s, seed=400 + s, n_families=3, ragged=True)
         Hq[:7] = H[:7]; Nq[:7] = N[:7]

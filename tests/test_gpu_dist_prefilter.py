@@ -191,7 +191,19 @@ def test_scattered_relatives_take_the_pair_list(gpu, oracle, monkeypatch, pair_m
     assert np.array_equal(lst["numer"], wf["numer"].ravel()[flat])
 
 
-@pytest.mark.parametrize("s", [1036, 2500, 10000])
+def test_tiled_merge_ends_at_sketch_size_1034(gpu):
+    # the prefilter runs in front of the tiled merge only: on at s = 1034, the largest sketch size whose 32-reference tile and
+    # query buffers fit shared memory, off at s = 1035, which takes the warp-per-pair merge
+    for s, tiled in ((1034, True), (1035, False)):
+        H, N, L = synth_sketches(40, s, seed=s)
+        job = gpu.dist_open(H, N, L, sketch_size=s, k=21, kmer_space=4.0 ** 21)
+        try:
+            assert job.prefilter_stats()["active"] == tiled, s
+        finally:
+            job.close()
+
+
+@pytest.mark.parametrize("s", [1035, 1036, 2500, 10000])
 def test_large_sketch_sizes_use_the_warp_per_pair_merge(gpu, oracle, s):
     # `mash sketch -s 10000` is a documented setting: sketches whose 32-reference tile does not fit shared memory are compared one
     # warp per pair (zooming union count) -- same results as the reference's sequential merge, ragged and empty rows included

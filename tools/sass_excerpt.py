@@ -17,9 +17,8 @@ KERNELS = {
     "scan_kernel_k21_canonical_ascii_screen": "_ZN7mashgpu11scan_kernelILi21ELb1ELb0ELb1EEEvNS_8ScanArgsE",
     "scan_bytes_kernel_k9": "_ZN7mashgpu17scan_bytes_kernelILi9EEEvNS_8ScanArgsE",        # protein sketches and the translated screen
     "translate6_kernel": "_ZN7mashgpu17translate6_kernelEPKhmiiPhNS_8TrFramesE",
-    "dist_kernel": "_ZN7mashgpu11dist_kernelILb0EEEvNS_8DistArgsE",
-    "dist_kernel_bulk_copy_variant": "_ZN7mashgpu11dist_kernelILb1EEEvNS_8DistArgsE",
-    "dist_probe_kernel": "_ZN7mashgpu17dist_probe_kernelILb0EEEvNS_8DistArgsE",
+    "dist_kernel": "_ZN7mashgpu11dist_kernelENS_8DistArgsE",
+    "dist_probe_kernel": "_ZN7mashgpu17dist_probe_kernelENS_8DistArgsE",
     "dist_pair_kernel": "_ZN7mashgpu16dist_pair_kernelENS_8DistArgs",
 }
 PIPES = {

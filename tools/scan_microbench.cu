@@ -15,10 +15,8 @@
 // ALU instructions to every window's filter word (the checksum stays the kernel's); the kernel's time over n tells which pipe
 // binds the hot loop.
 //
-// Variants of the kernel itself, whose checksums must all agree: -DSCAN_PREFETCH_SMEM=0 (next tile prefetched into
-// registers instead of the shared landing buffer), -DSCAN_RESOLVE_INLINE=1 (the per-tile resolution of the pass masks
-// inlined instead of called), -DSCAN_MIN_BLOCKS=n (resident CTAs per SM requested from ptxas).  SCAN_VOTE_GROUP applies to
-// the FULL kernels only and does not change the kernel timed here.
+// Variants of the kernel itself, whose checksums must agree with the default build's: -DSCAN_MIN_BLOCKS=n (resident CTAs
+// per SM requested from ptxas).
 //
 // Build one binary per variant and run them alternately, e.g.
 //   nvcc -std=c++17 -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -DSCAN_MIN_BLOCKS=3 -I mash_b200/csrc \
@@ -144,9 +142,7 @@ int main(int argc, char **argv)
     const double loop_cycles_256 = cyc / ((double)ntiles * (SCAN_TILE / SCAN_WARP_TILE) * (SCAN_WARP_TILE / 256));
     std::vector<float> sorted = ms; std::sort(sorted.begin(), sorted.end());
     const float med = sorted[reps / 2];
-    // SCAN_VOTE_GROUP only shapes the FULL kernels (k <= 16, screen); the kernel timed here resolves per-lane pass masks per tile
-    printf("{\"variant\": \"%s\", \"min_blocks\": %d, \"prefetch_smem\": %d, \"resolve_inline\": %d, \"vote_group_full_kernels_only\": %d, "
-           "\"extra_fma\": %d, \"extra_alu\": %d, \"regs\": %d, \"local_bytes\": %zu, \"occupancy\": %d, "
+    printf("{\"variant\": \"%s\", \"min_blocks\": %d, \"extra_fma\": %d, \"extra_alu\": %d, \"regs\": %d, \"local_bytes\": %zu, \"occupancy\": %d, "
            "\"units\": %u, \"bases\": %llu, \"ms_median\": %.3f, \"ms_min\": %.3f, \"ms_max\": %.3f, \"gbps_median\": %.1f, "
            "\"checksum\": \"%016llx\", \"candidates\": %llu, \"overflowed_units\": %llu, \"maxhash\": %llu, \"warps_per_scheduler\": %d, "
            "\"loop_cycles_per_256_windows_per_warp\": %.1f, \"gbps_min\": %.1f, \"gbps_max\": %.1f}\n",
@@ -155,7 +151,7 @@ int main(int argc, char **argv)
 #else
            "default",
 #endif
-           SCAN_MIN_BLOCKS, SCAN_PREFETCH_SMEM, SCAN_RESOLVE_INLINE, SCAN_VOTE_GROUP, SCAN_MB_EXTRA_FMA, SCAN_MB_EXTRA_ALU, fa.numRegs, (size_t)fa.localSizeBytes, per_sm, n_units, (unsigned long long)n, med,
+           SCAN_MIN_BLOCKS, SCAN_MB_EXTRA_FMA, SCAN_MB_EXTRA_ALU, fa.numRegs, (size_t)fa.localSizeBytes, per_sm, n_units, (unsigned long long)n, med,
            sorted[0], sorted[reps - 1], n / med / 1e6, h_sum[0], h_sum[1], (unsigned long long)nflag, (unsigned long long)nmax,
            per_sm * SCAN_WARPS / 4, SCAN_MB_CLOCK ? loop_cycles_256 : 0.0, n / sorted[reps - 1] / 1e6, n / sorted[0] / 1e6);
     return 0;
