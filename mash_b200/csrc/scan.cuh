@@ -629,6 +629,49 @@ __device__ __forceinline__ void scan_group(const ScanArgs &a, const uint32_t (&b
     }
 }
 
+// 4 ASCII bytes -> 4 codes, one per byte: A=0 C=1 G=2 T=3 as ascii4_to_nibbles, anything else 8 | (bits 1-2 of the
+// upper-cased byte's ((u >> 1) ^ (u >> 2)), which only the exact rebuild's validity test sees, and it looks at bit 3 alone)
+__device__ __forceinline__ uint32_t ascii4_to_codes(uint32_t w, uint32_t fold)
+{
+    const uint32_t u = w & fold;
+    const uint32_t t = (u >> 2) & ~(u >> 1) & 0x01010101u;                    // bit2 & ~bit1: 'T'
+    const uint32_t expect = (0x41414141u | (u & 0x06060606u)) ^ (t * 0x11u);  // the ACGT byte with these bits 1,2
+    const uint32_t bad = u ^ expect;
+    const uint32_t nz = (((bad & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | bad) & 0x80808080u;  // bit7 set where byte != 0
+    return (((u >> 1) ^ (u >> 2)) & 0x03030303u) | (nz >> 4);                  // A 0x41, C 0x43, G 0x47, T 0x54 -> 0 1 2 3
+}
+
+// 8 ASCII bytes -> one nibble word: the byte codes of both halves, even bytes and odd bytes gathered by two PRMT
+__device__ __forceinline__ uint32_t ascii8_to_word(uint32_t lo, uint32_t hi, uint32_t fold)
+{
+    const uint32_t x0 = ascii4_to_codes(lo, fold), x1 = ascii4_to_codes(hi, fold);
+    return __byte_perm(x0, x1, 0x6420) | (__byte_perm(x0, x1, 0x7531) << 4);
+}
+
+// the nibble word of the 8 bytes at stream offset `off`, with the bytes at or past stream_len made separators
+__device__ __forceinline__ uint32_t clip_word(uint32_t w, uint64_t off, uint64_t stream_len)
+{
+    if (off >= stream_len) return 0x88888888u;
+    if (off + 8 > stream_len) w |= 0x88888888u << (4 * (uint32_t)(stream_len - off));   // 1..7 bytes kept
+    return w;
+}
+
+// Filter-word kernels, ASCII source: a lane's staged words -- words 2 lane, 2 lane + 1 (w0, w1), 64 + 2 lane, 65 + 2 lane
+// (w2, w3) and halo word 128 + hw (w4) -- into a forward image and, canonical, its reverse-complement image
+template <bool CANON>
+__device__ __forceinline__ void stage_words(uint32_t *sm, uint32_t *smr, int lane, int hw, uint32_t w0, uint32_t w1, uint32_t w2,
+                                            uint32_t w3, uint32_t w4)
+{
+    *reinterpret_cast<uint2 *>(sm + 2 * lane) = make_uint2(w0, w1);
+    *reinterpret_cast<uint2 *>(sm + 2 * (lane + 32)) = make_uint2(w2, w3);
+    sm[128 + hw] = w4;
+    if (CANON) {
+        *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * lane)) = make_uint2(nibble_reverse(w1) ^ 0x33333333u, nibble_reverse(w0) ^ 0x33333333u);
+        *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * (lane + 32))) = make_uint2(nibble_reverse(w3) ^ 0x33333333u, nibble_reverse(w2) ^ 0x33333333u);
+        smr[SCAN_WARP_WORDS - 1 - 128 - hw] = nibble_reverse(w4) ^ 0x33333333u;
+    }
+}
+
 // 16 ASCII bytes at stream offset `off` -> two nibble words (bytes at or past stream_len become separators)
 __device__ __forceinline__ uint2 stage16(const uint4 q, uint64_t off, uint64_t stream_len, uint32_t fold)
 {
@@ -783,10 +826,12 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     uint64_t wt = wt_begin + (uint64_t)blockIdx.x * SCAN_WARPS + warp;
     if (wt >= wt_end) return;
 
-    // each lane stages vectors lane, lane+32 and one of the 4 halo vectors (64 + lane%4: eight lanes write the same
-    // words with the same values -- no lane-dependent branch, the warp never splits): 16 bytes -> 2 words each
-    static_assert(SCAN_WARP_VECS - 64 == 4, "halo = 4 vectors");
+    // FULL kernels: each lane stages vectors lane, lane+32 and one of the 4 halo vectors (64 + lane%4: eight lanes write the
+    // same words with the same values -- no lane-dependent branch, the warp never splits): 16 bytes -> 2 words each.
+    // Filter-word kernels: vectors lane and lane+32, and halo word 128 + lane%8 (8 bytes -> 1 word, four lanes alike).
+    static_assert(SCAN_WARP_VECS - 64 == 4 && SCAN_HALO_WORDS == 8, "halo = 4 vectors = 8 words");
     const int v2 = 64 + (lane & 3);
+    const int hw = lane & 7;
     uint4 q0, q1, q2;                      // ASCII source: three 16-byte vectors per lane
     uint64_t pc0 = 0, pc1 = 0;             // packed source: group (lane) and one of the 2 halo groups (32 + lane%2)
     uint32_t pm0 = 0, pm1 = 0;
@@ -821,7 +866,8 @@ scan_kernel(const __grid_constant__ ScanArgs a)
             } else {
                 q0 = lds_u128(land + 16 * lane);
                 q1 = lds_u128(land + 16 * (lane + 32));
-                q2 = lds_u128(land + 16 * v2);
+                const uint64_t h = lds_u64(land + 16 * 64 + 8 * hw);
+                q2 = make_uint4((uint32_t)h, (uint32_t)(h >> 32), 0u, 0u);
             }
         }
         if (SCAN_MB_STAGE_ONCE && wt != wt_first) {
@@ -836,6 +882,19 @@ scan_kernel(const __grid_constant__ ScanArgs a)
                 *reinterpret_cast<uint4 *>(smr + (SCAN_WARP_WORDS - 4 - 4 * hg)) =
                     make_uint4(nibble_reverse(e1.w) ^ 0x33333333u, nibble_reverse(e1.z) ^ 0x33333333u, nibble_reverse(e1.y) ^ 0x33333333u, nibble_reverse(e1.x) ^ 0x33333333u);
             }
+        } else if constexpr (!FULL) {
+            uint32_t w0 = ascii8_to_word(q0.x, q0.y, fold), w1 = ascii8_to_word(q0.z, q0.w, fold);
+            uint32_t w2 = ascii8_to_word(q1.x, q1.y, fold), w3 = ascii8_to_word(q1.z, q1.w, fold);
+            uint32_t w4 = ascii8_to_word(q2.x, q2.y, fold);
+            if (base + 16ull * SCAN_WARP_VECS > a.stream_len) {   // warp-uniform: only the last tile of a launch
+                const uint64_t o0 = base + 16ull * lane, o1 = o0 + 16ull * 32;
+                w0 = clip_word(w0, o0, a.stream_len);
+                w1 = clip_word(w1, o0 + 8, a.stream_len);
+                w2 = clip_word(w2, o1, a.stream_len);
+                w3 = clip_word(w3, o1 + 8, a.stream_len);
+                w4 = clip_word(w4, base + 16ull * 64 + 8ull * hw, a.stream_len);
+            }
+            stage_words<CANON>(sm, smr, lane, hw, w0, w1, w2, w3, w4);
         } else {
             const uint2 s0 = stage16(q0, base + 16ull * lane, a.stream_len, fold);
             const uint2 s1 = stage16(q1, base + 16ull * (lane + 32), a.stream_len, fold);

@@ -54,8 +54,9 @@ def hot_path_line(body):
     alu = sum(n for o, n in c.items() if o in PIPES["ALU (SHF/LOP3/IADD3/PRMT/ISETP/SEL/...)"] + ("VIADD",))
     ctl = ", ".join(f"{o} {c[o]}" for o in ("VOTE", "CALL", "BSSY", "BSYNC", "BRA") if c[o]) or "none"
     what = f"without the {len(skip)} survivor blocks behind the warp votes" if skip else "no warp vote in it: the whole loop"
+    span = body[-1][0] + 16 - body[0][0]
     return (f"hot path (longest innermost loop, {what}): {len(hot)} "
-            f"instructions per lane per 8 windows; ALU pipe {alu}, IMAD {c['IMAD']}, STL {c['STL']}, LDL {c['LDL']}, S2R {c['S2R']}; "
+            f"instructions per lane per loop trip, {span} bytes of code; ALU pipe {alu}, IMAD {c['IMAD']}, STL {c['STL']}, LDL {c['LDL']}, S2R {c['S2R']}; "
             f"control: {ctl}")
 
 
@@ -118,7 +119,7 @@ def main():
         for body in loops[:8]:
             lo = collections.Counter(re.sub(r"^@!?U?P\d+\s+", "", t).split()[0].split(".")[0] for _, t in body)
             summary.append("")
-            summary.append(f"innermost loop, {len(body)} instructions at {body[0][0]:#x}..{body[-1][0]:#x}: " + ", ".join(f"{o} {c}" for o, c in lo.most_common(12)))
+            summary.append(f"innermost loop, {len(body)} instructions ({body[-1][0] + 16 - body[0][0]} bytes) at {body[0][0]:#x}..{body[-1][0]:#x}: " + ", ".join(f"{o} {c}" for o, c in lo.most_common(12)))
         for i, body in enumerate(loops[:4]):
             # the scan kernels' hot loop in full, so that its control flow can be read off the listing
             keep = 1200 if i == 0 and name.startswith("scan_kernel") else 400
