@@ -55,7 +55,13 @@ typedef struct mashgpu_sketch_params {
                                  the sketch at its m-th occurrence.  0 or 1 = off.  The sketch is then the s smallest hashes seen at
                                  least m times, and the multiplicities follow the heap exactly (tests/test_gpu_sketch.py). */
     double target_cov;        /* `-c`: stop after the first read that brings the heap's average multiplicity to this value
-                                 (Sketch.cpp:1258-1262).  Only mashgpu_sketch_reads looks at it; <= 0 = off. */
+                                 (Sketch.cpp:1258-1262).  Only the reads paths look at it; <= 0 = off. */
+    uint64_t bloom_bytes;     /* `-b`: MinHashHeap memoryBoundBytes (Sketch.cpp:1186, MinHashHeap.cpp:19-41, 78-95): a hash enters the
+                                 sketch with count 2 when a Bloom filter of bloom_bytes bytes already holds it, else it is added to the
+                                 filter.  The filter is the reference's exactly: one hash function, 8 * bloom_bytes bits of which the
+                                 32-bit index reaches the first 2^32, so min(bloom_bytes, 2^29) bytes of device memory.  0 = off.  Only
+                                 the reads paths take it (every other entry point returns MASHGPU_ERR_UNSUPPORTED); together with
+                                 min_copies > 1 it is MASHGPU_ERR_INVALID, as the reference CLI refuses -b with -m. */
 } mashgpu_sketch_params;
 /* GPU path coverage: alphabet == {A,C,G,T} (canonical or not, any k 1..32, either case mode) runs the 4-bit
  * packed DNA kernels; any other alphabet requires noncanonical != 0 (the protein setting of the reference,
@@ -91,17 +97,35 @@ int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
                          const uint32_t *unit_of_record, uint64_t n_units,
                          uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length);
 
-/* One sketch of a read set, `mash sketch -r [-m min_copies] [-c target_cov]` (sketchFile with parameters.reads, Sketch.cpp:1186-1282):
- * all records in the order given (the caller interleaves several files round robin as Sketch.cpp:1202-1270 does).  With
- * target_cov > 0 the result is the heap as it stood after the first kept record that brought estimateMultiplicity() to the target
- * (Sketch.cpp:1258-1262) and *out_records_used (the "Reads used" line, :1324-1327) is the number of kept records up to and
- * including it; otherwise all kept records are used.  The stop depends on the order of the reads; it is found exactly: the
- * exact top of the heap at geometrically spaced prefixes bounds which k-mers can pass the heap's gate afterwards, those
- * k-mers are collected as events and replayed in stream order through the reference's heap logic on the device
- * (DESIGN.md 2.6).  out_counts nullable.  DNA alphabet only. */
+/* One sketch of a read set, `mash sketch -r [-m min_copies] [-c target_cov] [-b bloom_bytes]` (sketchFile with parameters.reads,
+ * Sketch.cpp:1186-1282): all records in the order given (the caller interleaves several files round robin as Sketch.cpp:1202-1270
+ * does).  With target_cov > 0 the result is the heap as it stood after the first kept record that brought estimateMultiplicity()
+ * to the target (Sketch.cpp:1258-1262) and *out_records_used (the "Reads used" line, :1324-1327) is the number of kept records up
+ * to and including it; otherwise all kept records are used.  With target_cov > 0 or bloom_bytes, or when the set does not fit in half
+ * of the free device memory, this is mashgpu_reads_open + one mashgpu_reads_feed + mashgpu_reads_finish + mashgpu_reads_close;
+ * otherwise the result does not depend on the order of the reads and the whole set is sketched in one parallel pass (same result,
+ * faster: DESIGN.md 2.6).  out_counts nullable.  DNA alphabet only. */
 int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
                          uint64_t n_records, const char *const *seq, const uint64_t *len,
                          uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used);
+
+/* The same as a streaming job, for read sets of any size: records are fed in order, in any number of feeds, and the result does not
+ * depend on how they are split.  Each staged buffer is scanned stretch by stretch with the heap's current top as threshold (a top
+ * never rises once the heap is full, so it bounds every k-mer after it that can change the heap); those k-mers are sorted by
+ * position and replayed through the reference's heap logic (MinHashHeap::tryInsert, the Bloom branch included) by one warp whose
+ * state stays in device memory (DESIGN.md 2.6).  Device memory is fixed at open by the parameters -- staging
+ * (MASHGPU_READS_STAGE_BYTES, default 128 MiB), events (MASHGPU_READS_EVENT_CAP, default 2^21), O(s + pending hashes) replay
+ * tables and min(bloom_bytes, 2^29) bytes of filter -- never by the size of the read set.  DNA alphabet only. */
+typedef struct mashgpu_reads_job mashgpu_reads_job;
+int mashgpu_reads_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, mashgpu_reads_job **job);
+/* The next n_records records, as mashgpu_sketch_reads takes them.  Records shorter than kmer_size are skipped; a record longer than
+ * the staging buffer is split with a (kmer_size-1)-base overlap and each of its windows is counted once.  Returns once the
+ * caller's buffers are free; *stopped (nullable) = 1 once the target coverage was reached, after which feeds are accepted and
+ * ignored. */
+int mashgpu_reads_feed(mashgpu_reads_job *job, uint64_t n_records, const char *const *seq, const uint64_t *len, int *stopped);
+/* The sketch (sketch_size slots, ascending) and the kept records used, as mashgpu_sketch_reads returns them.  out_counts nullable. */
+int mashgpu_reads_finish(mashgpu_reads_job *job, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used);
+int mashgpu_reads_close(mashgpu_reads_job *job);
 
 /* Same computation on a sequence stream already resident in device memory.  d_stream holds the units back to
  * back; unit u occupies bytes [unit_start[u], unit_start[u+1]) (host array of n_units+1 offsets); records inside
@@ -364,6 +388,9 @@ typedef struct mashgpu_stats {
     double translate_kernel_ms;    /* accumulated device time of the six-frame translation kernel (translated screen) */
     uint64_t translate_kernel_launches;
     double taxonomy_ms;            /* accumulated device time of mashgpu_screen_taxonomy's kernels, copies and scans */
+    uint64_t reads_events;         /* k-mers replayed through the heap by reads jobs */
+    double reads_replay_ms;        /* accumulated device time of the replay kernel of reads jobs (with timing on) */
+    uint64_t reads_peak_device_bytes;  /* largest device footprint of the last reads job opened (not cleared by reset) */
 } mashgpu_stats;
 /* timing != 0 brackets the dominant kernels with CUDA events (adds a sync at mashgpu_get_stats). */
 int mashgpu_set_timing(mashgpu_ctx *ctx, int timing);

@@ -31,7 +31,8 @@ class SketchParams(C.Structure):
     """mashgpu_sketch_params (Sketch::Parameters subset, reference Sketch.h:34-109)."""
     _fields_ = [("kmer_size", C.c_int32), ("sketch_size", C.c_uint32), ("seed", C.c_uint32),
                 ("use64", C.c_int32), ("noncanonical", C.c_int32), ("preserve_case", C.c_int32),
-                ("alphabet", C.c_uint8 * 256), ("min_copies", C.c_uint32), ("target_cov", C.c_double)]
+                ("alphabet", C.c_uint8 * 256), ("min_copies", C.c_uint32), ("target_cov", C.c_double),
+                ("bloom_bytes", C.c_uint64)]
 
     @property
     def kmer_space(self):
@@ -52,7 +53,8 @@ class SketchSet(C.Structure):
 class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("scan_kernel_ms", C.c_double), ("scan_kernel_launches", C.c_uint64),
                 ("dist_kernel_ms", C.c_double), ("dist_kernel_launches", C.c_uint64), ("exact_reruns", C.c_uint64),
-                ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64), ("taxonomy_ms", C.c_double)]
+                ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64), ("taxonomy_ms", C.c_double),
+                ("reads_events", C.c_uint64), ("reads_replay_ms", C.c_double), ("reads_peak_device_bytes", C.c_uint64)]
 
 
 class TaxRow(C.Structure):
@@ -94,6 +96,10 @@ def load_library():
     L.mashgpu_sketch_stream_dev.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.c_void_p, u64p, C.c_uint64,
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.mashgpu_sketch_reads.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.c_uint64, C.c_void_p, u64p, u64p, u32p, u32p, u64p]
+    L.mashgpu_reads_open.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.POINTER(C.c_void_p)]
+    L.mashgpu_reads_feed.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, u64p, C.POINTER(C.c_int)]
+    L.mashgpu_reads_finish.argtypes = [C.c_void_p, u64p, u32p, u32p, u64p]
+    L.mashgpu_reads_close.argtypes = [C.c_void_p]
     L.mashgpu_sketch_batch_packed.argtypes = [C.c_void_p, C.POINTER(SketchParams), u64p, C.c_uint64, u64p, C.c_uint64, u64p, C.c_uint64, u64p, u32p, u32p]
     L.mashgpu_host_pack.argtypes = [C.POINTER(SketchParams), C.c_uint64, C.c_void_p, u64p, C.c_int, u64p, u64p, C.c_uint64, u64p]
     L.mashgpu_hash_windows.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.c_void_p, C.c_uint64, u64p, u8p]
@@ -186,10 +192,12 @@ class Engine:
             raise MashGpuError(rc, (self.lib.mashgpu_last_error(self.h) or b"").decode())
 
     # ---- parameters (sketchParameterSetup / setAlphabetFromString) --------------------------------------
-    def params(self, k=21, s=1000, seed=42, alphabet=ALPHABET_NUCLEOTIDE, noncanonical=False, preserve_case=False, min_copies=1, target_cov=0.0):
+    def params(self, k=21, s=1000, seed=42, alphabet=ALPHABET_NUCLEOTIDE, noncanonical=False, preserve_case=False, min_copies=1, target_cov=0.0,
+               bloom_bytes=0):
         p = SketchParams()
         p.min_copies = min_copies
         p.target_cov = target_cov
+        p.bloom_bytes = bloom_bytes
         p.kmer_size = k
         p.sketch_size = s
         p.seed = seed
@@ -231,6 +239,10 @@ class Engine:
         self._check(self.lib.mashgpu_sketch_reads(self.h, C.byref(p), len(bufs), C.cast(ptrs, C.c_void_p), _p(lens, u64p), _p(out, u64p), _p(out_c, u32p),
                                                   C.byref(n), C.byref(used)))
         return out[:n.value].copy(), (out_c[:n.value].copy() if counts else None), used.value
+
+    def reads_open(self, p):
+        """A streaming `mash sketch -r` job: feed the read set in any number of pieces, then finish()."""
+        return ReadsJob(self, p)
 
     def host_pack(self, records, p, threads=1):
         """records -> (codes u64[ceil(L/32)], runs u64[n, 2], record_start u64[n_records + 1]) in the packed stream format
@@ -411,6 +423,37 @@ class DistJob:
     def close(self):
         if self.h:
             self.eng.lib.mashgpu_dist_close(self.h)
+            self.h = None
+
+
+class ReadsJob:
+    def __init__(self, eng, p):
+        self.eng = eng
+        self.p = p
+        h = C.c_void_p()
+        eng._check(eng.lib.mashgpu_reads_open(eng.h, C.byref(p), C.byref(h)))
+        self.h = h
+
+    def feed(self, records):
+        """The next records of the read set, in order.  Returns True once the target coverage (-c) was reached."""
+        bufs = [_as_u8(r) for r in records]
+        ptrs = (C.c_void_p * max(1, len(bufs)))(*[b.ctypes.data if b.size else None for b in bufs])
+        lens = np.array([b.size for b in bufs], dtype=np.uint64)
+        stopped = C.c_int(0)
+        self.eng._check(self.eng.lib.mashgpu_reads_feed(self.h, len(bufs), C.cast(ptrs, C.c_void_p), _p(lens, u64p), C.byref(stopped)))
+        return bool(stopped.value)
+
+    def finish(self):
+        """(hashes ascending, counts, records used) -- what Engine.sketch_reads returns with counts=True."""
+        s = self.p.sketch_size
+        out = np.zeros(s, np.uint64); out_c = np.zeros(s, np.uint32)
+        n = C.c_uint32(0); used = C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_reads_finish(self.h, _p(out, u64p), _p(out_c, u32p), C.byref(n), C.byref(used)))
+        return out[:n.value].copy(), out_c[:n.value].copy(), used.value
+
+    def close(self):
+        if self.h:
+            self.eng.lib.mashgpu_reads_close(self.h)
             self.h = None
 
 

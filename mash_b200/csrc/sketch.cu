@@ -23,6 +23,7 @@
 #include <mutex>
 #include <thread>
 #include <cstdlib>
+#include <memory>
 
 namespace mashgpu {
 
@@ -308,7 +309,7 @@ __global__ void emit_sorted_kernel(const uint64_t *sorted, uint32_t m, const uin
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-int validate_sketch_params(mashgpu_ctx *ctx, const mashgpu_sketch_params *p)
+int validate_sketch_params(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, bool reads)
 {
     if (!p) return fail(ctx, MASHGPU_ERR_INVALID, "params is NULL");
     if (p->kmer_size < 1 || p->kmer_size > 32) return fail(ctx, MASHGPU_ERR_INVALID, "kmer_size %d outside 1..32", p->kmer_size);
@@ -321,6 +322,7 @@ int validate_sketch_params(mashgpu_ctx *ctx, const mashgpu_sketch_params *p)
         return fail(ctx, MASHGPU_ERR_INVALID, "use64=%d contradicts the reference rule alphabetSize^k > 2^32 for k=%d, %d letters (Sketch.cpp:1136)", p->use64, p->kmer_size, n);
     if (p->alphabet[0]) return fail(ctx, MASHGPU_ERR_INVALID, "byte 0 cannot be an alphabet letter");
     if (p->min_copies > 255) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "min_copies (-m) above 255");
+    if (p->bloom_bytes && !reads) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "bloom_bytes (-b) only applies to reads mode (mashgpu_reads_*, mashgpu_sketch_reads)");
     if (!dna && !p->noncanonical)
         return fail(ctx, MASHGPU_ERR_UNSUPPORTED,
                     "canonical k-mers are only defined for the alphabet {A,C,G,T}; other alphabets must be non-canonical "
@@ -1237,16 +1239,15 @@ extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketc
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// `mash sketch -r -m -c`: the order-dependent stop at a target coverage, found exactly.
+// `mash sketch -r [-m] [-c] [-b]`: a streaming reads job, replayed exactly through the reference's heap (DESIGN.md 2.6).
 //
 // MinHashHeap::tryInsert only looks at a k-mer when the heap is not full or its hash is below the heap's top (MinHashHeap.cpp:70-74),
-// and once the heap is full the top never rises.  So the exact top at a stream position P (the largest hash of the ordinary
-// bottom-s(-m) sketch of the prefix [0, P), computed by the normal kernels) bounds every k-mer after P that can still change the
-// heap.  Prefixes at record boundaries near total / 2^j give position bands with a threshold each (the first band, and any
-// band that starts before the heap is full, keeps everything); one more scan collects the k-mers at or below their band's
-// threshold as events {position, hash}; sorted by position they are replayed through the reference's heap logic by
-// reads_replay_kernel -- a faithful, sequential restatement of MinHashHeap::tryInsert (MinHashHeap.cpp:68-146) with the stop
-// test of Sketch.cpp:1258-1262 at every read boundary.  A few 10^5 events for a read set of any size.
+// and once the heap is full the top never rises.  So the top at the start of any stretch of the stream (no limit while the heap is
+// not full) bounds every k-mer of the stretch that can change the heap.  Each stretch of a staged buffer is scanned once with that
+// threshold (SCAN_EVENTS); the events {position, hash} are sorted by position and replayed by reads_replay_kernel -- a faithful,
+// sequential restatement of MinHashHeap::tryInsert (MinHashHeap.cpp:68-146, the Bloom branch :78-95 included) with the stop test of
+// Sketch.cpp:1258-1262 -- through a replay state that stays in device memory for the whole job.  Device memory is fixed by the
+// parameters (staging, event buffers, O(s + pending) replay tables, the Bloom bits), never by the size of the read set.
 // ---------------------------------------------------------------------------------------------------------
 namespace mashgpu {
 
@@ -1307,96 +1308,519 @@ __device__ void rh_pop(uint64_t *heap, uint64_t &n)
     if (n) heap[i] = v;
 }
 
-// One thread replays the events.  acc = hashes + hashesQueue, pend = hashesPending + hashesQueuePending of MinHashHeap.
-__global__ void reads_replay_kernel(const uint64_t *ev_pos, const uint64_t *ev_hash, uint64_t n_ev, const uint64_t *rec_end, uint64_t n_rec,
-                                    uint32_t s, uint32_t m, double target_cov,
-                                    ReplayMap acc, uint64_t *acc_heap, ReplayMap pend, uint64_t *pend_heap,
-                                    uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_used)
+constexpr uint64_t NO_RECORD = ~0ull;
+
+// The heap between launches.  acc = hashes + hashesQueue, pend = hashesPending + hashesQueuePending of MinHashHeap.
+struct ReplayState {
+    uint64_t size, heap_n, pend_n, msum;
+    uint64_t cur;                   // record of the last event that passed the gate and has not had its stop test yet
+    uint64_t used;                  // records used, once stopped
+    uint64_t gate_t;                // EMPTY_KEY while the heap is not full, else its top: the scan threshold of the next stretch
+    unsigned long long ev_count;    // events of the last scan (may exceed the buffer: the stretch is then split)
+    uint32_t stopped;
+};
+
+// Bloom filter of MinHashHeap(use64, s, 1, b) (bloom_filter.hpp with false_positive_probability 0): one hash function, 8 b bits,
+// salt = predef_salt[0]^2 + (uint32)(random_seed * 0xA5A5A5A5 + 1) with the default random_seed, bit = hash_ap(key) mod 8 b
+// (the 32-bit hash_ap reaches only the first 2^32 bits).  The key is the hash's 8 little-endian bytes, or 4 with 32-bit hashes.
+constexpr uint32_t BLOOM_SALT = 0x9A0876E7u;
+constexpr uint64_t BLOOM_MAX_BYTES = 1ull << 29;
+
+__host__ __device__ inline uint32_t bloom_hash_ap(uint64_t key, bool use64)
 {
-    if (blockIdx.x || threadIdx.x) return;
-    uint64_t size = 0, heap_n = 0, pend_n = 0, msum = 0;
-    uint64_t rec = 0, cur = ~0ull, used = n_rec;
+    uint32_t h = BLOOM_SALT;
+    const uint32_t i1 = (uint32_t)key, i2 = (uint32_t)(key >> 32);
+    if (use64) h ^= (h << 7) ^ i1 * (h >> 3) ^ (~((h << 11) + (i2 ^ (h >> 5))));    // one 8-byte block
+    else h ^= ~((h << 11) + (i1 ^ (h >> 5)));                                        // the 4-byte tail, loop == 0
+    return h;
+}
+
+// After the sort: the record of every event (first record whose separator lies after the position) and its Bloom bit.
+__global__ void reads_event_meta_kernel(uint64_t *ev_pos_to_rec, const uint64_t *ev_hash, uint64_t n_ev, const uint64_t *rec_end,
+                                        uint64_t n_rec, uint64_t rec_base, uint64_t bloom_bits, int use64, uint32_t *ev_bit)
+{
+    const uint64_t e = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (e >= n_ev) return;
+    const uint64_t pos = ev_pos_to_rec[e];
+    uint64_t lo = 0, hi = n_rec;
+    while (lo < hi) { const uint64_t mid = (lo + hi) >> 1; if (rec_end[mid] <= pos) lo = mid + 1; else hi = mid; }
+    ev_pos_to_rec[e] = rec_base + lo;
+    if (bloom_bits) ev_bit[e] = (uint32_t)(bloom_hash_ap(ev_hash[e], use64) % bloom_bits);
+}
+
+__global__ void reads_fill_tmax_kernel(uint64_t *tile_tmax, uint64_t t0, uint64_t t1, const ReplayState *st)
+{
+    const uint64_t t = t0 + blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t < t1) tile_tmax[t] = st->gate_t;
+}
+
+__device__ __forceinline__ bool reads_stop_test(ReplayState &S, double target_cov)
+{
+    if (S.cur == NO_RECORD) return false;
+    const bool stop = target_cov > 0 && S.size && (double)S.msum / (double)S.size >= target_cov;      // Sketch.cpp:1258-1262
+    if (stop) { S.used = S.cur + 1; S.stopped = 1; }
+    S.cur = NO_RECORD;
+    return stop;
+}
+
+// One warp replays the events in order.  The heap's state only changes at events that pass its gate, so the stop test of record r
+// (after its last k-mer) is due when the next passing event lies in a later record, or at the end of a feed.  Lanes load 32 events
+// at a time and vote on the gate with the current top; lane 0 applies the passing ones one by one (the top only falls, so an
+// event that fails the vote fails the gate at its turn too).
+__global__ void reads_replay_kernel(ReplayState *state, const uint64_t *ev_rec, const uint64_t *ev_hash, const uint32_t *ev_bit, uint64_t n_ev,
+                                    uint32_t s, uint32_t m, double target_cov, ReplayMap acc, uint64_t *acc_heap, ReplayMap pend, uint64_t *pend_heap,
+                                    uint32_t *bloom)
+{
+    if (blockIdx.x) return;
+    const uint32_t lane = threadIdx.x;
+    ReplayState S = *state;
+    if (S.stopped) return;
     bool stopped = false;
-    for (uint64_t e = 0; e <= n_ev && !stopped; e++) {
-        uint64_t r = ~0ull;
-        if (e < n_ev) {
-            const uint64_t pos = ev_pos[e];
-            while (rec < n_rec && rec_end[rec] <= pos) rec++;
-            r = rec;
-        }
-        if (cur != ~0ull && r != cur) {                     // record `cur` is complete: Sketch.cpp:1258-1262
-            if (size && (double)msum / (double)size >= target_cov) { used = cur + 1; stopped = true; break; }
-        }
-        if (e == n_ev) break;
-        cur = r;
-        const uint64_t hash = ev_hash[e];
-        if (!(size < s || hash < acc_heap[0])) continue;    // MinHashHeap.cpp:70-74
-        uint32_t *c = rm_find(acc, hash);
-        if (!c) {
-            uint32_t *pc = m > 1 ? rm_find(pend, hash) : nullptr;
-            const uint64_t pending = pc ? *pc : 0;
-            if (m == 1 || pending == m - 1) {               // :96-108
-                rm_insert_new(acc, hash, m);
-                rh_push(acc_heap, heap_n, hash);
-                size++; msum += m;
-                if (m > 1 && pc) rm_erase(pend, hash);
-            } else if (!pc) {                               // :110-118
-                rh_push(pend_heap, pend_n, hash);
-                rm_insert_new(pend, hash, 1);
-            } else (*pc)++;
-        } else { (*c)++; msum++; }                          // :120-124
-        if (size > s) {                                     // :126-144
-            const uint64_t top = acc_heap[0];
-            uint32_t *tc = rm_find(acc, top);
-            msum -= tc ? *tc : 0;
-            rm_erase(acc, top);
-            while (pend_n > 0 && top < pend_heap[0]) {
-                if (rm_find(pend, pend_heap[0])) rm_erase(pend, pend_heap[0]);
-                rh_pop(pend_heap, pend_n);
+    for (uint64_t base = 0; base < n_ev && !stopped; base += 32) {
+        const uint64_t e = base + lane;
+        const bool valid = e < n_ev;
+        const uint64_t h = valid ? ev_hash[e] : 0, r = valid ? ev_rec[e] : 0;
+        const uint32_t bit = (valid && bloom) ? ev_bit[e] : 0;
+        uint32_t todo = __ballot_sync(0xFFFFFFFFu, valid);
+        for (;;) {
+            const uint64_t size = __shfl_sync(0xFFFFFFFFu, S.size, 0), top = __shfl_sync(0xFFFFFFFFu, S.gate_t, 0);
+            const uint32_t pass = __ballot_sync(0xFFFFFFFFu, valid && (size < s || h < top)) & todo;     // MinHashHeap.cpp:70-74
+            if (!pass) break;
+            const int src = __ffs(pass) - 1;
+            todo &= ~((2u << src) - 1u);
+            const uint64_t hash = __shfl_sync(0xFFFFFFFFu, h, src), rec = __shfl_sync(0xFFFFFFFFu, r, src);
+            const uint32_t b = __shfl_sync(0xFFFFFFFFu, bit, src);
+            int stop = 0;
+            if (lane == 0) {
+                if (S.cur != rec && reads_stop_test(S, target_cov)) stop = 1;
+                else {
+                    S.cur = rec;
+                    uint32_t *c = rm_find(acc, hash);
+                    if (!c) {
+                        if (bloom) {                                        // :78-95
+                            const uint32_t w = b >> 5, mask = 1u << (b & 31);
+                            if (bloom[w] & mask) {
+                                rm_insert_new(acc, hash, 2);
+                                rh_push(acc_heap, S.heap_n, hash);
+                                S.size++; S.msum += 2;
+                            } else bloom[w] |= mask;
+                        } else {
+                            uint32_t *pc = m > 1 ? rm_find(pend, hash) : nullptr;
+                            const uint64_t pending = pc ? *pc : 0;
+                            if (m == 1 || pending == m - 1) {               // :96-108
+                                rm_insert_new(acc, hash, m);
+                                rh_push(acc_heap, S.heap_n, hash);
+                                S.size++; S.msum += m;
+                                if (m > 1 && pc) rm_erase(pend, hash);
+                            } else if (!pc) {                               // :110-118
+                                rh_push(pend_heap, S.pend_n, hash);
+                                rm_insert_new(pend, hash, 1);
+                            } else (*pc)++;
+                        }
+                    } else { (*c)++; S.msum++; }                            // :120-124
+                    if (S.size > s) {                                       // :126-144
+                        const uint64_t t = acc_heap[0];
+                        uint32_t *tc = rm_find(acc, t);
+                        S.msum -= tc ? *tc : 0;
+                        rm_erase(acc, t);
+                        while (S.pend_n > 0 && t < pend_heap[0]) {
+                            if (rm_find(pend, pend_heap[0])) rm_erase(pend, pend_heap[0]);
+                            rh_pop(pend_heap, S.pend_n);
+                        }
+                        rh_pop(acc_heap, S.heap_n);
+                        S.size--;
+                    }
+                    S.gate_t = S.size >= s ? acc_heap[0] : EMPTY_KEY;
+                }
             }
-            rh_pop(acc_heap, heap_n);
-            size--;
+            if (__shfl_sync(0xFFFFFFFFu, stop, 0)) { stopped = true; break; }
         }
     }
-    // toHashList: ascending hashes + counts (HashSet.cpp:78-118); popping the max-heap yields them in descending order
+    if (lane == 0) *state = S;
+}
+
+// The stop test of the last record of a feed (a feed always ends with a whole record).
+__global__ void reads_feed_end_kernel(ReplayState *state, double target_cov)
+{
+    ReplayState S = *state;
+    if (!S.stopped) reads_stop_test(S, target_cov);
+    *state = S;
+}
+
+// Pending map growth: re-insert every entry of the old table into the new one (keys are distinct).
+__global__ void reads_rehash_kernel(ReplayMap from, ReplayMap to)
+{
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i <= from.mask; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t c = from.cnt[i];
+        if (!c) continue;
+        const uint64_t key = from.key[i];
+        uint64_t j = ((key * 0x9E3779B97F4A7C15ULL) >> 11) & to.mask;
+        while (atomicCAS(&to.cnt[j], 0u, c) != 0u) j = (j + 1) & to.mask;
+        to.key[j] = key;
+    }
+}
+
+// toHashList: ascending hashes + counts (HashSet.cpp:78-118); popping a copy of the max-heap yields them in descending order (the
+// job's own heap stays intact, so finish may be called again)
+__global__ void reads_emit_kernel(const ReplayState *state, ReplayMap acc, const uint64_t *acc_heap, uint64_t *heap_copy,
+                                  uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n)
+{
+    if (blockIdx.x || threadIdx.x) return;
+    uint64_t n = state->heap_n;
+    for (uint64_t i = 0; i < n; i++) heap_copy[i] = acc_heap[i];
+    const uint64_t size = state->size;
     *out_n = (uint32_t)size;
-    *out_used = used;
     for (uint64_t i = size; i-- > 0;) {
-        const uint64_t v = acc_heap[0];
+        const uint64_t v = heap_copy[0];
         out_hashes[i] = v;
-        if (out_counts) { const uint32_t *c = rm_find(acc, v); out_counts[i] = c ? *c : 0; }
-        rh_pop(acc_heap, heap_n);
+        const uint32_t *c = rm_find(acc, v);
+        out_counts[i] = c ? *c : 0;
+        rh_pop(heap_copy, n);
     }
 }
 
 }  // namespace mashgpu
 
-extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
-                                    uint64_t n_records, const char *const *seq, const uint64_t *len,
-                                    uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used)
+struct mashgpu_reads_job {
+    mashgpu_ctx *ctx = nullptr;
+    mashgpu_sketch_params params{};
+    uint32_t s = 0, m = 1;
+    uint64_t k = 0;
+    uint64_t stage_cap = 0, ev_cap = 0, bloom_bits = 0;
+    // staging: one pinned buffer, its device copy and the record ends (offsets of their separators) inside it
+    mashgpu::PinnedBuf<uint8_t> h_stage;
+    mashgpu::DevBuf<uint8_t> d_stage;
+    uint64_t fill = 0;
+    std::vector<uint64_t> rec_end;
+    mashgpu::DevBuf<uint64_t> d_rec_end, d_tmax;
+    uint64_t rec_base = 0;          // kept records that ended in earlier stages
+    uint64_t records = 0;           // kept records fed (the ones before the stop, once stopped)
+    std::vector<uint8_t> carry;     // the last k-1 bases of a record split across stages
+    // events
+    mashgpu::DevBuf<uint64_t> ev_pos, ev_hash, ev_pos2, ev_hash2;
+    mashgpu::DevBuf<uint32_t> ev_bit;
+    mashgpu::DevBuf<uint8_t> sort_tmp;
+    size_t sort_tmp_bytes = 0;
+    // replay state
+    mashgpu::DevBuf<mashgpu::ReplayState> d_state;
+    mashgpu::PinnedBuf<mashgpu::ReplayState> h_state;
+    mashgpu::DevBuf<uint64_t> a_key, a_heap, p_key, p_heap;
+    mashgpu::DevBuf<uint32_t> a_cnt, p_cnt, bloom;
+    uint64_t cap_a = 0, cap_p = 0, cap_ph = 0;
+    uint64_t gate_t = mashgpu::EMPTY_KEY;   // host copy of the threshold as of the last read-back (an older top is a valid bound)
+    bool stopped = false;
+    cudaEvent_t replay_ev[2] = {nullptr, nullptr};
+    uint64_t dev_bytes = 0;
+};
+
+namespace mashgpu {
+
+static uint64_t reads_env(const char *name, uint64_t dflt, uint64_t lo)
 {
-    if (!ctx) return MASHGPU_ERR_INVALID;
-    MG_TRY(validate_sketch_params(ctx, params));
-    if (!out_hashes || !out_n || !out_records_used) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    const char *env = getenv(name);
+    return env ? std::max<uint64_t>(lo, strtoull(env, nullptr, 10)) : dflt;
+}
+
+template <typename T>
+static bool reads_alloc(mashgpu_reads_job *job, DevBuf<T> &b, size_t n)
+{
+    const size_t before = b.n * sizeof(T);
+    if (b.alloc(n) != cudaSuccess) return false;
+    job->dev_bytes += n * sizeof(T);
+    job->dev_bytes -= before;
+    job->ctx->reads_peak_bytes = std::max(job->ctx->reads_peak_bytes, job->dev_bytes);
+    return true;
+}
+
+// Pending tables for `extra` more entries at load <= 1/2 (grown on the device, before the replay launch that needs them).
+static int reads_reserve_pending(mashgpu_reads_job *job, uint64_t pend_n, uint64_t extra)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint64_t need = pend_n + extra;
+    if (need + 2 > job->cap_ph) {
+        uint64_t cap = std::max<uint64_t>(2 * job->cap_ph, need + 2);
+        DevBuf<uint64_t> nh;
+        if (!reads_alloc(job, nh, cap)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending heap of %llu)", (unsigned long long)cap);
+        if (pend_n) MG_CUDA(ctx, cudaMemcpyAsync(nh.p, job->p_heap.p, pend_n * 8, cudaMemcpyDeviceToDevice, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        job->dev_bytes -= job->p_heap.n * 8;
+        std::swap(job->p_heap.p, nh.p); std::swap(job->p_heap.n, nh.n);
+        job->cap_ph = cap;
+    }
+    if (2 * need + 16 > job->cap_p) {
+        uint64_t cap = std::max<uint64_t>(16, job->cap_p);
+        while (cap < 2 * need + 16) cap <<= 1;
+        DevBuf<uint64_t> nk; DevBuf<uint32_t> nc;
+        if (!reads_alloc(job, nk, cap) || !reads_alloc(job, nc, cap)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending map of %llu)", (unsigned long long)cap);
+        MG_CUDA(ctx, cudaMemsetAsync(nc.p, 0, cap * 4, st));
+        if (job->cap_p) {
+            ReplayMap from{job->p_key.p, job->p_cnt.p, job->cap_p - 1}, to{nk.p, nc.p, cap - 1};
+            reads_rehash_kernel<<<(unsigned)std::min<uint64_t>((job->cap_p + 255) / 256, (uint64_t)ctx->sm_count * 8), 256, 0, st>>>(from, to);
+            ctx->kernel_launches++;
+            MG_CUDA(ctx, cudaGetLastError());
+        }
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        job->dev_bytes -= job->p_key.n * 8 + job->p_cnt.n * 4;
+        std::swap(job->p_key.p, nk.p); std::swap(job->p_key.n, nk.n);
+        std::swap(job->p_cnt.p, nc.p); std::swap(job->p_cnt.n, nc.n);
+        job->cap_p = cap;
+    }
+    return MASHGPU_OK;
+}
+
+// Scan, sort and replay the staged buffer, stretch by stretch.
+static int reads_process_stage(mashgpu_reads_job *job)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    const mashgpu_sketch_params *p = &job->params;
+    cudaStream_t st = ctx->stream;
+    const uint64_t len = job->fill;
+    const uint64_t n_rec = job->rec_end.size();
+    if (len == 0 || job->stopped) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_stage.p, job->h_stage.p, len, cudaMemcpyHostToDevice, st));
+    if (n_rec) MG_CUDA(ctx, cudaMemcpyAsync(job->d_rec_end.p, job->rec_end.data(), n_rec * 8, cudaMemcpyHostToDevice, st));
+    ScanArgs a;
+    memset(&a, 0, sizeof a);
+    a.stream = job->d_stage.p; a.stream_len = len;
+    a.tile_tmax = job->d_tmax.p;
+    a.seed = p->seed; a.use64 = p->use64; a.preserve_case = p->preserve_case;
+    fill_byte_lut(a, p);
+    a.mode = SCAN_EVENTS; a.only_unit = -1; a.min_copies = 1;
+    a.unit_start = nullptr; a.n_units = 1; a.unit_t = &job->d_state.p->gate_t;
+    a.ev_pos = job->ev_pos.p; a.ev_hash = job->ev_hash.p; a.ev_count = &job->d_state.p->ev_count; a.ev_capacity = job->ev_cap;
+    const uint64_t ntiles = (len + SCAN_TILE - 1) / SCAN_TILE;
+    const double space = p->use64 ? 18446744073709551616.0 : 4294967296.0;
+    const uint64_t budget = std::max<uint64_t>(SCAN_TILE, job->ev_cap / 4);     // expected events per stretch
+    const uint32_t sort_bits = std::max(1u, ceil_log2(len + 1));
+    uint64_t t0 = 0, span = 0;
+    while (t0 < ntiles) {
+        if (span == 0) {                     // stretch size from the threshold as of the last read-back
+            const double f = job->gate_t == EMPTY_KEY ? 1.0 : std::max(1.0, (double)job->gate_t) / space;
+            const double windows = std::max((double)(1 << 16), (double)budget / f);
+            span = (uint64_t)std::min<double>((double)ntiles, std::ceil(windows / SCAN_TILE));
+        }
+        const uint64_t t1 = std::min(ntiles, t0 + std::max<uint64_t>(1, span));
+        reads_fill_tmax_kernel<<<(unsigned)((t1 - t0 + 255) / 256), 256, 0, st>>>(job->d_tmax.p, t0, t1, job->d_state.p);
+        ctx->kernel_launches++;
+        MG_CUDA(ctx, cudaMemsetAsync(&job->d_state.p->ev_count, 0, sizeof(unsigned long long), st));
+        a.tile_begin = t0; a.tile_end = t1;
+        MG_TRY(launch_scan(ctx, p, a, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        const ReplayState H = *job->h_state.p;
+        if (H.stopped) break;                // the previous stretch's replay reached the target coverage
+        job->gate_t = H.gate_t;
+        const uint64_t n_ev = H.ev_count;
+        if (n_ev > job->ev_cap) {            // more events than the buffer holds: split the stretch, its bytes are still resident
+            span = std::max<uint64_t>(1, (t1 - t0) / 2);
+            if (t1 - t0 == 1) return fail(ctx, MASHGPU_ERR_INVALID, "event buffer below one tile");
+            continue;
+        }
+        if (n_ev) {
+            MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(job->sort_tmp.p, job->sort_tmp_bytes, job->ev_pos.p, job->ev_pos2.p, job->ev_hash.p,
+                                                         job->ev_hash2.p, (int)n_ev, 0, (int)sort_bits, st));
+            ctx->kernel_launches += 4;
+            reads_event_meta_kernel<<<(unsigned)((n_ev + 255) / 256), 256, 0, st>>>(job->ev_pos2.p, job->ev_hash2.p, n_ev, job->d_rec_end.p, n_rec,
+                                                                                    job->rec_base, job->bloom_bits, p->use64, job->ev_bit.p);
+            ctx->kernel_launches++;
+            if (job->m > 1 && !job->bloom_bits) MG_TRY(reads_reserve_pending(job, H.pend_n, n_ev));
+            ReplayMap acc{job->a_key.p, job->a_cnt.p, job->cap_a - 1}, pend{job->p_key.p, job->p_cnt.p, job->cap_p ? job->cap_p - 1 : 0};
+            if (ctx->timing) MG_CUDA(ctx, cudaEventRecord(job->replay_ev[0], st));
+            reads_replay_kernel<<<1, 32, 0, st>>>(job->d_state.p, job->ev_pos2.p, job->ev_hash2.p, job->ev_bit.p, n_ev, job->s, job->m,
+                                                  p->target_cov, acc, job->a_heap.p, pend, job->p_heap.p, job->bloom_bits ? job->bloom.p : nullptr);
+            ctx->kernel_launches++;
+            MG_CUDA(ctx, cudaGetLastError());
+            if (ctx->timing) {
+                MG_CUDA(ctx, cudaEventRecord(job->replay_ev[1], st));
+                MG_CUDA(ctx, cudaEventSynchronize(job->replay_ev[1]));
+                float ms = 0;
+                cudaEventElapsedTime(&ms, job->replay_ev[0], job->replay_ev[1]);
+                ctx->reads_replay_ms += ms;
+            }
+            ctx->reads_events += n_ev;
+        }
+        t0 = t1;
+        span = 0;
+    }
+    return MASHGPU_OK;
+}
+
+// Hand the staged buffer to the device; keep the last k-1 bases when a record continues into the next stage.
+static int reads_flush(mashgpu_reads_job *job, bool record_continues)
+{
+    if (record_continues) {
+        const uint64_t keep = std::min<uint64_t>(job->k - 1, job->fill);
+        job->carry.assign(job->h_stage.p + job->fill - keep, job->h_stage.p + job->fill);
+    } else job->carry.clear();
+    MG_TRY(reads_process_stage(job));
+    MG_CUDA(job->ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, job->ctx->stream));
+    MG_CUDA(job->ctx, cudaStreamSynchronize(job->ctx->stream));
+    if (job->h_state.p->stopped) job->stopped = true;
+    job->rec_base += job->rec_end.size();
+    job->rec_end.clear();
+    job->fill = 0;
+    if (!job->carry.empty()) { memcpy(job->h_stage.p, job->carry.data(), job->carry.size()); job->fill = job->carry.size(); }
+    return MASHGPU_OK;
+}
+
+}  // namespace mashgpu
+
+extern "C" int mashgpu_reads_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, mashgpu_reads_job **out)
+{
+    using namespace mashgpu;
+    if (!ctx || !out) return MASHGPU_ERR_INVALID;
+    *out = nullptr;
+    MG_TRY(validate_sketch_params(ctx, params, true));
+    if (!is_dna_alphabet(params)) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reads mode is only provided for the alphabet {A,C,G,T}");
+    if (params->bloom_bytes && params->min_copies > 1)
+        return fail(ctx, MASHGPU_ERR_INVALID, "bloom_bytes (-b) and min_copies (-m) > 1 exclude each other (as in the reference CLI)");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    auto *job = new mashgpu_reads_job();
+    std::unique_ptr<mashgpu_reads_job> guard(job);
+    job->ctx = ctx;
+    job->params = *params;
+    job->s = params->sketch_size;
+    job->m = std::max(1u, params->min_copies);
+    job->k = (uint64_t)params->kmer_size;
+    job->stage_cap = reads_env("MASHGPU_READS_STAGE_BYTES", 128ull << 20, 4 * job->k + 64);
+    job->ev_cap = std::min<uint64_t>(reads_env("MASHGPU_READS_EVENT_CAP", 1ull << 21, SCAN_TILE), 1ull << 30);    // cub takes int counts
+    job->bloom_bits = params->bloom_bytes * 8;
+    ctx->reads_peak_bytes = 0;
+    cudaStream_t st = ctx->stream;
+    const uint64_t max_rec = job->stage_cap / (job->k + 1) + 2;
+    const uint64_t max_tiles = (job->stage_cap + SCAN_TILE - 1) / SCAN_TILE;
+    job->cap_a = 16;
+    while (job->cap_a < 4ull * (job->s + 2)) job->cap_a <<= 1;
+    cub::DeviceRadixSort::SortPairs(nullptr, job->sort_tmp_bytes, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint64_t *)nullptr,
+                                    (int)job->ev_cap, 0, 64, st);
+    if (job->h_stage.alloc(job->stage_cap) != cudaSuccess || job->h_state.alloc(1) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory");
+    if (!reads_alloc(job, job->d_stage, ((job->stage_cap + 15) / 16) * 16 + 64) || !reads_alloc(job, job->d_rec_end, max_rec) ||
+        !reads_alloc(job, job->d_tmax, max_tiles) || !reads_alloc(job, job->ev_pos, job->ev_cap) || !reads_alloc(job, job->ev_hash, job->ev_cap) ||
+        !reads_alloc(job, job->ev_pos2, job->ev_cap) || !reads_alloc(job, job->ev_hash2, job->ev_cap) || (job->bloom_bits && !reads_alloc(job, job->ev_bit, job->ev_cap)) ||
+        !reads_alloc(job, job->sort_tmp, job->sort_tmp_bytes) || !reads_alloc(job, job->d_state, 1) || !reads_alloc(job, job->a_key, job->cap_a) ||
+        !reads_alloc(job, job->a_cnt, job->cap_a) || !reads_alloc(job, job->a_heap, job->s + 2) ||
+        (job->bloom_bits && !reads_alloc(job, job->bloom, (std::min(params->bloom_bytes, BLOOM_MAX_BYTES) + 3) / 4)))
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (reads job)");
+    MG_CUDA(ctx, cudaMemsetAsync(job->a_cnt.p, 0, job->cap_a * 4, st));
+    if (job->bloom_bits) MG_CUDA(ctx, cudaMemsetAsync(job->bloom.p, 0, job->bloom.n * 4, st));
+    ReplayState init;
+    memset(&init, 0, sizeof init);
+    init.cur = NO_RECORD; init.gate_t = EMPTY_KEY;
+    *job->h_state.p = init;
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_state.p, job->h_state.p, sizeof init, cudaMemcpyHostToDevice, st));
+    if (job->m > 1 && !job->bloom_bits) MG_TRY(reads_reserve_pending(job, 0, 1024));
+    MG_CUDA(ctx, cudaEventCreate(&job->replay_ev[0]));
+    MG_CUDA(ctx, cudaEventCreate(&job->replay_ev[1]));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    *out = guard.release();
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_reads_feed(mashgpu_reads_job *job, uint64_t n_records, const char *const *seq, const uint64_t *len, int *stopped)
+{
+    using namespace mashgpu;
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
     if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
-    if (!is_dna_alphabet(params)) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reads mode with a target coverage is only provided for the alphabet {A,C,G,T}");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    for (uint64_t r = 0; r < n_records && !job->stopped; r++) {
+        if (len[r] < job->k) continue;                              // Sketch.cpp:1222-1226
+        if (job->fill + len[r] + 1 > job->stage_cap && job->fill) MG_TRY(reads_flush(job, false));
+        if (job->stopped) break;
+        uint64_t done = 0;
+        while (len[r] - done + 1 > job->stage_cap - job->fill) {     // longer than the stage: split with a (k-1)-base overlap
+            const uint64_t take = job->stage_cap - job->fill;
+            memcpy(job->h_stage.p + job->fill, seq[r] + done, take);
+            job->fill += take; done += take;
+            MG_TRY(reads_flush(job, true));
+            if (job->stopped) break;
+        }
+        if (job->stopped) break;
+        memcpy(job->h_stage.p + job->fill, seq[r] + done, len[r] - done);
+        job->fill += len[r] - done;
+        job->rec_end.push_back(job->fill);
+        job->h_stage.p[job->fill++] = 0;                            // separator
+        job->records++;
+    }
+    if (!job->stopped && job->fill) MG_TRY(reads_flush(job, false));
+    if (!job->stopped) {
+        reads_feed_end_kernel<<<1, 1, 0, ctx->stream>>>(job->d_state.p, job->params.target_cov);
+        ctx->kernel_launches++;
+        MG_CUDA(ctx, cudaGetLastError());
+        MG_CUDA(ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, ctx->stream));
+        MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (job->h_state.p->stopped) job->stopped = true;
+    }
+    if (stopped) *stopped = job->stopped ? 1 : 0;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_reads_finish(mashgpu_reads_job *job, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used)
+{
+    using namespace mashgpu;
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!out_hashes || !out_n || !out_records_used) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    DevBuf<uint64_t> d_hashes, d_heap; DevBuf<uint32_t> d_counts, d_n;
+    if (d_hashes.alloc(job->s) != cudaSuccess || d_heap.alloc(job->s + 2) != cudaSuccess || d_counts.alloc(job->s) != cudaSuccess || d_n.alloc(1) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (outputs)");
+    ReplayMap acc{job->a_key.p, job->a_cnt.p, job->cap_a - 1};
+    reads_emit_kernel<<<1, 1, 0, st>>>(job->d_state.p, acc, job->a_heap.p, d_heap.p, d_hashes.p, d_counts.p, d_n.p);
+    ctx->kernel_launches++;
+    MG_CUDA(ctx, cudaGetLastError());
+    uint32_t n = 0;
+    MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    if (n) MG_CUDA(ctx, cudaMemcpyAsync(out_hashes, d_hashes.p, n * 8ull, cudaMemcpyDeviceToHost, st));
+    if (n && out_counts) MG_CUDA(ctx, cudaMemcpyAsync(out_counts, d_counts.p, n * 4ull, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    *out_n = n;
+    *out_records_used = job->h_state.p->stopped ? job->h_state.p->used : job->records;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_reads_close(mashgpu_reads_job *job)
+{
+    if (!job) return MASHGPU_OK;
+    cudaSetDevice(job->ctx->device);
+    cudaStreamSynchronize(job->ctx->stream);
+    for (cudaEvent_t &e : job->replay_ev) if (e) cudaEventDestroy(e);
+    delete job;
+    return MASHGPU_OK;
+}
+
+namespace mashgpu {
+
+// Without -c and -b the heap's result does not depend on the order of the reads: the s smallest hashes seen at least m times, with
+// the heap's multiplicities (DESIGN.md 2.6), which sketch_stream_core computes in one parallel pass.  A read set that fits in half
+// of the free device memory is sketched that way in one resident stream (0.2 s against 1.2 s for the replay at -m 2 on 0.5 Gbp,
+// DESIGN.md 2.6); MASHGPU_ERR_NOMEM sends a larger one to the streaming job.
+static int sketch_reads_whole_set(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, uint64_t n_records, const char *const *seq,
+                                  const uint64_t *len, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_used)
+{
+    MG_TRY(validate_sketch_params(ctx, params, true));
+    if (!is_dna_alphabet(params)) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reads mode is only provided for the alphabet {A,C,G,T}");
+    if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const uint32_t s = params->sketch_size;
     const uint64_t k = (uint64_t)params->kmer_size;
-    const uint32_t mc = std::max(1u, params->min_copies);
-    *out_n = 0; *out_records_used = 0;
-    // kept records -> one flat device stream (record, separator, record, ...) + the end offset of every kept record
-    std::vector<uint64_t> rec_end;
-    uint64_t total = 0;
+    uint64_t total = 0, n_rec = 0;
     for (uint64_t r = 0; r < n_records; r++)
-        if (len[r] >= k) { total += len[r] + 1; rec_end.push_back(total - 1); }
-    const uint64_t n_rec = rec_end.size();
+        if (len[r] >= k) { total += len[r] + 1; n_rec++; }
     if (n_rec == 0) return MASHGPU_OK;
-    DevBuf<uint8_t> d_stream; DevBuf<uint64_t> d_hashes, d_rec_end; DevBuf<uint32_t> d_n, d_counts;
+    size_t free_b = 0, total_b = 0;
+    MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+    if (total > free_b / 2) return MASHGPU_ERR_NOMEM;
+    DevBuf<uint8_t> d_stream; DevBuf<uint64_t> d_hashes; DevBuf<uint32_t> d_n, d_counts;
     if (d_stream.alloc(((total + 15) / 16) * 16 + 64) != cudaSuccess || d_hashes.alloc(s) != cudaSuccess || d_n.alloc(1) != cudaSuccess ||
-        d_counts.alloc(s) != cudaSuccess || d_rec_end.alloc(n_rec) != cudaSuccess)
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (read set of %llu B)", (unsigned long long)total);
+        d_counts.alloc(s) != cudaSuccess)
+        return MASHGPU_ERR_NOMEM;
     {
         const size_t chunk = 64ull << 20;
         PinnedBuf<uint8_t> stage[2];
@@ -1404,10 +1828,10 @@ extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_param
         cudaEvent_t done[2];
         MG_CUDA(ctx, cudaEventCreateWithFlags(&done[0], cudaEventDisableTiming));
         MG_CUDA(ctx, cudaEventCreateWithFlags(&done[1], cudaEventDisableTiming));
-        uint64_t off = 0, fill = 0, base = 0;
+        uint64_t fill = 0, base = 0;
         int b = 0;
         bool used_ev[2] = {false, false};
-        auto flush = [&]() -> cudaError_t {
+        auto flush = [&]() -> cudaError_t {           // double-buffered: the copy of one chunk overlaps the packing of the next
             if (!fill) return cudaSuccess;
             cudaError_t e = cudaMemcpyAsync(d_stream.p + base, stage[b].p, fill, cudaMemcpyHostToDevice, st);
             if (e != cudaSuccess) return e;
@@ -1423,12 +1847,11 @@ extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_param
             if (len[r] < k) continue;
             uint64_t done_r = 0;
             while (done_r < len[r] + 1 && e == cudaSuccess) {            // the record's bytes, then its separator
-                const uint64_t room = chunk - fill, want = len[r] + 1 - done_r;
-                const uint64_t take = std::min(room, want);
+                const uint64_t take = std::min<uint64_t>(chunk - fill, len[r] + 1 - done_r);
                 const uint64_t from_seq = done_r < len[r] ? std::min(take, len[r] - done_r) : 0;
                 if (from_seq) memcpy(stage[b].p + fill, seq[r] + done_r, from_seq);
                 if (take > from_seq) stage[b].p[fill + from_seq] = 0;
-                fill += take; done_r += take; off += take;
+                fill += take; done_r += take;
                 if (fill == chunk) e = flush();
             }
         }
@@ -1436,110 +1859,40 @@ extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_param
         cudaStreamSynchronize(st);
         cudaEventDestroy(done[0]); cudaEventDestroy(done[1]);
         if (e != cudaSuccess) return fail(ctx, MASHGPU_ERR_CUDA, "upload of the read set failed: %s", cudaGetErrorString(e));
-        (void)off;
     }
-    MG_CUDA(ctx, cudaMemcpyAsync(d_rec_end.p, rec_end.data(), n_rec * 8, cudaMemcpyHostToDevice, st));
-    auto prefix_sketch = [&](uint64_t end, bool want_counts) -> int {        // ordinary sketch of the stream prefix [0, end)
-        uint64_t us[2] = {0, end};
-        SketchStream S;
-        S.d_stream = d_stream.p; S.unit_start = us; S.n_units = 1;
-        return sketch_stream_core(ctx, params, S, d_hashes.p, want_counts ? d_counts.p : nullptr, d_n.p, st, nullptr);
-    };
-    auto emit_result = [&](uint64_t used) -> int {
-        uint32_t n = 0;
-        MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 4, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-        if (n) MG_CUDA(ctx, cudaMemcpyAsync(out_hashes, d_hashes.p, n * 8ull, cudaMemcpyDeviceToHost, st));
-        if (n && out_counts) MG_CUDA(ctx, cudaMemcpyAsync(out_counts, d_counts.p, n * 4ull, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-        *out_n = n; *out_records_used = used;
-        return MASHGPU_OK;
-    };
-    if (!(params->target_cov > 0)) {
-        MG_TRY(prefix_sketch(total, out_counts != nullptr));
-        return emit_result(n_rec);
-    }
-    // ---- position bands: record boundaries near total / 2^j, down to ~2^20 positions; threshold = exact top of the heap at the band's start
-    std::vector<uint64_t> band_start(1, 0), band_t(1, EMPTY_KEY);
-    {
-        std::vector<uint64_t> cuts;
-        for (uint64_t target = total / 2; target >= (1ull << 20); target /= 2) {
-            auto it = std::upper_bound(rec_end.begin(), rec_end.end(), target);     // first record that ends after the target
-            if (it == rec_end.begin()) break;
-            const uint64_t cut = *(it - 1) + 1;                                     // the position after that record's separator
-            if (cuts.empty() || cut < cuts.back()) cuts.push_back(cut);
-        }
-        std::reverse(cuts.begin(), cuts.end());
-        for (uint64_t cut : cuts) {
-            if (cut <= band_start.back()) continue;
-            MG_TRY(prefix_sketch(cut, false));
-            uint32_t n = 0; uint64_t top = EMPTY_KEY;
-            MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 4, cudaMemcpyDeviceToHost, st));
-            MG_CUDA(ctx, cudaStreamSynchronize(st));
-            if (n == s) {
-                MG_CUDA(ctx, cudaMemcpyAsync(&top, d_hashes.p + (s - 1), 8, cudaMemcpyDeviceToHost, st));
-                MG_CUDA(ctx, cudaStreamSynchronize(st));
-            }
-            band_start.push_back(cut);
-            band_t.push_back(n == s ? top : EMPTY_KEY);                             // heap not full yet: its gate is open
-        }
-    }
-    // ---- events
-    const uint32_t n_bands = (uint32_t)band_start.size();
-    const uint64_t ev_cap = 1ull << 24;
-    DevBuf<uint64_t> d_bstart, d_bt, ev_pos, ev_hash, ev_pos2, ev_hash2, d_tmax; DevBuf<unsigned long long> ev_count; DevBuf<uint8_t> tmp;
-    const uint64_t ntiles = (total + SCAN_TILE - 1) / SCAN_TILE;
-    if (d_bstart.alloc(n_bands + 1) != cudaSuccess || d_bt.alloc(n_bands) != cudaSuccess || ev_pos.alloc(ev_cap) != cudaSuccess || ev_hash.alloc(ev_cap) != cudaSuccess ||
-        ev_pos2.alloc(ev_cap) != cudaSuccess || ev_hash2.alloc(ev_cap) != cudaSuccess || ev_count.alloc(1) != cudaSuccess || d_tmax.alloc(ntiles) != cudaSuccess)
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (event buffers)");
-    band_start.push_back(total);
-    MG_CUDA(ctx, cudaMemcpyAsync(d_bstart.p, band_start.data(), (n_bands + 1) * 8ull, cudaMemcpyHostToDevice, st));
-    MG_CUDA(ctx, cudaMemcpyAsync(d_bt.p, band_t.data(), n_bands * 8ull, cudaMemcpyHostToDevice, st));
-    MG_CUDA(ctx, cudaMemsetAsync(ev_count.p, 0, 8, st));
-    tile_tmax_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, st>>>(d_bstart.p, n_bands, d_bt.p, total, params->kmer_size, 0, ntiles, d_tmax.p, nullptr);
-    ScanArgs a;
-    memset(&a, 0, sizeof a);
-    a.stream = d_stream.p; a.stream_len = total;
-    a.tile_begin = 0; a.tile_end = ntiles; a.tile_tmax = d_tmax.p;
-    a.seed = params->seed; a.use64 = params->use64; a.preserve_case = params->preserve_case;
-    fill_byte_lut(a, params);
-    a.mode = SCAN_EVENTS; a.only_unit = -1; a.min_copies = 1;
-    a.unit_start = d_bstart.p; a.n_units = n_bands; a.unit_t = d_bt.p;
-    a.ev_pos = ev_pos.p; a.ev_hash = ev_hash.p; a.ev_count = ev_count.p; a.ev_capacity = ev_cap;
-    MG_TRY(launch_scan(ctx, params, a, st));
-    unsigned long long n_ev = 0;
-    MG_CUDA(ctx, cudaMemcpyAsync(&n_ev, ev_count.p, 8, cudaMemcpyDeviceToHost, st));
+    uint64_t us[2] = {0, total};
+    SketchStream S;
+    S.d_stream = d_stream.p; S.unit_start = us; S.n_units = 1;
+    MG_TRY(sketch_stream_core(ctx, params, S, d_hashes.p, out_counts ? d_counts.p : nullptr, d_n.p, st, nullptr));
+    uint32_t n = 0;
+    MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 4, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
-    ctx->kernel_launches++;
-    if (n_ev > ev_cap)
-        return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "-c: %llu k-mers could pass the heap's gate (more than %llu): the heap fills too slowly on this read set "
-                                                  "(very low coverage or a high -m)", n_ev, (unsigned long long)ev_cap);
-    if (n_ev) {
-        size_t tb = 0;
-        cub::DeviceRadixSort::SortPairs(nullptr, tb, ev_pos.p, ev_pos2.p, ev_hash.p, ev_hash2.p, (int)n_ev, 0, 64, st);
-        if (tmp.alloc(tb) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (sort scratch)");
-        MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tb, ev_pos.p, ev_pos2.p, ev_hash.p, ev_hash2.p, (int)n_ev, 0, 64, st));
-        ctx->kernel_launches += 8;
-    }
-    // ---- replay
-    uint64_t cap_a = 16, cap_p = 16;
-    while (cap_a < 4ull * (s + 2)) cap_a <<= 1;
-    while (cap_p < 2 * n_ev + 16) cap_p <<= 1;
-    DevBuf<uint64_t> a_key, a_heap, p_key, p_heap, d_used; DevBuf<uint32_t> a_cnt, p_cnt;
-    if (a_key.alloc(cap_a) != cudaSuccess || a_cnt.alloc(cap_a) != cudaSuccess || a_heap.alloc(s + 2) != cudaSuccess || p_key.alloc(cap_p) != cudaSuccess ||
-        p_cnt.alloc(cap_p) != cudaSuccess || p_heap.alloc(n_ev + 2) != cudaSuccess || d_used.alloc(1) != cudaSuccess)
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (replay tables)");
-    MG_CUDA(ctx, cudaMemsetAsync(a_cnt.p, 0, cap_a * 4, st));
-    MG_CUDA(ctx, cudaMemsetAsync(p_cnt.p, 0, cap_p * 4, st));
-    ReplayMap acc{a_key.p, a_cnt.p, cap_a - 1}, pend{p_key.p, p_cnt.p, cap_p - 1};
-    reads_replay_kernel<<<1, 32, 0, st>>>(ev_pos2.p, ev_hash2.p, n_ev, d_rec_end.p, n_rec, s, mc, params->target_cov, acc, a_heap.p, pend, p_heap.p,
-                                          d_hashes.p, d_counts.p, d_n.p, d_used.p);
-    ctx->kernel_launches++;
-    MG_CUDA(ctx, cudaGetLastError());
-    uint64_t used = 0;
-    MG_CUDA(ctx, cudaMemcpyAsync(&used, d_used.p, 8, cudaMemcpyDeviceToHost, st));
+    if (n) MG_CUDA(ctx, cudaMemcpyAsync(out_hashes, d_hashes.p, n * 8ull, cudaMemcpyDeviceToHost, st));
+    if (n && out_counts) MG_CUDA(ctx, cudaMemcpyAsync(out_counts, d_counts.p, n * 4ull, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
-    return emit_result(used);
+    *out_n = n; *out_used = n_rec;
+    return MASHGPU_OK;
+}
+
+}  // namespace mashgpu
+
+extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
+                                    uint64_t n_records, const char *const *seq, const uint64_t *len,
+                                    uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used)
+{
+    if (!ctx) return MASHGPU_ERR_INVALID;
+    if (!out_hashes || !out_n || !out_records_used) return mashgpu::fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *out_n = 0; *out_records_used = 0;
+    if (params && params->bloom_bytes == 0 && !(params->target_cov > 0)) {
+        const int rc = mashgpu::sketch_reads_whole_set(ctx, params, n_records, seq, len, out_hashes, out_counts, out_n, out_records_used);
+        if (rc != MASHGPU_ERR_NOMEM) return rc;                     // too large for one resident stream: stream it through a job
+    }
+    mashgpu_reads_job *job = nullptr;
+    MG_TRY(mashgpu_reads_open(ctx, params, &job));
+    int rc = mashgpu_reads_feed(job, n_records, seq, len, nullptr);
+    if (rc == MASHGPU_OK) rc = mashgpu_reads_finish(job, out_hashes, out_counts, out_n, out_records_used);
+    mashgpu_reads_close(job);
+    return rc;
 }
 
 extern "C" int mashgpu_host_pack(const mashgpu_sketch_params *params, uint64_t n_records, const char *const *seq, const uint64_t *len,

@@ -44,7 +44,8 @@ struct SketchTicket {
     std::vector<uint8_t> scan_args;         // the ScanArgs of the pass (base of the re-runs), kept opaque here
 };
 
-int validate_sketch_params(mashgpu_ctx *ctx, const mashgpu_sketch_params *p);
+// reads = the entry point is a reads-mode path (the only ones that take bloom_bytes)
+int validate_sketch_params(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, bool reads = false);
 bool is_dna_alphabet(const mashgpu_sketch_params *p);
 int sketch_stream_core(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const SketchStream &S,
                        uint64_t *d_out_hashes, uint32_t *d_out_counts, uint32_t *d_out_n, cudaStream_t st,

@@ -14,6 +14,7 @@
 #include <iostream>
 #include <chrono>
 #include <condition_variable>
+#include <functional>
 #include <list>
 #include <mutex>
 #include <thread>
@@ -80,6 +81,7 @@ void fillGpuParams(mashgpu_sketch_params &p, const Sketch::Parameters &parameter
     for (int i = 0; i < 256; i++) p.alphabet[i] = parameters.alphabet[i];
     p.min_copies = parameters.reads ? parameters.minCov : 1;      // reference Sketch.cpp:1186: MinHashHeap(use64, s, reads ? minCov : 1, ...)
     p.target_cov = parameters.reads ? parameters.targetCov : 0;   // reference Sketch.cpp:1258
+    p.bloom_bytes = parameters.reads ? parameters.memoryBound : 0; // reference Sketch.cpp:1186 (-b)
 }
 
 bool hasSuffix(string const &whole, string const &suffix)   // reference Sketch.cpp:897-905
@@ -145,7 +147,6 @@ struct Sketch::Batch {
     vector<uint32_t> unitOfRecord;
     vector<Reference> refs;          // one per unit, name/comment filled at parse time
     uint64_t bytes = 0;
-    bool reads = false;              // -r: length = genome size or estimateSetSize()
 };
 
 static const uint64_t batchBytesMax = 1ull << 28;
@@ -174,17 +175,8 @@ void Sketch::flushBatch(Batch &batch)
     vector<uint32_t> n(units), counts(parameters.counts ? units * s : 0);
     mashgpu_ctx *ctx = gpuContext();
     const double tFlush = nowMs();
-    int rc;
-    uint64_t readsUsed = 0;
-    vector<uint32_t> readCounts;
-    if (batch.reads) {
-        // one sketch of all reads (sketchFile with parameters.reads, reference Sketch.cpp:1186-1282): -m and the -c stop inside
-        readCounts.resize(s);
-        rc = mashgpu_sketch_reads(ctx, &p, ptrs.size(), ptrs.data(), lens.data(), hashes.data(), readCounts.data(), n.data(), &readsUsed);
-        if (parameters.counts) std::copy(readCounts.begin(), readCounts.end(), counts.begin());
-    } else
-        rc = mashgpu_sketch_batch(ctx, &p, ptrs.size(), ptrs.data(), lens.data(), batch.unitOfRecord.data(), units,
-                                  hashes.data(), parameters.counts ? counts.data() : 0, n.data(), lengths.data());
+    const int rc = mashgpu_sketch_batch(ctx, &p, ptrs.size(), ptrs.data(), lens.data(), batch.unitOfRecord.data(), units,
+                                        hashes.data(), parameters.counts ? counts.data() : 0, n.data(), lengths.data());
     if (traceOn()) cerr << "[mash] sketch batch: " << units << " units, " << batch.bytes / 1e6 << " MB in " << nowMs() - tFlush << " ms" << endl;
     if (rc != MASHGPU_OK) {
         cerr << "ERROR: " << mashgpu_last_error(ctx) << endl;
@@ -197,38 +189,21 @@ void Sketch::flushBatch(Batch &batch)
         for (uint32_t i = 0; i < n[u]; i++) reference.hashesSorted.push_back64(hashes[u * s + i]);
         if (parameters.counts) reference.counts.assign(counts.begin() + u * s, counts.begin() + u * s + n[u]);
         reference.countsSorted = true;
-        if (batch.reads) {   // reference Sketch.cpp:1272-1282, 1319-1328; estimateSetSize = MinHashHeap.h:45
-            double setSize = n[u] ? pow(2.0, parameters.use64 ? 64.0 : 32.0) * (double)n[u] / (double)hashes[u * s + n[u] - 1] : 0;
-            reference.length = parameters.genomeSize != 0 ? parameters.genomeSize : (uint64_t)setSize;
-            double multiplicity = 0;                         // estimateMultiplicity, MinHashHeap.h:44
-            if (n[u]) {
-                uint64_t sum = 0;
-                for (uint32_t i = 0; i < n[u]; i++) sum += readCounts[i];
-                multiplicity = (double)sum / n[u];
-            }
-            cerr << "Estimated genome size: " << setSize << endl;
-            cerr << "Estimated coverage:    " << multiplicity << endl;
-            if (parameters.targetCov > 0) cerr << "Reads used:            " << readsUsed << endl;      // reference Sketch.cpp:1324-1327
-        } else {
-            reference.length = lengths[u];
-        }
+        reference.length = lengths[u];
     }
     references.insert(references.end(), batch.refs.begin(), batch.refs.end());   // == useThreadOutput, reference Sketch.cpp:372-377
     batch = Batch();
 }
 
-static void unsupportedReadsOptions(const Sketch::Parameters &parameters)
-{
-    if (parameters.memoryBound != 0) {
-        cerr << "ERROR: the Bloom filter -b is not available in the GPU engine: it is the reference's memory-saving approximation of -m "
-                "(unique k-mers may pass, copies are not counted beyond 2); use -m, which is exact here (see DESIGN.md)." << endl;
-        exit(1);
-    }
-}
+// One unit over all records of the listed files, round robin (sketchFile, reference Sketch.cpp:1147-1336).  With `drain` (reads
+// mode) the records are handed over whenever `bytes` passes drainBytes and at the end; drain returns the number of records used
+// once the sketch is complete (the -c stop), which ends the reading and is the count of the comment, as in the reference's loop.
+typedef std::function<uint64_t(vector<mashhost::SeqBuffer> &, vector<uint32_t> &, uint64_t &)> DrainFn;
+static const uint64_t drainBytes = 1ull << 24;
 
-// One unit over all records of the listed files, round robin (sketchFile, reference Sketch.cpp:1147-1336).
 static void parseUnit(const vector<string> &fileNames, const Sketch::Parameters &parameters, Sketch::Reference &reference,
-                      vector<mashhost::SeqBuffer> &seqs, vector<uint32_t> &unitOfRecord, uint32_t unit, uint64_t &bytes)
+                      vector<mashhost::SeqBuffer> &seqs, vector<uint32_t> &unitOfRecord, uint32_t unit, uint64_t &bytes,
+                      const DrainFn &drain = DrainFn())
 {
     int count = 0;
     bool skipped = false;
@@ -275,6 +250,12 @@ static void parseUnit(const vector<string> &fileNames, const Sketch::Parameters 
         unitOfRecord.push_back(unit);
         it++;
         if (it == readers.end()) it = readers.begin();
+        if (drain && bytes >= drainBytes) {
+            if (const uint64_t used = drain(seqs, unitOfRecord, bytes)) { count = (int)used; l = -1; break; }
+        }
+    }
+    if (drain && l == -1) {
+        if (const uint64_t used = drain(seqs, unitOfRecord, bytes)) count = (int)used;
     }
     if (count > 1) {
         reference.comment.insert(0, " seqs] ");
@@ -299,13 +280,71 @@ static void parseUnit(const vector<string> &fileNames, const Sketch::Parameters 
 void Sketch::initFromReads(const vector<string> &files, const Parameters &parametersNew)   // reference Sketch.cpp:96-103
 {
     parameters = parametersNew;
-    unsupportedReadsOptions(parameters);
     gpuContextBegin();
-    Batch batch;
-    batch.reads = true;
-    batch.refs.resize(1);
-    parseUnit(files, parameters, batch.refs[0], batch.seqs, batch.unitOfRecord, 0, batch.bytes);
-    flushBatch(batch);
+    // one sketch of all reads (sketchFile with parameters.reads, reference Sketch.cpp:1186-1282), streamed through a reads job: the
+    // host holds one feed of records at a time and the device a fixed working set, whatever the size of the read set
+    mashgpu_sketch_params p;
+    fillGpuParams(p, parameters);
+    mashgpu_ctx *ctx = gpuContext();
+    mashgpu_reads_job *job = 0;
+    auto check = [&](int rc) {
+        if (rc != MASHGPU_OK) {
+            cerr << "ERROR: " << mashgpu_last_error(ctx) << endl;
+            exit(1);
+        }
+    };
+    check(mashgpu_reads_open(ctx, &p, &job));
+    bool stopped = false;
+    DrainFn drain = [&](vector<mashhost::SeqBuffer> &seqs, vector<uint32_t> &unitOfRecord, uint64_t &bytes) -> uint64_t {
+        if (!stopped && !seqs.empty()) {
+            vector<const char *> ptrs(seqs.size());
+            vector<uint64_t> lens(seqs.size());
+            for (size_t i = 0; i < seqs.size(); i++) { ptrs[i] = seqs[i].data(); lens[i] = seqs[i].size(); }
+            int st = 0;
+            check(mashgpu_reads_feed(job, seqs.size(), ptrs.data(), lens.data(), &st));
+            stopped = st != 0;
+        }
+        seqs.clear();
+        unitOfRecord.clear();
+        bytes = 0;
+        if (!stopped) return 0;
+        vector<uint64_t> hashes(p.sketch_size);                    // only the count of reads used is needed here
+        vector<uint32_t> counts(p.sketch_size);
+        uint32_t n = 0;
+        uint64_t used = 0;
+        check(mashgpu_reads_finish(job, hashes.data(), counts.data(), &n, &used));
+        return used;
+    };
+    Reference reference;
+    vector<mashhost::SeqBuffer> seqs;
+    vector<uint32_t> unitOfRecord;
+    uint64_t bytes = 0;
+    parseUnit(files, parameters, reference, seqs, unitOfRecord, 0, bytes, drain);
+    const uint32_t s = p.sketch_size;
+    vector<uint64_t> hashes(s);
+    vector<uint32_t> counts(s);
+    uint32_t n = 0;
+    uint64_t readsUsed = 0;
+    check(mashgpu_reads_finish(job, hashes.data(), counts.data(), &n, &readsUsed));
+    mashgpu_reads_close(job);
+    reference.hashesSorted.setUse64(parameters.use64);             // == setMinHashesForReference, reference Sketch.cpp:1139-1145
+    reference.hashesSorted.clear();
+    for (uint32_t i = 0; i < n; i++) reference.hashesSorted.push_back64(hashes[i]);
+    if (parameters.counts) reference.counts.assign(counts.begin(), counts.begin() + n);
+    reference.countsSorted = true;
+    // reference Sketch.cpp:1272-1282, 1319-1328; estimateSetSize = MinHashHeap.h:45
+    const double setSize = n ? pow(2.0, parameters.use64 ? 64.0 : 32.0) * (double)n / (double)hashes[n - 1] : 0;
+    reference.length = parameters.genomeSize != 0 ? parameters.genomeSize : (uint64_t)setSize;
+    double multiplicity = 0;                                        // estimateMultiplicity, MinHashHeap.h:44
+    if (n) {
+        uint64_t sum = 0;
+        for (uint32_t i = 0; i < n; i++) sum += counts[i];
+        multiplicity = (double)sum / n;
+    }
+    cerr << "Estimated genome size: " << setSize << endl;
+    cerr << "Estimated coverage:    " << multiplicity << endl;
+    if (parameters.targetCov > 0) cerr << "Reads used:            " << readsUsed << endl;      // reference Sketch.cpp:1324-1327
+    references.push_back(reference);
     createIndex();
 }
 
