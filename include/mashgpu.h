@@ -101,10 +101,11 @@ int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
  * Sketch.cpp:1186-1282): all records in the order given (the caller interleaves several files round robin as Sketch.cpp:1202-1270
  * does).  With target_cov > 0 the result is the heap as it stood after the first kept record that brought estimateMultiplicity()
  * to the target (Sketch.cpp:1258-1262) and *out_records_used (the "Reads used" line, :1324-1327) is the number of kept records up
- * to and including it; otherwise all kept records are used.  With target_cov > 0 or bloom_bytes, or when the set does not fit in half
- * of the free device memory, this is mashgpu_reads_open + one mashgpu_reads_feed + mashgpu_reads_finish + mashgpu_reads_close;
- * otherwise the result does not depend on the order of the reads and the whole set is sketched in one parallel pass (same result,
- * faster: DESIGN.md 2.6).  out_counts nullable.  DNA alphabet only. */
+ * to and including it; otherwise all kept records are used.  With target_cov > 0 or bloom_bytes, or with min_copies > 1 when the set
+ * does not fit in half of the free device memory, this is mashgpu_reads_open + one mashgpu_reads_feed + mashgpu_reads_finish +
+ * mashgpu_reads_close; otherwise the result does not depend on the order of the reads and the whole set is sketched in one parallel
+ * pass (same result, faster: DESIGN.md 2.6), or, beyond that memory limit, streamed through a unit job (mashgpu_unit_*).
+ * out_counts nullable.  DNA alphabet only. */
 int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
                          uint64_t n_records, const char *const *seq, const uint64_t *len,
                          uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used);
@@ -126,6 +127,28 @@ int mashgpu_reads_feed(mashgpu_reads_job *job, uint64_t n_records, const char *c
 /* The sketch (sketch_size slots, ascending) and the kept records used, as mashgpu_sketch_reads returns them.  out_counts nullable. */
 int mashgpu_reads_finish(mashgpu_reads_job *job, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_records_used);
 int mashgpu_reads_close(mashgpu_reads_job *job);
+
+/* One sketch unit of any size as a streaming job: exactly one unit of mashgpu_sketch_batch (one sketchFile job with minCov 1 and no
+ * Bloom filter, Sketch.cpp:1147-1336), with records fed in order, in any number of feeds; the result does not depend on how they are
+ * split.  Every configuration mashgpu_sketch_batch takes (DNA and byte alphabets, k 1..32, any sketch size, either case mode,
+ * canonical or not) except min_copies > 1, target_cov > 0 and bloom_bytes, which return MASHGPU_ERR_UNSUPPORTED (they need the
+ * order of the records: mashgpu_reads_*).  The stream is sketched stage by stage -- with the running s-th smallest hash as the
+ * threshold once s hashes are held -- and each stage's bottom-s merged into the running one, counts summed, the reference's
+ * top-of-heap count included (DESIGN.md 2.7).  Device memory is fixed at open by the parameters: two staging buffers
+ * (MASHGPU_UNIT_STAGE_BYTES each, default 128 MiB; the copy of one overlaps the scan of the other), a candidate table sized from s
+ * and the stage, and O(s) state.  mashgpu_sketch_batch routes a unit whose stream exceeds half of the free device memory here,
+ * and mashgpu_sketch_reads a read set without -m > 1, -c or -b beyond that limit. */
+typedef struct mashgpu_unit_job mashgpu_unit_job;
+int mashgpu_unit_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, mashgpu_unit_job **job);
+/* The next n_records records of the unit.  Records shorter than kmer_size are skipped and not counted; a record longer than a stage
+ * is split with a (kmer_size-1)-base overlap and each of its windows is counted once.  Returns once the caller's buffers are free.
+ * MASHGPU_ERR_INVALID after mashgpu_unit_finish. */
+int mashgpu_unit_feed(mashgpu_unit_job *job, uint64_t n_records, const char *const *seq, const uint64_t *len);
+/* The unit's sketch (out_hashes: sketch_size slots, ascending; out_counts nullable: the HashSet counts), *out_length = sum of the kept
+ * records' lengths, *out_records = their number.  May be called again; no feed is accepted after it. */
+int mashgpu_unit_finish(mashgpu_unit_job *job, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length,
+                        uint64_t *out_records);
+int mashgpu_unit_close(mashgpu_unit_job *job);
 
 /* Same computation on a sequence stream already resident in device memory.  d_stream holds the units back to
  * back; unit u occupies bytes [unit_start[u], unit_start[u+1]) (host array of n_units+1 offsets); records inside
@@ -391,6 +414,8 @@ typedef struct mashgpu_stats {
     uint64_t reads_events;         /* k-mers replayed through the heap by reads jobs */
     double reads_replay_ms;        /* accumulated device time of the replay kernel of reads jobs (with timing on) */
     uint64_t reads_peak_device_bytes;  /* largest device footprint of the last reads job opened (not cleared by reset) */
+    uint64_t unit_stages;          /* stages merged by unit jobs (mashgpu_unit_*, and the units and read sets routed to them) */
+    uint64_t unit_peak_device_bytes;   /* largest device footprint of the last unit job opened (not cleared by reset) */
 } mashgpu_stats;
 /* timing != 0 brackets the dominant kernels with CUDA events (adds a sync at mashgpu_get_stats). */
 int mashgpu_set_timing(mashgpu_ctx *ctx, int timing);

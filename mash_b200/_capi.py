@@ -54,7 +54,8 @@ class Stats(C.Structure):
     _fields_ = [("kernel_launches", C.c_uint64), ("scan_kernel_ms", C.c_double), ("scan_kernel_launches", C.c_uint64),
                 ("dist_kernel_ms", C.c_double), ("dist_kernel_launches", C.c_uint64), ("exact_reruns", C.c_uint64),
                 ("translate_kernel_ms", C.c_double), ("translate_kernel_launches", C.c_uint64), ("taxonomy_ms", C.c_double),
-                ("reads_events", C.c_uint64), ("reads_replay_ms", C.c_double), ("reads_peak_device_bytes", C.c_uint64)]
+                ("reads_events", C.c_uint64), ("reads_replay_ms", C.c_double), ("reads_peak_device_bytes", C.c_uint64),
+                ("unit_stages", C.c_uint64), ("unit_peak_device_bytes", C.c_uint64)]
 
 
 class TaxRow(C.Structure):
@@ -100,6 +101,10 @@ def load_library():
     L.mashgpu_reads_feed.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, u64p, C.POINTER(C.c_int)]
     L.mashgpu_reads_finish.argtypes = [C.c_void_p, u64p, u32p, u32p, u64p]
     L.mashgpu_reads_close.argtypes = [C.c_void_p]
+    L.mashgpu_unit_open.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.POINTER(C.c_void_p)]
+    L.mashgpu_unit_feed.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, u64p]
+    L.mashgpu_unit_finish.argtypes = [C.c_void_p, u64p, u32p, u32p, u64p, u64p]
+    L.mashgpu_unit_close.argtypes = [C.c_void_p]
     L.mashgpu_sketch_batch_packed.argtypes = [C.c_void_p, C.POINTER(SketchParams), u64p, C.c_uint64, u64p, C.c_uint64, u64p, C.c_uint64, u64p, u32p, u32p]
     L.mashgpu_host_pack.argtypes = [C.POINTER(SketchParams), C.c_uint64, C.c_void_p, u64p, C.c_int, u64p, u64p, C.c_uint64, u64p]
     L.mashgpu_hash_windows.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.c_void_p, C.c_uint64, u64p, u8p]
@@ -243,6 +248,10 @@ class Engine:
     def reads_open(self, p):
         """A streaming `mash sketch -r` job: feed the read set in any number of pieces, then finish()."""
         return ReadsJob(self, p)
+
+    def unit_open(self, p):
+        """A streaming sketch unit (one unit of Engine.sketch, any size): feed its records in any number of pieces, then finish()."""
+        return UnitJob(self, p)
 
     def host_pack(self, records, p, threads=1):
         """records -> (codes u64[ceil(L/32)], runs u64[n, 2], record_start u64[n_records + 1]) in the packed stream format
@@ -454,6 +463,35 @@ class ReadsJob:
     def close(self):
         if self.h:
             self.eng.lib.mashgpu_reads_close(self.h)
+            self.h = None
+
+
+class UnitJob:
+    def __init__(self, eng, p):
+        self.eng = eng
+        self.p = p
+        h = C.c_void_p()
+        eng._check(eng.lib.mashgpu_unit_open(eng.h, C.byref(p), C.byref(h)))
+        self.h = h
+
+    def feed(self, records):
+        """The next records of the unit, in order."""
+        bufs = [_as_u8(r) for r in records]
+        ptrs = (C.c_void_p * max(1, len(bufs)))(*[b.ctypes.data if b.size else None for b in bufs])
+        lens = np.array([b.size for b in bufs], dtype=np.uint64)
+        self.eng._check(self.eng.lib.mashgpu_unit_feed(self.h, len(bufs), C.cast(ptrs, C.c_void_p), _p(lens, u64p)))
+
+    def finish(self, counts=True):
+        """(hashes ascending, counts | None, length, records): one row of Engine.sketch with the kept records' number."""
+        s = self.p.sketch_size
+        out = np.zeros(s, np.uint64); out_c = np.zeros(s, np.uint32) if counts else None
+        n = C.c_uint32(0); length = C.c_uint64(0); recs = C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_unit_finish(self.h, _p(out, u64p), _p(out_c, u32p), C.byref(n), C.byref(length), C.byref(recs)))
+        return out[:n.value].copy(), (out_c[:n.value].copy() if counts else None), length.value, recs.value
+
+    def close(self):
+        if self.h:
+            self.eng.lib.mashgpu_unit_close(self.h)
             self.h = None
 
 

@@ -114,10 +114,13 @@ extern "C" int mashgpu_get_stats(mashgpu_ctx *ctx, mashgpu_stats *out, int reset
     out->reads_events = ctx->reads_events;
     out->reads_replay_ms = ctx->reads_replay_ms;
     out->reads_peak_device_bytes = ctx->reads_peak_bytes;
+    out->unit_stages = ctx->unit_stages;
+    out->unit_peak_device_bytes = ctx->unit_peak_bytes;
     if (reset) {
         ctx->kernel_launches = ctx->scan_launches = ctx->dist_launches = ctx->exact_reruns = ctx->translate_launches = 0;
         ctx->scan_ms = ctx->dist_ms = ctx->translate_ms = ctx->tax_ms = 0;
         ctx->reads_events = 0;
+        ctx->unit_stages = 0;
         ctx->reads_replay_ms = 0;
     }
     return MASHGPU_OK;

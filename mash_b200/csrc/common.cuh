@@ -58,6 +58,7 @@ struct mashgpu_ctx {
     std::vector<mashgpu::EventPair> scan_events, dist_events, translate_events, tax_events;
     uint64_t reads_events = 0, reads_peak_bytes = 0;   // reads jobs: events replayed; device footprint of the last job
     double reads_replay_ms = 0;
+    uint64_t unit_stages = 0, unit_peak_bytes = 0;     // unit jobs: stages merged; device footprint of the last job
     // sketch_stream_core scratch
     mashgpu::Scratch sc_start, sc_t, sc_off, sc_log2, sc_flags, sc_maxhash, sc_keys, sc_cnt, sc_tmax, sc_tunit, sc_first, sc_last, sc_qtarget, sc_qtstar;
     // mashgpu_sketch_batch: wave stream buffers and outputs

@@ -754,6 +754,17 @@ namespace {
 
 struct Wave { uint64_t unit_begin, unit_end, rec_begin, rec_end, bytes; };
 
+}  // namespace
+
+namespace mashgpu {
+static int unit_stream_limit(mashgpu_ctx *ctx, uint64_t *limit);
+static int sketch_unit_streamed(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, uint64_t n_records, const char *const *seq,
+                                const uint64_t *len, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length,
+                                uint64_t *out_records);
+}  // namespace mashgpu
+
+namespace {
+
 constexpr uint64_t WAVE_BYTES = 1ull << 30;        // stream bytes per wave (the two feed paths share the waves of a batch: finer than 2 GiB balances better)
 constexpr uint32_t SEP_LIST_MAX = 1u << 15;        // directly copied records per wave whose separators go through the list
 constexpr uint64_t DIRECT_COPY_MIN = 1ull << 18;   // records at least this long are copied straight from the caller's buffer
@@ -798,6 +809,42 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
                 if (len[r] >= k) L += len[r];
             out_length[u] = L;
         }
+
+    // a unit whose stream does not fit on the device at once (the whole-set rule of mashgpu_sketch_reads) streams through a unit job
+    // fed from the caller's buffers; the runs of units between such units take the waves below (DESIGN.md 2.7)
+    if (params->min_copies <= 1) {
+        uint64_t limit = 0;
+        MG_TRY(unit_stream_limit(ctx, &limit));
+        bool any = false;
+        for (uint64_t u = 0; u < n_units; u++) any |= unit_bytes[u] > limit;
+        if (any) {
+            mashgpu_sketch_params q = *params;
+            q.target_cov = 0;                    // not a reads-mode setting: ignored here as in the waves
+            std::vector<uint32_t> uor;
+            for (uint64_t u0 = 0; u0 < n_units;) {
+                const uint64_t rb = unit_rec_begin[u0];
+                if (unit_bytes[u0] > limit) {
+                    MG_TRY(sketch_unit_streamed(ctx, &q, unit_rec_begin[u0 + 1] - rb, seq + rb, len + rb, out_hashes + u0 * s,
+                                                out_counts ? out_counts + u0 * s : nullptr, out_n + u0, out_length ? out_length + u0 : nullptr, nullptr));
+                    u0++;
+                    continue;
+                }
+                uint64_t u1 = u0 + 1;
+                while (u1 < n_units && unit_bytes[u1] <= limit) u1++;
+                const uint64_t re = unit_rec_begin[u1];
+                const uint32_t *sub = nullptr;
+                if (unit_of_record) {
+                    uor.resize(re - rb);
+                    for (uint64_t r = rb; r < re; r++) uor[r - rb] = unit_of_record[r] - (uint32_t)u0;
+                    sub = uor.data();
+                }
+                MG_TRY(mashgpu_sketch_batch(ctx, params, re - rb, seq + rb, len + rb, sub, u1 - u0, out_hashes + u0 * s,
+                                            out_counts ? out_counts + u0 * s : nullptr, out_n + u0, out_length ? out_length + u0 : nullptr));
+                u0 = u1;
+            }
+            return MASHGPU_OK;
+        }
+    }
 
     // waves: cut by stream bytes and by unit count (outputs and candidate tables grow with the number of units, not with their
     // length -- a multi-FASTA of millions of short records must not allocate units x s outputs at once)
@@ -1479,6 +1526,71 @@ __global__ void reads_emit_kernel(const ReplayState *state, ReplayMap acc, const
     }
 }
 
+// Pinned staging of whole records for the streaming jobs (reads and unit jobs): kept records back to back, one separator byte after
+// each, and the offsets of those separators.  A record longer than the space left is split; the buffer after the split starts with
+// its last k-1 bases (the carry), so each window of the record lies whole in exactly one stage.  With two buffers the caller fills
+// one while the other is still being copied to the device.
+struct RecordStage {
+    PinnedBuf<uint8_t> buf[2];
+    int nbuf = 1, cur = 0;
+    uint64_t cap = 0, k = 0, fill = 0;
+    uint64_t records = 0, bases = 0;    // kept records staged so far and the sum of their lengths
+    std::vector<uint64_t> rec_end;      // separator offsets of the records that end in the current buffer
+    std::vector<uint8_t> carry;         // the last k-1 bases of a record split across stages
+    uint8_t *h() { return buf[cur].p; }
+    cudaError_t open(uint64_t cap_, uint64_t k_, int nbuf_)
+    {
+        cap = cap_; k = k_; nbuf = nbuf_;
+        for (int b = 0; b < nbuf; b++)
+            if (const cudaError_t e = buf[b].alloc(cap)) return e;
+        return cudaSuccess;
+    }
+};
+
+// Hand the current buffer (fill bytes, rec_end) to `process`; keep the last k-1 bases when a record continues into the next stage.
+template <typename F>
+static int stage_flush(RecordStage &S, bool record_continues, F &&process)
+{
+    if (record_continues) {
+        const uint64_t keep = std::min<uint64_t>(S.k - 1, S.fill);
+        S.carry.assign(S.h() + S.fill - keep, S.h() + S.fill);
+    } else S.carry.clear();
+    MG_TRY(process());
+    S.rec_end.clear();
+    S.fill = 0;
+    S.cur = (S.cur + 1) % S.nbuf;
+    if (!S.carry.empty()) { memcpy(S.h(), S.carry.data(), S.carry.size()); S.fill = S.carry.size(); }
+    return MASHGPU_OK;
+}
+
+// Stage the next records in order (those shorter than k are skipped, Sketch.cpp:1222-1226); flush(record_continues) runs whenever
+// the buffer is full, and staging ends early once stopped() holds.
+template <typename Flush, typename Stopped>
+static int stage_records(RecordStage &S, uint64_t n_records, const char *const *seq, const uint64_t *len, Flush &&flush, Stopped &&stopped)
+{
+    for (uint64_t r = 0; r < n_records && !stopped(); r++) {
+        if (len[r] < S.k) continue;
+        if (S.fill + len[r] + 1 > S.cap && S.fill) MG_TRY(flush(false));
+        if (stopped()) break;
+        uint64_t done = 0;
+        while (len[r] - done + 1 > S.cap - S.fill) {           // longer than the stage: split with a (k-1)-base overlap
+            const uint64_t take = S.cap - S.fill;
+            memcpy(S.h() + S.fill, seq[r] + done, take);
+            S.fill += take; done += take;
+            MG_TRY(flush(true));
+            if (stopped()) break;
+        }
+        if (stopped()) break;
+        memcpy(S.h() + S.fill, seq[r] + done, len[r] - done);
+        S.fill += len[r] - done;
+        S.rec_end.push_back(S.fill);
+        S.h()[S.fill++] = 0;                                    // separator
+        S.records++;
+        S.bases += len[r];
+    }
+    return MASHGPU_OK;
+}
+
 }  // namespace mashgpu
 
 struct mashgpu_reads_job {
@@ -1486,16 +1598,12 @@ struct mashgpu_reads_job {
     mashgpu_sketch_params params{};
     uint32_t s = 0, m = 1;
     uint64_t k = 0;
-    uint64_t stage_cap = 0, ev_cap = 0, bloom_bits = 0;
-    // staging: one pinned buffer, its device copy and the record ends (offsets of their separators) inside it
-    mashgpu::PinnedBuf<uint8_t> h_stage;
+    uint64_t ev_cap = 0, bloom_bits = 0;
+    // staging: one pinned buffer (records: kept records fed, the ones before the stop once stopped), its device copy
+    mashgpu::RecordStage stage;
     mashgpu::DevBuf<uint8_t> d_stage;
-    uint64_t fill = 0;
-    std::vector<uint64_t> rec_end;
     mashgpu::DevBuf<uint64_t> d_rec_end, d_tmax;
     uint64_t rec_base = 0;          // kept records that ended in earlier stages
-    uint64_t records = 0;           // kept records fed (the ones before the stop, once stopped)
-    std::vector<uint8_t> carry;     // the last k-1 bases of a record split across stages
     // events
     mashgpu::DevBuf<uint64_t> ev_pos, ev_hash, ev_pos2, ev_hash2;
     mashgpu::DevBuf<uint32_t> ev_bit;
@@ -1575,11 +1683,11 @@ static int reads_process_stage(mashgpu_reads_job *job)
     mashgpu_ctx *ctx = job->ctx;
     const mashgpu_sketch_params *p = &job->params;
     cudaStream_t st = ctx->stream;
-    const uint64_t len = job->fill;
-    const uint64_t n_rec = job->rec_end.size();
+    const uint64_t len = job->stage.fill;
+    const uint64_t n_rec = job->stage.rec_end.size();
     if (len == 0 || job->stopped) return MASHGPU_OK;
-    MG_CUDA(ctx, cudaMemcpyAsync(job->d_stage.p, job->h_stage.p, len, cudaMemcpyHostToDevice, st));
-    if (n_rec) MG_CUDA(ctx, cudaMemcpyAsync(job->d_rec_end.p, job->rec_end.data(), n_rec * 8, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_stage.p, job->stage.h(), len, cudaMemcpyHostToDevice, st));
+    if (n_rec) MG_CUDA(ctx, cudaMemcpyAsync(job->d_rec_end.p, job->stage.rec_end.data(), n_rec * 8, cudaMemcpyHostToDevice, st));
     ScanArgs a;
     memset(&a, 0, sizeof a);
     a.stream = job->d_stage.p; a.stream_len = len;
@@ -1649,19 +1757,14 @@ static int reads_process_stage(mashgpu_reads_job *job)
 // Hand the staged buffer to the device; keep the last k-1 bases when a record continues into the next stage.
 static int reads_flush(mashgpu_reads_job *job, bool record_continues)
 {
-    if (record_continues) {
-        const uint64_t keep = std::min<uint64_t>(job->k - 1, job->fill);
-        job->carry.assign(job->h_stage.p + job->fill - keep, job->h_stage.p + job->fill);
-    } else job->carry.clear();
-    MG_TRY(reads_process_stage(job));
-    MG_CUDA(job->ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, job->ctx->stream));
-    MG_CUDA(job->ctx, cudaStreamSynchronize(job->ctx->stream));
-    if (job->h_state.p->stopped) job->stopped = true;
-    job->rec_base += job->rec_end.size();
-    job->rec_end.clear();
-    job->fill = 0;
-    if (!job->carry.empty()) { memcpy(job->h_stage.p, job->carry.data(), job->carry.size()); job->fill = job->carry.size(); }
-    return MASHGPU_OK;
+    return stage_flush(job->stage, record_continues, [&]() -> int {
+        MG_TRY(reads_process_stage(job));
+        MG_CUDA(job->ctx, cudaMemcpyAsync(job->h_state.p, job->d_state.p, sizeof(ReplayState), cudaMemcpyDeviceToHost, job->ctx->stream));
+        MG_CUDA(job->ctx, cudaStreamSynchronize(job->ctx->stream));
+        if (job->h_state.p->stopped) job->stopped = true;
+        job->rec_base += job->stage.rec_end.size();
+        return MASHGPU_OK;
+    });
 }
 
 }  // namespace mashgpu
@@ -1683,20 +1786,20 @@ extern "C" int mashgpu_reads_open(mashgpu_ctx *ctx, const mashgpu_sketch_params 
     job->s = params->sketch_size;
     job->m = std::max(1u, params->min_copies);
     job->k = (uint64_t)params->kmer_size;
-    job->stage_cap = reads_env("MASHGPU_READS_STAGE_BYTES", 128ull << 20, 4 * job->k + 64);
+    const uint64_t stage_cap = reads_env("MASHGPU_READS_STAGE_BYTES", 128ull << 20, 4 * job->k + 64);
     job->ev_cap = std::min<uint64_t>(reads_env("MASHGPU_READS_EVENT_CAP", 1ull << 21, SCAN_TILE), 1ull << 30);    // cub takes int counts
     job->bloom_bits = params->bloom_bytes * 8;
     ctx->reads_peak_bytes = 0;
     cudaStream_t st = ctx->stream;
-    const uint64_t max_rec = job->stage_cap / (job->k + 1) + 2;
-    const uint64_t max_tiles = (job->stage_cap + SCAN_TILE - 1) / SCAN_TILE;
+    const uint64_t max_rec = stage_cap / (job->k + 1) + 2;
+    const uint64_t max_tiles = (stage_cap + SCAN_TILE - 1) / SCAN_TILE;
     job->cap_a = 16;
     while (job->cap_a < 4ull * (job->s + 2)) job->cap_a <<= 1;
     cub::DeviceRadixSort::SortPairs(nullptr, job->sort_tmp_bytes, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint64_t *)nullptr, (uint64_t *)nullptr,
                                     (int)job->ev_cap, 0, 64, st);
-    if (job->h_stage.alloc(job->stage_cap) != cudaSuccess || job->h_state.alloc(1) != cudaSuccess)
+    if (job->stage.open(stage_cap, job->k, 1) != cudaSuccess || job->h_state.alloc(1) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory");
-    if (!reads_alloc(job, job->d_stage, ((job->stage_cap + 15) / 16) * 16 + 64) || !reads_alloc(job, job->d_rec_end, max_rec) ||
+    if (!reads_alloc(job, job->d_stage, ((stage_cap + 15) / 16) * 16 + 64) || !reads_alloc(job, job->d_rec_end, max_rec) ||
         !reads_alloc(job, job->d_tmax, max_tiles) || !reads_alloc(job, job->ev_pos, job->ev_cap) || !reads_alloc(job, job->ev_hash, job->ev_cap) ||
         !reads_alloc(job, job->ev_pos2, job->ev_cap) || !reads_alloc(job, job->ev_hash2, job->ev_cap) || (job->bloom_bits && !reads_alloc(job, job->ev_bit, job->ev_cap)) ||
         !reads_alloc(job, job->sort_tmp, job->sort_tmp_bytes) || !reads_alloc(job, job->d_state, 1) || !reads_alloc(job, job->a_key, job->cap_a) ||
@@ -1725,26 +1828,8 @@ extern "C" int mashgpu_reads_feed(mashgpu_reads_job *job, uint64_t n_records, co
     mashgpu_ctx *ctx = job->ctx;
     if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    for (uint64_t r = 0; r < n_records && !job->stopped; r++) {
-        if (len[r] < job->k) continue;                              // Sketch.cpp:1222-1226
-        if (job->fill + len[r] + 1 > job->stage_cap && job->fill) MG_TRY(reads_flush(job, false));
-        if (job->stopped) break;
-        uint64_t done = 0;
-        while (len[r] - done + 1 > job->stage_cap - job->fill) {     // longer than the stage: split with a (k-1)-base overlap
-            const uint64_t take = job->stage_cap - job->fill;
-            memcpy(job->h_stage.p + job->fill, seq[r] + done, take);
-            job->fill += take; done += take;
-            MG_TRY(reads_flush(job, true));
-            if (job->stopped) break;
-        }
-        if (job->stopped) break;
-        memcpy(job->h_stage.p + job->fill, seq[r] + done, len[r] - done);
-        job->fill += len[r] - done;
-        job->rec_end.push_back(job->fill);
-        job->h_stage.p[job->fill++] = 0;                            // separator
-        job->records++;
-    }
-    if (!job->stopped && job->fill) MG_TRY(reads_flush(job, false));
+    MG_TRY(stage_records(job->stage, n_records, seq, len, [&](bool cont) { return reads_flush(job, cont); }, [&] { return job->stopped; }));
+    if (!job->stopped && job->stage.fill) MG_TRY(reads_flush(job, false));
     if (!job->stopped) {
         reads_feed_end_kernel<<<1, 1, 0, ctx->stream>>>(job->d_state.p, job->params.target_cov);
         ctx->kernel_launches++;
@@ -1780,7 +1865,7 @@ extern "C" int mashgpu_reads_finish(mashgpu_reads_job *job, uint64_t *out_hashes
     if (n && out_counts) MG_CUDA(ctx, cudaMemcpyAsync(out_counts, d_counts.p, n * 4ull, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     *out_n = n;
-    *out_records_used = job->h_state.p->stopped ? job->h_state.p->used : job->records;
+    *out_records_used = job->h_state.p->stopped ? job->h_state.p->used : job->stage.records;
     return MASHGPU_OK;
 }
 
@@ -1790,6 +1875,371 @@ extern "C" int mashgpu_reads_close(mashgpu_reads_job *job)
     cudaSetDevice(job->ctx->device);
     cudaStreamSynchronize(job->ctx->stream);
     for (cudaEvent_t &e : job->replay_ev) if (e) cudaEventDestroy(e);
+    delete job;
+    return MASHGPU_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Streaming unit job (mashgpu_unit_*, DESIGN.md 2.7): one sketchFile unit with minCov 1 and no Bloom filter, of any size, in device
+// memory fixed by the parameters.  The bottom-s of a set does not depend on order, so each stage of the stream is sketched on its
+// own -- the one-unit pass of sketch_stream_core, with the running s-th smallest hash as the threshold once s hashes are held --
+// and its bottom-s (count, first and last position of each hash) is merged into the running state: the bottom-s hashes, their
+// summed counts, and the current top's count at positions <= t* (tests/unit_stream_model.py restates the merge).
+// ---------------------------------------------------------------------------------------------------------
+namespace mashgpu {
+
+// The stage's bottom-s, ascending, with the count and the global first / last position of each hash.
+__global__ void unit_emit_kernel(const uint64_t *sorted, uint32_t m, const uint64_t *keys, const uint32_t *cnt, const uint64_t *first,
+                                 const uint64_t *last, uint32_t log2cap, uint64_t base, uint64_t *c_key, uint32_t *c_cnt, uint64_t *c_first,
+                                 uint64_t *c_last)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint64_t key = sorted[i];
+    const int64_t slot = table_find(keys, log2cap, key);
+    c_key[i] = key;
+    c_cnt[i] = cnt[slot];
+    c_first[i] = base + first[slot];
+    c_last[i] = base + last[slot];
+}
+
+}  // namespace mashgpu
+
+struct mashgpu_unit_job {
+    mashgpu_ctx *ctx = nullptr;
+    mashgpu_sketch_params params{};
+    uint32_t s = 0;
+    mashgpu::RecordStage stage;                 // two pinned buffers: one fills while the other is copied
+    mashgpu::DevBuf<uint8_t> d_stage[2];
+    cudaEvent_t copied[2] = {nullptr, nullptr};
+    // the stage in flight: scanned (or being scanned), not merged yet
+    int pending = -1;                           // its buffer, -1 = none
+    uint64_t pend_len = 0, pend_base = 0;       // its length and the global stream position of its first byte
+    uint64_t pend_t = 0;                        // its threshold
+    uint32_t pend_lg = 0;                       // log2 of its table's capacity
+    double pend_factor = 0;                     // its plan_unit survivor factor
+    uint64_t next_base = 0;                     // global stream position of the next stage's first byte
+    // candidate table of one stage, its compaction and sort
+    mashgpu::DevBuf<uint64_t> t_keys, t_first, t_last, comp, sorted, c_key, c_first, c_last, d_meta;   // d_meta: [threshold, 0]
+    mashgpu::DevBuf<uint32_t> t_cnt, c_cnt, d_small;       // d_small: [log2, flags, maxhash, recount]
+    mashgpu::DevBuf<unsigned long long> d_n;
+    mashgpu::DevBuf<uint8_t> sort_tmp;
+    size_t sort_tmp_bytes = 0;
+    uint32_t lg_cap = 0;                        // capacity of the table buffers
+    // running state
+    std::vector<uint64_t> keys;                 // bottom-s so far, ascending
+    std::vector<uint32_t> tot;                  // their counts summed over the stages
+    uint32_t top_at_tstar = 0;                  // the top's count at positions <= t*
+    bool finished = false;
+    uint64_t dev_bytes = 0;
+};
+
+namespace mashgpu {
+
+template <typename T>
+static bool unit_alloc(mashgpu_unit_job *job, DevBuf<T> &b, size_t n)
+{
+    const size_t before = b.n * sizeof(T);
+    if (b.alloc(n) != cudaSuccess) return false;
+    job->dev_bytes += n * sizeof(T);
+    job->dev_bytes -= before;
+    job->ctx->unit_peak_bytes = std::max(job->ctx->unit_peak_bytes, job->dev_bytes);
+    return true;
+}
+
+// Table, compaction and sort buffers for 2^lg slots (grown only by a re-run that needs a larger table).
+static int unit_reserve_table(mashgpu_unit_job *job, uint32_t lg)
+{
+    if (lg <= job->lg_cap) return MASHGPU_OK;
+    const uint64_t cap = 1ull << lg;
+    size_t tmp = 0;
+    cub::DeviceRadixSort::SortKeys(nullptr, tmp, (uint64_t *)nullptr, (uint64_t *)nullptr, (int)cap, 0, 64, job->ctx->stream);
+    if (!unit_alloc(job, job->t_keys, cap) || !unit_alloc(job, job->t_cnt, cap) || !unit_alloc(job, job->t_first, cap) ||
+        !unit_alloc(job, job->t_last, cap) || !unit_alloc(job, job->comp, cap) || !unit_alloc(job, job->sorted, cap) ||
+        !unit_alloc(job, job->sort_tmp, tmp))
+        return fail(job->ctx, MASHGPU_ERR_NOMEM, "out of device memory (unit job table of %llu slots)", (unsigned long long)cap);
+    job->sort_tmp_bytes = tmp;
+    job->lg_cap = lg;
+    return MASHGPU_OK;
+}
+
+// Threshold and table of the pending stage for a survivor factor; once s hashes are held nothing above the running top can enter.
+static int unit_plan(mashgpu_unit_job *job, double factor)
+{
+    plan_unit(&job->params, job->pend_len, factor, &job->pend_t, &job->pend_lg);
+    if (job->keys.size() == job->s) job->pend_t = std::min(job->pend_t, job->keys.back());
+    job->pend_factor = factor;
+    return unit_reserve_table(job, job->pend_lg);
+}
+
+static ScanArgs unit_scan_args(mashgpu_unit_job *job)
+{
+    const mashgpu_sketch_params *p = &job->params;
+    ScanArgs a;
+    memset(&a, 0, sizeof a);
+    a.stream = job->d_stage[job->pending].p;
+    a.stream_len = job->pend_len;
+    a.tile_begin = 0;
+    a.tile_end = (job->pend_len + SCAN_TILE - 1) / SCAN_TILE;
+    a.coarse_t = job->pend_t;
+    a.seed = p->seed; a.use64 = p->use64; a.preserve_case = p->preserve_case;
+    fill_byte_lut(a, p);
+    a.mode = SCAN_SKETCH;
+    a.unit_start = nullptr;          // one unit: the scan never looks a unit up
+    a.n_units = 1;
+    a.unit_t = job->d_meta.p;
+    a.tab_off = job->d_meta.p + 1;
+    a.tab_log2 = job->d_small.p;
+    a.unit_flags = job->d_small.p + 1;
+    a.unit_maxhash = job->d_small.p + 2;
+    a.tab_keys = job->t_keys.p; a.tab_cnt = job->t_cnt.p; a.tab_first = job->t_first.p; a.tab_last = job->t_last.p;
+    a.only_unit = -1;
+    a.min_copies = 1;
+    return a;
+}
+
+// Enqueue the scan of the pending stage into a cleared table (after its copy has landed).
+static int unit_scan(mashgpu_unit_job *job)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint64_t cap = 1ull << job->pend_lg;
+    MG_CUDA(ctx, cudaMemsetAsync(job->t_keys.p, 0xFF, cap * 8, st));
+    MG_CUDA(ctx, cudaMemsetAsync(job->t_cnt.p, 0, cap * 4, st));
+    MG_CUDA(ctx, cudaMemsetAsync(job->t_first.p, 0xFF, cap * 8, st));
+    MG_CUDA(ctx, cudaMemsetAsync(job->t_last.p, 0, cap * 8, st));
+    const uint64_t meta[2] = {job->pend_t, 0};
+    const uint32_t small[4] = {job->pend_lg, 0, 0, 0};
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_meta.p, meta, sizeof meta, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_small.p, small, sizeof small, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaStreamWaitEvent(st, job->copied[job->pending], 0));
+    return launch_scan(ctx, &job->params, unit_scan_args(job), st);
+}
+
+// Finish the pending stage: exactness guard (re-run with a larger threshold while its bytes are resident), its bottom-s, and the merge.
+static int unit_complete(mashgpu_unit_job *job)
+{
+    if (job->pending < 0) return MASHGPU_OK;
+    mashgpu_ctx *ctx = job->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint32_t s = job->s;
+    uint32_t small[4];
+    unsigned long long n = 0;
+    for (;;) {
+        MG_CUDA(ctx, cudaMemcpyAsync(small, job->d_small.p, sizeof small, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        bool rerun = (small[1] & 1u) != 0;                                          // table overflow
+        if (!rerun) {
+            const uint64_t cap = 1ull << job->pend_lg;
+            MG_CUDA(ctx, cudaMemsetAsync(job->d_n.p, 0, 8, st));
+            compact_table_kernel<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(job->t_keys.p, job->t_cnt.p, 1, cap, job->comp.p, job->d_n.p);
+            ctx->kernel_launches++;
+            MG_CUDA(ctx, cudaGetLastError());
+            MG_CUDA(ctx, cudaMemcpyAsync(&n, job->d_n.p, 8, cudaMemcpyDeviceToHost, st));
+            MG_CUDA(ctx, cudaStreamSynchronize(st));
+            // fewer than s survivors although k-mers were dropped: the stage's bottom-s may lie above the threshold -- unless the
+            // threshold is the running top, above which nothing can enter
+            const uint64_t total = n + (small[2] ? 1 : 0);
+            const bool capped = job->keys.size() == s && job->pend_t == job->keys.back();
+            rerun = total < s && job->pend_t != EMPTY_KEY && !capped;
+        }
+        if (!rerun) break;
+        ctx->exact_reruns++;
+        MG_TRY(unit_plan(job, job->pend_factor * 8.0));
+        MG_TRY(unit_scan(job));
+    }
+    const uint32_t m = (uint32_t)std::min<uint64_t>(n, s);
+    if (n) {
+        MG_CUDA(ctx, cub::DeviceRadixSort::SortKeys(job->sort_tmp.p, job->sort_tmp_bytes, job->comp.p, job->sorted.p, (int)n, 0, 64, st));
+        ctx->kernel_launches += 8;
+        unit_emit_kernel<<<(m + 255) / 256, 256, 0, st>>>(job->sorted.p, m, job->t_keys.p, job->t_cnt.p, job->t_first.p, job->t_last.p,
+                                                          job->pend_lg, job->pend_base, job->c_key.p, job->c_cnt.p, job->c_first.p, job->c_last.p);
+        ctx->kernel_launches++;
+        MG_CUDA(ctx, cudaGetLastError());
+    }
+    std::vector<uint64_t> ck(m + 1), cf(m + 1), cl(m + 1);
+    std::vector<uint32_t> cc(m + 1);
+    if (m) {
+        MG_CUDA(ctx, cudaMemcpyAsync(ck.data(), job->c_key.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(cc.data(), job->c_cnt.p, m * 4ull, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(cf.data(), job->c_first.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(cl.data(), job->c_last.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+    uint32_t nc = m;
+    if (small[2] && m < s) { ck[nc] = EMPTY_KEY; cc[nc] = small[2]; cf[nc] = cl[nc] = job->pend_base; nc++; }   // 2^64-1: not a table key
+    // merge: bottom-s of the union, counts summed; t* = the latest first occurrence among the hashes that entered in this stage
+    std::vector<uint64_t> nk; std::vector<uint32_t> nt;
+    nk.reserve(s); nt.reserve(s);
+    const std::vector<uint64_t> &rk = job->keys;
+    size_t i = 0, j = 0;
+    int64_t top_r = -1, top_c = -1;             // where the last emitted hash came from
+    bool entered = false;
+    uint64_t tstar = 0;
+    while (nk.size() < s && (i < rk.size() || j < nc)) {
+        if (j == nc || (i < rk.size() && rk[i] < ck[j])) { nk.push_back(rk[i]); nt.push_back(job->tot[i]); top_r = (int64_t)i++; top_c = -1; }
+        else if (i == rk.size() || ck[j] < rk[i]) {
+            nk.push_back(ck[j]); nt.push_back(cc[j]); top_r = -1; top_c = (int64_t)j;
+            tstar = entered ? std::max(tstar, cf[j]) : cf[j];
+            entered = true;
+            j++;
+        } else { nk.push_back(rk[i]); nt.push_back(job->tot[i] + cc[j]); top_r = (int64_t)i++; top_c = (int64_t)j++; }
+    }
+    if (entered && nk.back() != EMPTY_KEY) {
+        // the top's count at positions <= t*: its total before this stage plus its occurrences in the stage up to t*, which its first
+        // and last positions in the stage usually decide; otherwise count them over [stage start, t*] of the still-resident stage
+        uint32_t part = 0;
+        if (top_c >= 0) {
+            const uint64_t f = cf[top_c], l = cl[top_c];
+            if (l <= tstar) part = cc[top_c];
+            else if (f > tstar) part = 0;
+            else if (f == tstar) part = 1;
+            else {
+                MG_TRY(recount_hash(ctx, &job->params, unit_scan_args(job), 0, tstar - job->pend_base, nk.back(), job->d_small.p + 3, st));
+                MG_CUDA(ctx, cudaMemcpyAsync(&part, job->d_small.p + 3, 4, cudaMemcpyDeviceToHost, st));
+                MG_CUDA(ctx, cudaStreamSynchronize(st));
+            }
+        }
+        job->top_at_tstar = (top_r >= 0 ? job->tot[top_r] : 0) + part;
+    }
+    job->keys.swap(nk);
+    job->tot.swap(nt);
+    job->pending = -1;
+    ctx->unit_stages++;
+    return MASHGPU_OK;
+}
+
+// The current buffer is full (or the unit ends): copy it to the device, merge the stage before it (whose running top is this stage's
+// threshold), then enqueue this stage's scan.  The host fills the other buffer while the scan runs.
+static int unit_process(mashgpu_unit_job *job)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    const int b = job->stage.cur;
+    const uint64_t len = job->stage.fill;
+    if (len == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_stage[b].p, job->stage.h(), len, cudaMemcpyHostToDevice, ctx->copy_stream));
+    MG_CUDA(ctx, cudaEventRecord(job->copied[b], ctx->copy_stream));
+    MG_TRY(unit_complete(job));
+    job->pending = b;
+    job->pend_len = len;
+    job->pend_base = job->next_base;
+    job->next_base += len - job->stage.carry.size();      // the next stage starts with the carried k-1 bases
+    MG_TRY(unit_plan(job, SURVIVOR_FACTOR));
+    return unit_scan(job);
+}
+
+static int unit_flush(mashgpu_unit_job *job, bool record_continues)
+{
+    return stage_flush(job->stage, record_continues, [&]() { return unit_process(job); });
+}
+
+// Device bytes of a one-unit stream above which the unit streams through a unit job (half of the free device memory, as
+// sketch_reads_whole_set uses; MASHGPU_UNIT_STREAM_BYTES lowers it, for tests).
+static int unit_stream_limit(mashgpu_ctx *ctx, uint64_t *limit)
+{
+    size_t free_b = 0, total_b = 0;
+    MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+    *limit = free_b / 2;
+    if (const char *env = getenv("MASHGPU_UNIT_STREAM_BYTES")) *limit = std::min<uint64_t>(*limit, strtoull(env, nullptr, 10));
+    return MASHGPU_OK;
+}
+
+// One unit through a unit job, fed from the caller's buffers.
+static int sketch_unit_streamed(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, uint64_t n_records, const char *const *seq,
+                                const uint64_t *len, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length,
+                                uint64_t *out_records)
+{
+    mashgpu_unit_job *job = nullptr;
+    MG_TRY(mashgpu_unit_open(ctx, params, &job));
+    uint64_t length = 0, records = 0;
+    int rc = mashgpu_unit_feed(job, n_records, seq, len);
+    if (rc == MASHGPU_OK) rc = mashgpu_unit_finish(job, out_hashes, out_counts, out_n, &length, &records);
+    mashgpu_unit_close(job);
+    if (out_length) *out_length = length;
+    if (out_records) *out_records = records;
+    return rc;
+}
+
+}  // namespace mashgpu
+
+extern "C" int mashgpu_unit_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, mashgpu_unit_job **out)
+{
+    using namespace mashgpu;
+    if (!ctx || !out) return MASHGPU_ERR_INVALID;
+    *out = nullptr;
+    MG_TRY(validate_sketch_params(ctx, params));
+    if (params->min_copies > 1 || params->target_cov > 0)
+        return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "the unit job takes neither min_copies (-m) > 1 nor target_cov (-c): use mashgpu_reads_*");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    auto *job = new mashgpu_unit_job();
+    std::unique_ptr<mashgpu_unit_job> guard(job);
+    job->ctx = ctx;
+    job->params = *params;
+    job->s = params->sketch_size;
+    const uint64_t k = (uint64_t)params->kmer_size;
+    const uint64_t stage_cap = reads_env("MASHGPU_UNIT_STAGE_BYTES", 128ull << 20, 4 * k + 64);
+    ctx->unit_peak_bytes = 0;
+    if (job->stage.open(stage_cap, k, 2) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (unit job staging)");
+    const uint64_t d_stage_bytes = ((stage_cap + 15) / 16) * 16 + 64;
+    if (!unit_alloc(job, job->d_stage[0], d_stage_bytes) || !unit_alloc(job, job->d_stage[1], d_stage_bytes) || !unit_alloc(job, job->d_meta, 2) ||
+        !unit_alloc(job, job->d_small, 4) || !unit_alloc(job, job->d_n, 1) || !unit_alloc(job, job->c_key, job->s) ||
+        !unit_alloc(job, job->c_cnt, job->s) || !unit_alloc(job, job->c_first, job->s) || !unit_alloc(job, job->c_last, job->s))
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (unit job)");
+    // the table of any stage's first pass: a full stage, or a short one that plan_unit keeps whole (span <= 6 s)
+    uint64_t t; uint32_t lg_full, lg_short;
+    plan_unit(params, stage_cap, SURVIVOR_FACTOR, &t, &lg_full);
+    plan_unit(params, std::min<uint64_t>(stage_cap, 2 * (uint64_t)(SURVIVOR_FACTOR * job->s) + 2), SURVIVOR_FACTOR, &t, &lg_short);
+    MG_TRY(unit_reserve_table(job, std::max(lg_full, lg_short)));
+    MG_CUDA(ctx, cudaEventCreateWithFlags(&job->copied[0], cudaEventDisableTiming));
+    MG_CUDA(ctx, cudaEventCreateWithFlags(&job->copied[1], cudaEventDisableTiming));
+    *out = guard.release();
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_unit_feed(mashgpu_unit_job *job, uint64_t n_records, const char *const *seq, const uint64_t *len)
+{
+    using namespace mashgpu;
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (job->finished) return fail(ctx, MASHGPU_ERR_INVALID, "mashgpu_unit_feed after mashgpu_unit_finish");
+    if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    return stage_records(job->stage, n_records, seq, len, [&](bool cont) { return unit_flush(job, cont); }, [] { return false; });
+}
+
+extern "C" int mashgpu_unit_finish(mashgpu_unit_job *job, uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length,
+                                   uint64_t *out_records)
+{
+    using namespace mashgpu;
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!out_hashes || !out_n || !out_length || !out_records) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    if (!job->finished) {
+        if (job->stage.fill) MG_TRY(unit_flush(job, false));
+        MG_TRY(unit_complete(job));
+        job->finished = true;
+    }
+    const size_t n = job->keys.size();
+    std::copy(job->keys.begin(), job->keys.end(), out_hashes);
+    if (out_counts) {
+        std::copy(job->tot.begin(), job->tot.end(), out_counts);
+        // the reference's top-of-heap quirk (quirk_kernel): a full heap's top counts its occurrences up to t* only
+        if (n == job->s && job->keys.back() != EMPTY_KEY) out_counts[n - 1] = job->top_at_tstar;
+    }
+    *out_n = (uint32_t)n;
+    *out_length = job->stage.bases;
+    *out_records = job->stage.records;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_unit_close(mashgpu_unit_job *job)
+{
+    if (!job) return MASHGPU_OK;
+    cudaSetDevice(job->ctx->device);
+    cudaStreamSynchronize(job->ctx->stream);
+    cudaStreamSynchronize(job->ctx->copy_stream);
+    for (cudaEvent_t &e : job->copied) if (e) cudaEventDestroy(e);
     delete job;
     return MASHGPU_OK;
 }
@@ -1814,9 +2264,9 @@ static int sketch_reads_whole_set(mashgpu_ctx *ctx, const mashgpu_sketch_params 
     for (uint64_t r = 0; r < n_records; r++)
         if (len[r] >= k) { total += len[r] + 1; n_rec++; }
     if (n_rec == 0) return MASHGPU_OK;
-    size_t free_b = 0, total_b = 0;
-    MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
-    if (total > free_b / 2) return MASHGPU_ERR_NOMEM;
+    uint64_t limit = 0;
+    MG_TRY(unit_stream_limit(ctx, &limit));
+    if (total > limit) return MASHGPU_ERR_NOMEM;
     DevBuf<uint8_t> d_stream; DevBuf<uint64_t> d_hashes; DevBuf<uint32_t> d_n, d_counts;
     if (d_stream.alloc(((total + 15) / 16) * 16 + 64) != cudaSuccess || d_hashes.alloc(s) != cudaSuccess || d_n.alloc(1) != cudaSuccess ||
         d_counts.alloc(s) != cudaSuccess)
@@ -1886,6 +2336,8 @@ extern "C" int mashgpu_sketch_reads(mashgpu_ctx *ctx, const mashgpu_sketch_param
     if (params && params->bloom_bytes == 0 && !(params->target_cov > 0)) {
         const int rc = mashgpu::sketch_reads_whole_set(ctx, params, n_records, seq, len, out_hashes, out_counts, out_n, out_records_used);
         if (rc != MASHGPU_ERR_NOMEM) return rc;                     // too large for one resident stream: stream it through a job
+        if (params->min_copies <= 1)                                // order-independent: the parallel unit job, not the replay
+            return mashgpu::sketch_unit_streamed(ctx, params, n_records, seq, len, out_hashes, out_counts, out_n, nullptr, out_records_used);
     }
     mashgpu_reads_job *job = nullptr;
     MG_TRY(mashgpu_reads_open(ctx, params, &job));

@@ -195,6 +195,64 @@ void Sketch::flushBatch(Batch &batch)
     batch = Batch();
 }
 
+// A file-mode unit whose parsed sequence passes this many bytes is not held whole: the batch before it is flushed (input order) and
+// the unit streams through a unit job (mashgpu_unit_*, DESIGN.md 2.7), 16 MiB of records at a time.  MASHGPU_CLI_STREAM_BYTES
+// lowers it (tests).
+static uint64_t unitStreamBytes()
+{
+    static const uint64_t v = getenv("MASHGPU_CLI_STREAM_BYTES") ? strtoull(getenv("MASHGPU_CLI_STREAM_BYTES"), 0, 10) : batchBytesMax;
+    return v;
+}
+
+static void gpuCheck(mashgpu_ctx *ctx, int rc)
+{
+    if (rc != MASHGPU_OK) {
+        cerr << "ERROR: " << mashgpu_last_error(ctx) << endl;
+        exit(1);
+    }
+}
+
+static mashgpu_unit_job *openUnitJob(const Sketch::Parameters &parameters)
+{
+    mashgpu_sketch_params p;
+    fillGpuParams(p, parameters);
+    mashgpu_ctx *ctx = gpuContext();
+    mashgpu_unit_job *job = 0;
+    gpuCheck(ctx, mashgpu_unit_open(ctx, &p, &job));
+    return job;
+}
+
+static void feedUnitJob(mashgpu_unit_job *job, vector<mashhost::SeqBuffer> &seqs)
+{
+    vector<const char *> ptrs(seqs.size());
+    vector<uint64_t> lens(seqs.size());
+    for (size_t i = 0; i < seqs.size(); i++) { ptrs[i] = seqs[i].data(); lens[i] = seqs[i].size(); }
+    gpuCheck(gpuContext(), mashgpu_unit_feed(job, seqs.size(), ptrs.data(), lens.data()));
+    seqs.clear();
+}
+
+// Finish and close the job; the sketch goes into `reference` as flushBatch puts a unit's.  Returns the kept records' number.
+static uint64_t finishUnitJob(mashgpu_unit_job *job, const Sketch::Parameters &parameters, Sketch::Reference &reference,
+                              vector<uint64_t> &hashes, vector<uint32_t> &counts)
+{
+    const uint32_t s = (uint32_t)parameters.minHashesPerWindow;
+    hashes.assign(s, 0);
+    counts.assign(s, 0);
+    uint32_t n = 0;
+    uint64_t length = 0, records = 0;
+    gpuCheck(gpuContext(), mashgpu_unit_finish(job, hashes.data(), counts.data(), &n, &length, &records));
+    mashgpu_unit_close(job);
+    hashes.resize(n);
+    counts.resize(n);
+    reference.hashesSorted.setUse64(parameters.use64);
+    reference.hashesSorted.clear();
+    for (uint32_t i = 0; i < n; i++) reference.hashesSorted.push_back64(hashes[i]);
+    if (parameters.counts) reference.counts.assign(counts.begin(), counts.end());
+    reference.countsSorted = true;
+    reference.length = length;
+    return records;
+}
+
 // One unit over all records of the listed files, round robin (sketchFile, reference Sketch.cpp:1147-1336).  With `drain` (reads
 // mode) the records are handed over whenever `bytes` passes drainBytes and at the end; drain returns the number of records used
 // once the sketch is complete (the -c stop), which ends the reading and is the count of the comment, as in the reference's loop.
@@ -287,15 +345,19 @@ void Sketch::initFromReads(const vector<string> &files, const Parameters &parame
     fillGpuParams(p, parameters);
     mashgpu_ctx *ctx = gpuContext();
     mashgpu_reads_job *job = 0;
-    auto check = [&](int rc) {
-        if (rc != MASHGPU_OK) {
-            cerr << "ERROR: " << mashgpu_last_error(ctx) << endl;
-            exit(1);
-        }
-    };
-    check(mashgpu_reads_open(ctx, &p, &job));
+    auto check = [&](int rc) { gpuCheck(ctx, rc); };
+    // without -m > 1, -c and -b the sketch does not depend on the order of the reads: the parallel unit job, not the heap's replay
+    mashgpu_unit_job *unitJob = 0;
+    if (p.min_copies <= 1 && !(p.target_cov > 0) && p.bloom_bytes == 0) unitJob = openUnitJob(parameters);
+    else check(mashgpu_reads_open(ctx, &p, &job));
     bool stopped = false;
     DrainFn drain = [&](vector<mashhost::SeqBuffer> &seqs, vector<uint32_t> &unitOfRecord, uint64_t &bytes) -> uint64_t {
+        if (unitJob) {
+            feedUnitJob(unitJob, seqs);
+            unitOfRecord.clear();
+            bytes = 0;
+            return 0;
+        }
         if (!stopped && !seqs.empty()) {
             vector<const char *> ptrs(seqs.size());
             vector<uint64_t> lens(seqs.size());
@@ -325,13 +387,18 @@ void Sketch::initFromReads(const vector<string> &files, const Parameters &parame
     vector<uint32_t> counts(s);
     uint32_t n = 0;
     uint64_t readsUsed = 0;
-    check(mashgpu_reads_finish(job, hashes.data(), counts.data(), &n, &readsUsed));
-    mashgpu_reads_close(job);
-    reference.hashesSorted.setUse64(parameters.use64);             // == setMinHashesForReference, reference Sketch.cpp:1139-1145
-    reference.hashesSorted.clear();
-    for (uint32_t i = 0; i < n; i++) reference.hashesSorted.push_back64(hashes[i]);
-    if (parameters.counts) reference.counts.assign(counts.begin(), counts.begin() + n);
-    reference.countsSorted = true;
+    if (unitJob) {
+        readsUsed = finishUnitJob(unitJob, parameters, reference, hashes, counts);
+        n = (uint32_t)hashes.size();
+    } else {
+        check(mashgpu_reads_finish(job, hashes.data(), counts.data(), &n, &readsUsed));
+        mashgpu_reads_close(job);
+        reference.hashesSorted.setUse64(parameters.use64);         // == setMinHashesForReference, reference Sketch.cpp:1139-1145
+        reference.hashesSorted.clear();
+        for (uint32_t i = 0; i < n; i++) reference.hashesSorted.push_back64(hashes[i]);
+        if (parameters.counts) reference.counts.assign(counts.begin(), counts.begin() + n);
+        reference.countsSorted = true;
+    }
     // reference Sketch.cpp:1272-1282, 1319-1328; estimateSetSize = MinHashHeap.h:45
     const double setSize = n ? pow(2.0, parameters.use64 ? 64.0 : 32.0) * (double)n / (double)hashes[n - 1] : 0;
     reference.length = parameters.genomeSize != 0 ? parameters.genomeSize : (uint64_t)setSize;
@@ -411,10 +478,16 @@ int Sketch::initFromFiles(const vector<string> &files, const Parameters &paramet
                     if (test == NULL) { cerr << "ERROR: could not open " << files[i + t] << " for reading." << endl; exit(1); }
                     fclose(test);
                 }
-                struct Parsed { Reference ref; vector<mashhost::SeqBuffer> seqs; vector<uint32_t> unitOfRecord; uint64_t bytes = 0; bool ready = false; };
+                // A file past unitStreamBytes() is not parsed whole: its worker hands each 16 MiB of records to this thread, which
+                // feeds them to a unit job once the file's turn has come (the GPU context stays on this thread), and waits until
+                // they are taken.
+                struct Parsed {
+                    Reference ref; vector<mashhost::SeqBuffer> seqs; vector<uint32_t> unitOfRecord; uint64_t bytes = 0; bool ready = false;
+                    bool streaming = false, chunkReady = false; vector<mashhost::SeqBuffer> chunk;
+                };
                 vector<Parsed> parsed(run);
                 std::mutex mu;
-                std::condition_variable cvReady, cvRoom;
+                std::condition_variable cvReady, cvRoom, cvTaken;
                 size_t nextFile = 0, consumed = 0;
                 const size_t window = 2 * (size_t)parameters.parallelism;      // files parsed ahead of the consumer
                 const size_t nWorkers = std::min<size_t>((size_t)parameters.parallelism, run);
@@ -430,22 +503,56 @@ int Sketch::initFromFiles(const vector<string> &files, const Parameters &paramet
                                 cvRoom.wait(lock, [&] { return t < consumed + window; });
                             }
                             vector<string> file(1, files[i + t]);
-                            parseUnit(file, parameters, parsed[t].ref, parsed[t].seqs, parsed[t].unitOfRecord, 0, parsed[t].bytes);
+                            DrainFn drain = [&, t](vector<mashhost::SeqBuffer> &s, vector<uint32_t> &u, uint64_t &b) -> uint64_t {
+                                if (!parsed[t].streaming && b < unitStreamBytes()) return 0;
+                                std::unique_lock<std::mutex> lock(mu);
+                                parsed[t].streaming = true;
+                                parsed[t].chunk = std::move(s);
+                                parsed[t].chunkReady = true;
+                                cvReady.notify_all();
+                                cvTaken.wait(lock, [&] { return !parsed[t].chunkReady; });
+                                s.clear();
+                                u.clear();
+                                b = 0;
+                                return 0;
+                            };
+                            parseUnit(file, parameters, parsed[t].ref, parsed[t].seqs, parsed[t].unitOfRecord, 0, parsed[t].bytes, drain);
                             { std::lock_guard<std::mutex> lock(mu); parsed[t].ready = true; }
                             cvReady.notify_all();
                         }
                     });
                 for (size_t t = 0; t < run; t++) {
                     if (t > 0 && verbosity > 0) cerr << "Sketching " << files[i + t] << "..." << endl;
-                    {
-                        std::unique_lock<std::mutex> lock(mu);
-                        cvReady.wait(lock, [&] { return parsed[t].ready; });
+                    mashgpu_unit_job *job = 0;
+                    for (;;) {
+                        vector<mashhost::SeqBuffer> chunk;
+                        {
+                            std::unique_lock<std::mutex> lock(mu);
+                            cvReady.wait(lock, [&] { return parsed[t].ready || parsed[t].chunkReady; });
+                            if (!parsed[t].chunkReady) break;
+                            chunk = std::move(parsed[t].chunk);
+                            parsed[t].chunk.clear();
+                            parsed[t].chunkReady = false;
+                        }
+                        cvTaken.notify_all();
+                        if (!job) {
+                            flushBatch(batch);           // keep input order
+                            job = openUnitJob(parameters);
+                        }
+                        feedUnitJob(job, chunk);
                     }
-                    const uint32_t unit = (uint32_t)batch.refs.size();
-                    batch.refs.push_back(std::move(parsed[t].ref));
-                    for (auto &q : parsed[t].seqs) batch.seqs.push_back(std::move(q));
-                    batch.unitOfRecord.insert(batch.unitOfRecord.end(), parsed[t].seqs.size(), unit);
-                    batch.bytes += parsed[t].bytes;
+                    if (job) {
+                        feedUnitJob(job, parsed[t].seqs);
+                        vector<uint64_t> h; vector<uint32_t> c;
+                        finishUnitJob(job, parameters, parsed[t].ref, h, c);
+                        references.push_back(std::move(parsed[t].ref));
+                    } else {
+                        const uint32_t unit = (uint32_t)batch.refs.size();
+                        batch.refs.push_back(std::move(parsed[t].ref));
+                        for (auto &q : parsed[t].seqs) batch.seqs.push_back(std::move(q));
+                        batch.unitOfRecord.insert(batch.unitOfRecord.end(), parsed[t].seqs.size(), unit);
+                        batch.bytes += parsed[t].bytes;
+                    }
                     vector<mashhost::SeqBuffer>().swap(parsed[t].seqs);
                     { std::lock_guard<std::mutex> lock(mu); consumed = t + 1; }
                     cvRoom.notify_all();
@@ -454,9 +561,36 @@ int Sketch::initFromFiles(const vector<string> &files, const Parameters &paramet
                 for (auto &w : workers) w.join();
                 i += run - 1;
             } else if (parameters.concatenated) {
+                // the unit is parsed on its own; past unitStreamBytes() it streams through a unit job, else it joins the batch
                 vector<string> file(1, files[i]);
-                batch.refs.emplace_back();
-                parseUnit(file, parameters, batch.refs.back(), batch.seqs, batch.unitOfRecord, (uint32_t)batch.refs.size() - 1, batch.bytes);
+                Reference ref;
+                vector<mashhost::SeqBuffer> seqs;
+                vector<uint32_t> unitOfRecord;
+                uint64_t bytes = 0;
+                mashgpu_unit_job *job = 0;
+                DrainFn drain = [&](vector<mashhost::SeqBuffer> &s, vector<uint32_t> &u, uint64_t &b) -> uint64_t {
+                    if (!job && b < unitStreamBytes()) return 0;
+                    if (!job) {
+                        flushBatch(batch);
+                        job = openUnitJob(parameters);
+                    }
+                    feedUnitJob(job, s);
+                    u.clear();
+                    b = 0;
+                    return 0;
+                };
+                parseUnit(file, parameters, ref, seqs, unitOfRecord, 0, bytes, drain);
+                if (job) {
+                    vector<uint64_t> h; vector<uint32_t> c;
+                    finishUnitJob(job, parameters, ref, h, c);
+                    references.push_back(ref);
+                } else {
+                    const uint32_t unit = (uint32_t)batch.refs.size();
+                    batch.refs.push_back(std::move(ref));
+                    for (auto &q : seqs) batch.seqs.push_back(std::move(q));
+                    batch.unitOfRecord.insert(batch.unitOfRecord.end(), seqs.size(), unit);
+                    batch.bytes += bytes;
+                }
             } else {
                 // one sketch per record (sketchFileBySequence / sketchSequence, reference Sketch.cpp:326-370, 1338-1365)
                 gzFile fp = mashhost::FastxReader::openPath(files[i]);
