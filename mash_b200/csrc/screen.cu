@@ -606,7 +606,7 @@ extern "C" int mashgpu_screen_finish(mashgpu_screen_job *job, uint64_t *shared, 
         d_ident.p = reinterpret_cast<double *>(outs + 2 * n); d_p.p = reinterpret_cast<double *>(outs + 3 * n);
         uint32_t N = 2;
         while (N < job->stride) N <<= 1;
-        if ((size_t)N * 4 > 200 * 1024) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketches larger than 51200 hashes");
+        if ((size_t)N * 4 > 200 * 1024) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketches larger than 32768 hashes");
         if ((size_t)N * 4 > 48 * 1024)
             MG_CUDA(ctx, cudaFuncSetAttribute(screen_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)N * 4)));
         screen_reduce_kernel<<<(unsigned)n, SCR_THREADS, (size_t)N * 4, st>>>(job->ref_hashes, job->stride, job->ref_n, job->keys.p, job->slot_idx.p, job->cnt.p, job->log2cap,
