@@ -318,7 +318,11 @@ typedef struct mashgpu_screen_job mashgpu_screen_job;
  *                                    'A' on the reverse strand only, as the reference's complement table has it) and its
  *                                    non-canonical amino-acid k-mers are screened; kmer space 20^k;
  *   any other alphabet (-z)          byte k-mers of the reads as they stand.
- * Non-nucleotide jobs always upload ASCII (MASHGPU_SCREEN_HOST_PACK is ignored). */
+ * Non-nucleotide jobs always upload ASCII (MASHGPU_SCREEN_HOST_PACK is ignored).
+ * Refused before any table is built: sketch_size > 8192 (MASHGPU_ERR_UNSUPPORTED); a row with n_hashes[r] > stride
+ * (MASHGPU_ERR_INVALID); a reference sketch of more than 32768 hashes (MASHGPU_ERR_UNSUPPORTED; the stride may be larger);
+ * a reference hash >= 2^32 in a 32-bit job, i.e. when the k-mer space is at most 2^32 (MASHGPU_ERR_INVALID); the hash value
+ * 2^64-1 (MASHGPU_ERR_UNSUPPORTED). */
 int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, const mashgpu_sketch_set *refs,
                         mashgpu_screen_job **job);
 /* One HashInput (CommandScreen.h:104-133): a '*'-joined chunk of reads (CommandScreen.cpp:224-262; any byte

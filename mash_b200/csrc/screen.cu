@@ -32,9 +32,10 @@
 namespace mashgpu {
 
 constexpr int SCR_THREADS = 256;
+constexpr uint32_t SCREEN_MAX_REF_HASHES = 1u << 15;      // per reference sketch: the reduce sorts its depths in 128 KB of shared memory
 
 // valid hashes of all reference sketches -> dense list (order irrelevant: sorted next)
-__global__ void screen_gather_kernel(const uint64_t *hashes, uint64_t stride, const uint32_t *n_hashes, uint64_t n_rows,
+__global__ void screen_gather_kernel(const uint64_t *hashes, uint64_t stride, const uint32_t *n_hashes, uint64_t n_rows, int use64,
                                      uint64_t *out, unsigned long long *out_n, uint32_t *err)
 {
     const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -43,6 +44,9 @@ __global__ void screen_gather_kernel(const uint64_t *hashes, uint64_t stride, co
     if (i >= n_hashes[row]) return;
     const uint64_t key = hashes[t];
     if (key == EMPTY_KEY) { atomicOr(err, 1u); return; }   // 2^64-1 cannot be a table key (probability 2^-64 per hash)
+    // a 32-bit job's k-mers hash below 2^32: a larger key is another sketch's hash, and it would index the bitmap (built from
+    // the top bits of a 32-bit value) far past its end
+    if (!use64 && (key >> 32)) { atomicOr(err, 2u); return; }
     out[atomicAdd(out_n, 1ull)] = key;
 }
 
@@ -244,6 +248,7 @@ struct mashgpu_screen_job {
     bool winner = false;     // -w
     std::vector<uint64_t> h_len;      // Reference::length per sketch (tie break of -w), zeros when the caller gave none
     std::vector<uint32_t> h_n;        // hashes per sketch
+    uint32_t max_n = 0;               // largest of them (<= SCREEN_MAX_REF_HASHES): sizes the reduce's shared array
     // translated screen (protein sketches): each chunk is translated in six frames into pep[slot] and the peptide stream is
     // scanned; a slot's buffer stays untouched until its chunk is collected (the exact re-run reads it again)
     bool translate = false;
@@ -283,6 +288,23 @@ extern "C" int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params
     job->translate = is_protein_alphabet(params);
     if (!is_dna_alphabet(params)) job->host_pack = 0;
     auto bail = [&](int rc) { delete job; return rc; };
+    // the row lengths first: the kernels below trust them (gather, reduce and winner read n_hashes[r] entries of row r)
+    job->h_n.assign(refs->n, 0); job->h_len.assign(refs->n, 0);
+    if (refs->n) {
+        if (refs->on_device) {
+            cudaError_t e = cudaMemcpy(job->h_n.data(), refs->n_hashes, refs->n * 4, cudaMemcpyDeviceToHost);
+            if (e == cudaSuccess && refs->length) e = cudaMemcpy(job->h_len.data(), refs->length, refs->n * 8, cudaMemcpyDeviceToHost);
+            if (e != cudaSuccess) return bail(fail(ctx, MASHGPU_ERR_CUDA, "reading the reference set's n_hashes failed: %s", cudaGetErrorString(e)));
+        } else {
+            memcpy(job->h_n.data(), refs->n_hashes, refs->n * 4);
+            if (refs->length) memcpy(job->h_len.data(), refs->length, refs->n * 8);
+        }
+    }
+    for (uint32_t v : job->h_n) job->max_n = std::max(job->max_n, v);
+    if (job->max_n > refs->stride)
+        return bail(fail(ctx, MASHGPU_ERR_INVALID, "a reference sketch holds %u hashes in rows of %llu", job->max_n, (unsigned long long)refs->stride));
+    if (job->max_n > SCREEN_MAX_REF_HASHES)
+        return bail(fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketches larger than %u hashes", SCREEN_MAX_REF_HASHES));
     const uint64_t total = refs->n * refs->stride;
     if (refs->on_device) { job->ref_hashes = refs->hashes; job->ref_n = refs->n_hashes; }
     else {
@@ -308,12 +330,14 @@ extern "C" int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params
     cudaMemsetAsync(d_err.p, 0, 4, st);
     unsigned long long n_valid = 0; uint32_t err = 0; uint64_t n_distinct = 0; unsigned long long hmax = 0;
     if (total) {
-        screen_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(job->ref_hashes, refs->stride, job->ref_n, refs->n, gathered.p, d_count.p, d_err.p);
+        screen_gather_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(job->ref_hashes, refs->stride, job->ref_n, refs->n, params->use64,
+                                                                                 gathered.p, d_count.p, d_err.p);
         cudaMemcpyAsync(&n_valid, d_count.p, 8, cudaMemcpyDeviceToHost, st);
         cudaMemcpyAsync(&err, d_err.p, 4, cudaMemcpyDeviceToHost, st);
         cudaError_t e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) return bail(fail(ctx, MASHGPU_ERR_CUDA, "screen table build failed: %s", cudaGetErrorString(e)));
-        if (err) return bail(fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketch contains the hash value 2^64-1"));
+        if (err & 1) return bail(fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketch contains the hash value 2^64-1"));
+        if (err & 2) return bail(fail(ctx, MASHGPU_ERR_INVALID, "reference hash >= 2^32 in a 32-bit sketch (k-mer space <= 2^32)"));
         if (n_valid >= 0x7FFFFFFFull) return bail(fail(ctx, MASHGPU_ERR_UNSUPPORTED, "more than 2^31 reference hashes"));
         if (n_valid) {
             size_t tb1 = 0, tb2 = 0;
@@ -351,16 +375,6 @@ extern "C" int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params
         if (e != cudaSuccess) return bail(fail(ctx, MASHGPU_ERR_CUDA, "screen table build failed: %s", cudaGetErrorString(e)));
     }
     job->hmax = hmax;
-    job->h_n.assign(refs->n, 0); job->h_len.assign(refs->n, 0);
-    if (refs->n) {
-        if (refs->on_device) {
-            MG_CUDA(ctx, cudaMemcpy(job->h_n.data(), refs->n_hashes, refs->n * 4, cudaMemcpyDeviceToHost));
-            if (refs->length) MG_CUDA(ctx, cudaMemcpy(job->h_len.data(), refs->length, refs->n * 8, cudaMemcpyDeviceToHost));
-        } else {
-            memcpy(job->h_n.data(), refs->n_hashes, refs->n * 4);
-            if (refs->length) memcpy(job->h_len.data(), refs->length, refs->n * 8);
-        }
-    }
     if (!ctx->attr_merge) {   // per context: function attributes are per device
         cudaFuncSetAttribute(merge_bottom_s_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 128 * 1024);
         ctx->attr_merge = true;
@@ -605,8 +619,7 @@ extern "C" int mashgpu_screen_finish(mashgpu_screen_job *job, uint64_t *shared, 
         d_shared.p = outs; d_median.p = outs + n;
         d_ident.p = reinterpret_cast<double *>(outs + 2 * n); d_p.p = reinterpret_cast<double *>(outs + 3 * n);
         uint32_t N = 2;
-        while (N < job->stride) N <<= 1;
-        if ((size_t)N * 4 > 200 * 1024) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "reference sketches larger than 32768 hashes");
+        while (N < job->max_n) N <<= 1;         // <= SCREEN_MAX_REF_HASHES (refused at open): 128 KB
         if ((size_t)N * 4 > 48 * 1024)
             MG_CUDA(ctx, cudaFuncSetAttribute(screen_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)N * 4)));
         screen_reduce_kernel<<<(unsigned)n, SCR_THREADS, (size_t)N * 4, st>>>(job->ref_hashes, job->stride, job->ref_n, job->keys.p, job->slot_idx.p, job->cnt.p, job->log2cap,
