@@ -393,14 +393,23 @@ class DistJob:
         self.h = h
         return self
 
-    def run(self, q_begin, q_count):
+    DIST_OUTPUTS = (("numer", np.uint32, u32p), ("denom", np.uint32, u32p), ("distance", np.float64, f64p), ("pvalue", np.float64, f64p),
+                    ("pass", np.uint8, u8p))
+
+    def run(self, q_begin, q_count, outputs=("numer", "denom", "distance", "pvalue", "pass")):
+        """(q_count, n_ref) arrays of the named outputs; the others are passed as NULL (neither copied back nor allocated)."""
         n = q_count * self.n_ref
-        numer = np.zeros(n, np.uint32); denom = np.zeros(n, np.uint32)
-        dist = np.zeros(n, np.float64); pv = np.zeros(n, np.float64); ok = np.zeros(n, np.uint8)
-        self.eng._check(self.eng.lib.mashgpu_dist_run(self.h, q_begin, q_count, _p(numer, u32p), _p(denom, u32p), _p(dist, f64p), _p(pv, f64p), _p(ok, u8p)))
+        unknown = set(outputs) - {name for name, _, _ in self.DIST_OUTPUTS}
+        if unknown:
+            raise ValueError(f"unknown dist outputs {sorted(unknown)}")
+        arrs = {name: np.zeros(n, dt) for name, dt, _ in self.DIST_OUTPUTS if name in outputs}
+        ptrs = [_p(arrs[name], pt) if name in arrs else None for name, _, pt in self.DIST_OUTPUTS]
+        self.eng._check(self.eng.lib.mashgpu_dist_run(self.h, q_begin, q_count, *ptrs))
         shp = (q_count, self.n_ref)
-        return {"numer": numer.reshape(shp), "denom": denom.reshape(shp), "distance": dist.reshape(shp),
-                "pvalue": pv.reshape(shp), "pass": ok.reshape(shp).astype(bool)}
+        out = {name: a.reshape(shp) for name, a in arrs.items()}
+        if "pass" in out:
+            out["pass"] = out["pass"].astype(bool)
+        return out
 
     def run_list(self, q_begin, q_count, capacity):
         """Passing pairs only, sorted by pair index. Returns (n_pass, dict of arrays) -- arrays empty when n_pass > capacity."""

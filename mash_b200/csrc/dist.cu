@@ -67,8 +67,11 @@ struct DistArgs {
     uint32_t tri_r0;            // row of reference 0 in the query numbering (0 for a self comparison; the shard offset of an encoded job)
     int use_qlist;              // dist_kernel: take the queries of a tile from qlist instead of the dense range
     // sparse related pairs (dist_probe_kernel -> dist_pair_kernel): when a query may share hashes with at most pair_max references
-    // of a tile, only those (query, reference) pairs are merged, one warp per pair, instead of all 32 in lockstep
-    uint2 *pair_list; unsigned long long *pair_count; uint64_t pair_capacity; unsigned long long *pair_total;
+    // of a tile, only those (query, reference) pairs are merged, one warp per pair, instead of all 32 in lockstep.  A warp reserves its
+    // slots with one atomicAdd on pair_count; pair_full holds ~(start of the first reservation that did not fit), 0 while all fit
+    // (complemented so that zeroed memory means "none" and atomicMax keeps the smallest start).  Slots from that start on may be
+    // unwritten -- a reservation that straddles the capacity writes nothing -- and are not merged.
+    uint2 *pair_list; unsigned long long *pair_count, *pair_full; uint64_t pair_capacity; unsigned long long *pair_total;
     int pair_max;               // 0: every flagged (query, tile) combination goes to the tile's work list
     int pair_dense;             // dist_pair_kernel enumerates every pair of the run itself (sketch sizes beyond the tiled merge)
     // deferred p-values (dist_fix_kernel): pairs with shared hashes whose binomial tail is evaluated in a dense second pass
@@ -489,7 +492,11 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
                 at = __shfl_sync(0xFFFFFFFFu, at, 0);
                 if (at + __popc(want) <= a.pair_capacity) {
                     if ((want >> lane) & 1u) a.pair_list[at + __popc(want & ((1u << lane) - 1u))] = make_uint2(q, r);
-                } else dense = true;
+                } else {
+                    // the counter has moved past slots this warp leaves unwritten: the consumer stops at the first such start
+                    if (lane == 0) atomicMax(a.pair_full, ~at);
+                    dense = true;
+                }
             }
         }
         if (dense) {
@@ -563,8 +570,10 @@ __global__ void __launch_bounds__(PAIR_WARPS_MAX * 32) dist_pair_kernel(const Di
     uint64_t total;
     if (a.pair_dense) total = (uint64_t)a.q_count * a.n_ref;
     else {
-        const unsigned long long listed = *a.pair_count;
-        total = listed < a.pair_capacity ? listed : a.pair_capacity;
+        // every slot below both bounds was written by this run (a reservation below the first failed one fit); without a failed
+        // reservation pair_count <= pair_capacity
+        const unsigned long long listed = *a.pair_count, written = ~*a.pair_full;
+        total = listed < written ? listed : written;
         if (blockIdx.x == 0 && threadIdx.x == 0 && a.pair_total) atomicAdd(a.pair_total, (unsigned long long)total);
     }
     for (uint64_t idx = (uint64_t)blockIdx.x * warps + warp; idx < total; idx += (uint64_t)gridDim.x * warps) {
@@ -816,7 +825,8 @@ struct mashgpu_dist_job {
     bool auto_off = false;
     DevBuf<uint32_t> qlist, qcount;
     DevBuf<uint2> pair_list;            // sparse related pairs of the run in flight (dist_probe_kernel -> dist_pair_kernel)
-    DevBuf<unsigned long long> pair_count;      // [0] pairs listed by the run in flight, [1] pairs merged from lists since the job was opened
+    DevBuf<unsigned long long> pair_count;      // [0] slots reserved by the run in flight, [1] its DistArgs::pair_full, [2] pairs merged from
+                                                // lists since the job was opened
     int pair_max = 4;                   // a (query, tile) combination with at most this many candidate references goes to the pair list;
                                         // 0 = pair path off (MASHGPU_DIST_PAIR_MAX)
     DevBuf<FixEntry> fix_list;
@@ -1222,7 +1232,7 @@ extern "C" int mashgpu_dist_pair_stats(mashgpu_dist_job *job, uint64_t *pairs_me
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     MG_CUDA(ctx, cudaDeviceSynchronize());
     unsigned long long v = 0;
-    MG_CUDA(ctx, cudaMemcpy(&v, job->pair_count.p + 1, 8, cudaMemcpyDeviceToHost));
+    MG_CUDA(ctx, cudaMemcpy(&v, job->pair_count.p + 2, 8, cudaMemcpyDeviceToHost));
     *pairs_merged_from_lists = v;
     return MASHGPU_OK;
 }
@@ -1252,7 +1262,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     a.qlist = nullptr; a.qcount = nullptr; a.qlist_stride = 0; a.flag_total = nullptr; a.use_qlist = 0; a.q_per_cta = 0;
     a.triangle = job->triangle ? 1 : 0;
     a.tri_r0 = job->self ? 0u : (uint32_t)job->ref_row0;
-    a.pair_list = nullptr; a.pair_count = nullptr; a.pair_capacity = 0; a.pair_total = nullptr; a.pair_max = 0; a.pair_dense = 0;
+    a.pair_list = nullptr; a.pair_count = nullptr; a.pair_full = nullptr; a.pair_capacity = 0; a.pair_total = nullptr; a.pair_max = 0; a.pair_dense = 0;
     {   // queue for the deferred p-values: 1/16 of the pairs (at least 2^20); beyond that dist_emit evaluates in place
         const uint64_t pairs = q_count * job->n_ref;
         const uint64_t cap = std::min<uint64_t>(pairs, std::max<uint64_t>(1ull << 20, pairs / 16));
@@ -1322,11 +1332,11 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
             const uint64_t cap = std::max<uint64_t>(1ull << 20, pairs / 16);
             if (job->pair_list.n < cap && job->pair_list.alloc(cap) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pair list)");
             if (!job->pair_count.p) {
-                if (job->pair_count.alloc(2) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pair counter)");
-                MG_CUDA(ctx, cudaMemsetAsync(job->pair_count.p, 0, 16, st));
+                if (job->pair_count.alloc(3) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pair counter)");
+                MG_CUDA(ctx, cudaMemsetAsync(job->pair_count.p, 0, 24, st));
             }
-            MG_CUDA(ctx, cudaMemsetAsync(job->pair_count.p, 0, 8, st));
-            a.pair_list = job->pair_list.p; a.pair_count = job->pair_count.p; a.pair_total = job->pair_count.p + 1;
+            MG_CUDA(ctx, cudaMemsetAsync(job->pair_count.p, 0, 16, st));
+            a.pair_list = job->pair_list.p; a.pair_count = job->pair_count.p; a.pair_full = job->pair_count.p + 1; a.pair_total = job->pair_count.p + 2;
             a.pair_capacity = job->pair_list.n; a.pair_max = job->pair_max;
         }
         // probe: one CTA keeps its filter for a long run of queries (the build costs about as much as probing ~100 queries)
