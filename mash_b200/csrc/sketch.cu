@@ -296,14 +296,29 @@ __global__ void apply_runs_kernel(const PackRun *runs, uint64_t n_runs, uint32_t
     }
 }
 
-__global__ void emit_sorted_kernel(const uint64_t *sorted, uint32_t m, const uint64_t *keys, const uint32_t *cnt, uint32_t log2cap,
-                                   uint32_t maxhash_cnt, uint32_t n_sorted, uint64_t *out_hashes, uint32_t *out_counts)
+// The bottom-m of a single-unit pass, ascending, each hash with its count and (first != NULL) its promoting occurrence (level mc-1)
+// and its last occurrence, positions + base.  Entry n_sorted, when m > n_sorted, is the hash 2^64-1, which the table cannot hold: its
+// side count, positions at the unit's start.
+__global__ void unit_emit_kernel(const uint64_t *sorted, uint32_t n_sorted, uint32_t m, const uint64_t *keys, const uint32_t *cnt,
+                                 const uint64_t *first, const uint64_t *last, uint32_t log2cap, uint32_t mc, uint32_t maxhash_cnt,
+                                 uint64_t start, uint64_t base, uint64_t *c_key, uint32_t *c_cnt, uint64_t *c_first, uint64_t *c_last)
 {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
-    uint64_t key = i < n_sorted ? sorted[i] : EMPTY_KEY;
-    out_hashes[i] = key;
-    if (out_counts) out_counts[i] = i < n_sorted ? table_count(keys, cnt, log2cap, key) : maxhash_cnt;
+    if (i == n_sorted) {
+        c_key[i] = EMPTY_KEY;
+        c_cnt[i] = maxhash_cnt;
+        if (first) c_first[i] = c_last[i] = base + start;
+        return;
+    }
+    const uint64_t key = sorted[i];
+    const int64_t slot = table_find(keys, log2cap, key);
+    c_key[i] = key;
+    c_cnt[i] = cnt[slot];
+    if (first) {
+        c_first[i] = base + first[slot * mc + mc - 1];
+        c_last[i] = base + last[slot];
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -362,12 +377,41 @@ void plan_unit(const mashgpu_sketch_params *p, uint64_t span, double factor, uin
     *log2_out = std::max(4u, ceil_log2((uint64_t)(TABLE_SLACK * expect) + 2));
 }
 
-void fill_byte_lut(ScanArgs &a, const mashgpu_sketch_params *p)
+// The fields every pass over a stream shares: its source (ASCII, or packed codes and mask), its length and tiles, the hashing
+// parameters; one unit, none skipped, no `-m`.
+static ScanArgs scan_base(const mashgpu_sketch_params *p, const void *stream, uint64_t stream_len, const uint64_t *codes = nullptr,
+                          const uint32_t *inval = nullptr)
 {
+    ScanArgs a;
+    memset(&a, 0, sizeof a);
+    a.stream = (const uint8_t *)stream;
+    a.codes = codes;
+    a.inval = inval;
+    a.stream_len = stream_len;
+    a.tile_end = (stream_len + SCAN_TILE - 1) / SCAN_TILE;
+    a.seed = p->seed;
+    a.use64 = p->use64;
+    a.preserve_case = p->preserve_case;
     for (int b = 0; b < 256; b++) {
         int u = (!p->preserve_case && b > 96 && b < 123) ? b - 32 : b;     // reference Sketch.cpp:524-530
         a.byte_lut[b] = p->alphabet[u] ? (uint8_t)u : 0;
     }
+    a.n_units = 1;
+    a.only_unit = -1;
+    a.min_copies = 1;
+    return a;
+}
+
+// A job's device allocation: `bytes` follows what the job holds, `peak` its largest value.
+template <typename T>
+static bool tracked_alloc(DevBuf<T> &b, size_t n, uint64_t &bytes, uint64_t &peak)
+{
+    const size_t before = b.n * sizeof(T);
+    if (b.alloc(n) != cudaSuccess) return false;
+    bytes += n * sizeof(T);
+    bytes -= before;
+    peak = std::max(peak, bytes);
+    return true;
 }
 
 static int launch_scan(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const ScanArgs &a, cudaStream_t st)
@@ -403,46 +447,87 @@ static int recount_hash(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const 
     return launch_scan(ctx, p, c, st);
 }
 
-// Exact re-run of one unit with growing thresholds, ending at keep-all (always succeeds).
-static int rerun_unit(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const SketchStream &S, uint32_t u,
-                      uint64_t *d_out_hashes, uint32_t *d_out_counts, uint32_t *d_out_n, cudaStream_t st,
-                      const ScanArgs &base)
-{
-    const uint64_t span = S.unit_start[u + 1] - S.unit_start[u];
-    const uint32_t s = p->sketch_size;
-    const uint32_t mc = std::max(1u, p->min_copies);
-    double factor = SURVIVOR_FACTOR;
-    ctx->exact_reruns++;
-    for (int attempt = 0; attempt < 64; attempt++) {
-        factor *= 8.0;
-        uint64_t t; uint32_t lg;
-        plan_unit(p, span, factor, &t, &lg);
-        const bool keep_all = (t == EMPTY_KEY);
-        const uint64_t cap = 1ull << lg;
-        DevBuf<uint64_t> keys; DevBuf<uint32_t> cnt; DevBuf<uint64_t> meta;   // meta: [t, off, quirk target, quirk t*]
-        DevBuf<uint32_t> small;                                                   // [log2, flags, maxhash]
-        DevBuf<uint64_t> first, last;
-        const bool want_counts = d_out_counts != nullptr;
-        if (keys.alloc(cap) != cudaSuccess || cnt.alloc(cap) != cudaSuccess || meta.alloc(4) != cudaSuccess || small.alloc(3) != cudaSuccess ||
-            (want_counts && (first.alloc(cap * mc) != cudaSuccess || last.alloc(cap) != cudaSuccess)))
-            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory in exact re-run (table of %llu slots)", (unsigned long long)cap);
-        MG_CUDA(ctx, cudaMemsetAsync(keys.p, 0xFF, cap * 8, st));
-        MG_CUDA(ctx, cudaMemsetAsync(cnt.p, 0, cap * 4, st));
-        if (want_counts) {
-            MG_CUDA(ctx, cudaMemsetAsync(first.p, 0xFF, cap * mc * 8, st));
-            MG_CUDA(ctx, cudaMemsetAsync(last.p, 0, cap * 8, st));
+// One unit sketched alone and exactly in a global-memory candidate table (DESIGN.md 2.3): the exact re-run of a flagged unit, and
+// each stage of a unit job (2.7).  The owner sets the stream (`base`: its source and unit lookup), the unit (index u, stream
+// positions [lo, hi)) and pos_base, which is added to every position the pass reports.  Buffers only grow; their bytes are counted
+// in the owner's counters.
+struct UnitPass {
+    mashgpu_ctx *ctx = nullptr;
+    const mashgpu_sketch_params *p = nullptr;
+    cudaStream_t st = nullptr;
+    uint64_t *bytes = nullptr, *peak = nullptr;
+    bool positions = false;             // keep the first / last positions of every key (counts)
+    uint32_t mc = 1;                    // `-m`: mc first positions per key; candidates need cnt >= mc
+    ScanArgs base;
+    uint32_t u = 0;
+    uint64_t lo = 0, hi = 0, pos_base = 0;
+    // the last scan: survivor factor, threshold (clamped to cap_t, above which nothing can enter), table size, scans of this unit
+    double factor = 0;
+    uint64_t t = 0, cap_t = EMPTY_KEY;
+    uint32_t lg = 0, lg_cap = 0, scans = 0;
+    DevBuf<uint64_t> keys, first, last, comp, sorted, c_key, c_first, c_last, meta;   // meta: [threshold, table offset 0]
+    DevBuf<uint32_t> cnt, c_cnt, small;                                               // small: [log2, flags, maxhash, recount]
+    DevBuf<unsigned long long> d_n;
+    DevBuf<uint8_t> sort_tmp;
+    size_t sort_tmp_bytes = 0;
+    // the bottom-s of the last finish(): hash, count, promoting and last position
+    std::vector<uint64_t> h_key, h_first, h_last;
+    std::vector<uint32_t> h_cnt;
+
+    template <typename T>
+    bool alloc(DevBuf<T> &b, size_t n) { return tracked_alloc(b, n, *bytes, *peak); }
+
+    int open(mashgpu_ctx *ctx_, const mashgpu_sketch_params *p_, cudaStream_t st_, bool positions_, uint64_t *bytes_, uint64_t *peak_)
+    {
+        ctx = ctx_; p = p_; st = st_; positions = positions_; bytes = bytes_; peak = peak_;
+        mc = std::max(1u, p->min_copies);
+        const uint32_t s = p->sketch_size;
+        if (!alloc(meta, 2) || !alloc(small, 4) || !alloc(d_n, 1) || !alloc(c_key, s) || !alloc(c_cnt, s) ||
+            (positions && (!alloc(c_first, s) || !alloc(c_last, s))))
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (single-unit pass)");
+        return MASHGPU_OK;
+    }
+
+    // Table, compaction and sort buffers for 2^l slots.
+    int reserve(uint32_t l)
+    {
+        if (l <= lg_cap) return MASHGPU_OK;
+        const uint64_t cap = 1ull << l;
+        size_t tmp = 0;
+        cub::DeviceRadixSort::SortKeys(nullptr, tmp, (uint64_t *)nullptr, (uint64_t *)nullptr, (int)std::min<uint64_t>(cap, 0x7FFFFFFF), 0, 64, st);
+        if (!alloc(keys, cap) || !alloc(cnt, cap) || (positions && (!alloc(first, cap * mc) || !alloc(last, cap))) || !alloc(comp, cap) ||
+            !alloc(sorted, cap) || !alloc(sort_tmp, tmp))
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (single-unit table of %llu slots)", (unsigned long long)cap);
+        sort_tmp_bytes = tmp;
+        lg_cap = l;
+        return MASHGPU_OK;
+    }
+
+    // Plan the threshold for f x s expected survivors, clamp it to `cap`, clear the table and enqueue the scan of the unit.
+    int scan(double f, uint64_t cap)
+    {
+        factor = f;
+        cap_t = cap;
+        plan_unit(p, hi - lo, factor, &t, &lg);
+        t = std::min(t, cap_t);
+        MG_TRY(reserve(lg));
+        const uint64_t n = 1ull << lg;
+        MG_CUDA(ctx, cudaMemsetAsync(keys.p, 0xFF, n * 8, st));
+        MG_CUDA(ctx, cudaMemsetAsync(cnt.p, 0, n * 4, st));
+        if (positions) {
+            MG_CUDA(ctx, cudaMemsetAsync(first.p, 0xFF, n * mc * 8, st));
+            MG_CUDA(ctx, cudaMemsetAsync(last.p, 0, n * 8, st));
         }
-        uint64_t h_meta[4] = {t, 0, 0, 0};
-        uint32_t h_small[3] = {lg, 0, 0};
+        const uint64_t h_meta[2] = {t, 0};
+        const uint32_t h_small[4] = {lg, 0, 0, 0};
         MG_CUDA(ctx, cudaMemcpyAsync(meta.p, h_meta, sizeof h_meta, cudaMemcpyHostToDevice, st));
         MG_CUDA(ctx, cudaMemcpyAsync(small.p, h_small, sizeof h_small, cudaMemcpyHostToDevice, st));
-        // The scan looks units up by index u: give it views shifted so that index u lands on our single entries.
         ScanArgs a = base;
-        a.tile_begin = S.unit_start[u] / SCAN_TILE;
-        a.tile_end = (S.unit_start[u + 1] + SCAN_TILE - 1) / SCAN_TILE;
-        a.tile_tmax = nullptr;
-        a.tile_unit = nullptr;
+        a.mode = SCAN_SKETCH;           // a screen pass's reference hits were counted by its first scan
+        a.tile_begin = lo / SCAN_TILE;
+        a.tile_end = (hi + SCAN_TILE - 1) / SCAN_TILE;
         a.coarse_t = t;
+        // the scan looks units up by index: views shifted so that index u lands on the pass's single entries
         a.only_unit = u;
         a.unit_t = meta.p - u;
         a.tab_off = meta.p + 1 - u;
@@ -451,53 +536,152 @@ static int rerun_unit(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const Sk
         a.unit_maxhash = small.p + 2 - u;
         a.tab_keys = keys.p;
         a.tab_cnt = cnt.p;
-        a.tab_first = want_counts ? first.p : nullptr;
-        a.tab_last = want_counts ? last.p : nullptr;
-        MG_TRY(launch_scan(ctx, p, a, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(h_small, small.p, sizeof h_small, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-        if (h_small[1] & 1u) continue;                                            // overflow: grow
-        // compact + sort
-        DevBuf<uint64_t> comp, sorted; DevBuf<unsigned long long> d_n;
-        if (comp.alloc(cap) != cudaSuccess || sorted.alloc(cap) != cudaSuccess || d_n.alloc(1) != cudaSuccess)
-            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory in exact re-run");
-        MG_CUDA(ctx, cudaMemsetAsync(d_n.p, 0, 8, st));
-        compact_table_kernel<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(keys.p, cnt.p, mc, cap, comp.p, d_n.p);
-        ctx->kernel_launches++;
+        a.tab_first = positions ? first.p : nullptr;
+        a.tab_last = positions ? last.p : nullptr;
+        a.min_copies = mc;
+        return launch_scan(ctx, p, a, st);
+    }
+
+    // The exactness guard: while the table overflows, or fewer than s hashes survive a threshold that dropped k-mers and is not the
+    // cap, scan again with 8x the survivor factor (ending at keep-all).  Then the bottom-s, ascending, into h_*.
+    int finish()
+    {
+        const uint32_t s = p->sketch_size;
+        uint32_t h_small[4];
         unsigned long long n = 0;
-        MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 8, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-        const uint64_t total = n + ((h_small[2] && h_small[2] >= mc) ? 1 : 0);
-        if (total < s && !keep_all) continue;                                     // still too few: grow
-        size_t tmp_bytes = 0;
-        cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, comp.p, sorted.p, (int)n, 0, 64, st);
-        DevBuf<uint8_t> tmp;
-        if (tmp.alloc(tmp_bytes) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (sort scratch)");
-        if (n) {
-            MG_CUDA(ctx, cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, comp.p, sorted.p, (int)n, 0, 64, st));
-            ctx->kernel_launches += 8;
+        uint64_t total = 0;
+        for (scans = 1;; scans++) {
+            MG_CUDA(ctx, cudaMemcpyAsync(h_small, small.p, sizeof h_small, cudaMemcpyDeviceToHost, st));
+            MG_CUDA(ctx, cudaStreamSynchronize(st));
+            bool again = (h_small[1] & 1u) != 0;
+            if (!again) {
+                const uint64_t cap = 1ull << lg;
+                MG_CUDA(ctx, cudaMemsetAsync(d_n.p, 0, 8, st));
+                compact_table_kernel<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(keys.p, cnt.p, mc, cap, comp.p, d_n.p);
+                ctx->kernel_launches++;
+                MG_CUDA(ctx, cudaGetLastError());
+                MG_CUDA(ctx, cudaMemcpyAsync(&n, d_n.p, 8, cudaMemcpyDeviceToHost, st));
+                MG_CUDA(ctx, cudaStreamSynchronize(st));
+                total = n + (h_small[2] >= mc ? 1 : 0);
+                again = total < s && t != EMPTY_KEY && t != cap_t;
+            }
+            if (!again) break;
+            if (scans == 64) return fail(ctx, MASHGPU_ERR_CUDA, "exact sketch of one unit did not converge");
+            MG_TRY(scan(factor * 8.0, cap_t));
         }
         const uint32_t m = (uint32_t)std::min<uint64_t>(total, s);
-        if (m)
-            emit_sorted_kernel<<<(m + 255) / 256, 256, 0, st>>>(sorted.p, m, keys.p, cnt.p, lg, h_small[2], (uint32_t)n,
-                                                               d_out_hashes + (uint64_t)u * s,
-                                                               d_out_counts ? d_out_counts + (uint64_t)u * s : nullptr);
-        ctx->kernel_launches++;
-        MG_CUDA(ctx, cudaMemcpyAsync(d_out_n + u, &m, 4, cudaMemcpyHostToDevice, st));
-        if (want_counts && m == s) {   // the reference's top-of-heap counting quirk (see quirk_kernel)
-            quirk_kernel<<<1, SEL_THREADS, 0, st>>>(u, 1, s, d_out_hashes, d_out_counts, d_out_n, meta.p + 1 - u, small.p - u, keys.p, cnt.p,
-                                                    first.p, last.p, small.p + 1 - u, meta.p + 2 - u, meta.p + 3 - u, mc);
-            ctx->kernel_launches++;
-            MG_CUDA(ctx, cudaMemcpyAsync(h_small, small.p, sizeof h_small, cudaMemcpyDeviceToHost, st));
-            MG_CUDA(ctx, cudaMemcpyAsync(h_meta, meta.p, sizeof h_meta, cudaMemcpyDeviceToHost, st));
-            MG_CUDA(ctx, cudaStreamSynchronize(st));
-            if (h_small[1] & 8u)
-                MG_TRY(recount_hash(ctx, p, base, S.unit_start[u], h_meta[3], h_meta[2], d_out_counts + (uint64_t)u * s + s - 1, st));
+        if (n) {
+            MG_CUDA(ctx, cub::DeviceRadixSort::SortKeys(sort_tmp.p, sort_tmp_bytes, comp.p, sorted.p, (int)n, 0, 64, st));
+            ctx->kernel_launches += 8;
         }
+        if (m) {
+            unit_emit_kernel<<<(m + 255) / 256, 256, 0, st>>>(sorted.p, (uint32_t)std::min<uint64_t>(n, m), m, keys.p, cnt.p,
+                                                              positions ? first.p : nullptr, last.p, lg, mc, h_small[2], lo, pos_base,
+                                                              c_key.p, c_cnt.p, c_first.p, c_last.p);
+            ctx->kernel_launches++;
+            MG_CUDA(ctx, cudaGetLastError());
+        }
+        h_key.resize(m); h_cnt.resize(m); h_first.resize(m); h_last.resize(m);
+        if (m) {
+            MG_CUDA(ctx, cudaMemcpyAsync(h_key.data(), c_key.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+            MG_CUDA(ctx, cudaMemcpyAsync(h_cnt.data(), c_cnt.p, m * 4ull, cudaMemcpyDeviceToHost, st));
+            if (positions) {
+                MG_CUDA(ctx, cudaMemcpyAsync(h_first.data(), c_first.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+                MG_CUDA(ctx, cudaMemcpyAsync(h_last.data(), c_last.p, m * 8ull, cudaMemcpyDeviceToHost, st));
+            }
+            MG_CUDA(ctx, cudaStreamSynchronize(st));
+        }
+        return MASHGPU_OK;
+    }
+
+    // Occurrences of `key` at positions [unit start, tstar] (tstar as reported, pos_base included) -> *out.
+    int recount(uint64_t key, uint64_t tstar, uint32_t *out)
+    {
+        MG_TRY(recount_hash(ctx, p, base, lo, tstar - pos_base, key, small.p + 3, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(out, small.p + 3, 4, cudaMemcpyDeviceToHost, st));
         MG_CUDA(ctx, cudaStreamSynchronize(st));
         return MASHGPU_OK;
     }
-    return fail(ctx, MASHGPU_ERR_CUDA, "exact re-run of unit %u did not converge", u);
+};
+
+// The bottom-s of a unit sketched in parts (DESIGN.md 2.7, tests/unit_stream_model.py): its hashes, their counts summed over the
+// parts, and the current top's count at positions <= t*.
+struct UnitSketch {
+    std::vector<uint64_t> keys;
+    std::vector<uint32_t> tot;
+    uint32_t top_at_tstar = 0;
+};
+
+// Merge the bottom-s of a pass into R.  A part changes the set only when a hash first seen in it enters; t* is then the latest
+// promoting position among those entrants.  The top's count at positions <= t* is its total before the part plus its occurrences in
+// the part up to t*: all of them when its last position is <= t*, none when it was promoted after t*, mc when it was promoted at t*,
+// otherwise a recount over [part start, t*].  For m = 1 this is MinHashHeap's top-of-heap quirk (MinHashHeap.cpp:70-74), and a
+// merge into an empty state restates quirk_kernel for one unit.
+static int unit_merge(UnitPass &P, UnitSketch &R)
+{
+    const uint32_t s = P.p->sketch_size;
+    const std::vector<uint64_t> &ck = P.h_key, &cf = P.h_first, &cl = P.h_last, &rk = R.keys;
+    const std::vector<uint32_t> &cc = P.h_cnt;
+    const size_t nc = ck.size();
+    std::vector<uint64_t> nk;
+    std::vector<uint32_t> nt;
+    nk.reserve(s); nt.reserve(s);
+    size_t i = 0, j = 0;
+    int64_t top_r = -1, top_c = -1;             // where the last emitted hash came from
+    bool entered = false;
+    uint64_t tstar = 0;
+    while (nk.size() < s && (i < rk.size() || j < nc)) {
+        if (j == nc || (i < rk.size() && rk[i] < ck[j])) { nk.push_back(rk[i]); nt.push_back(R.tot[i]); top_r = (int64_t)i++; top_c = -1; }
+        else if (i == rk.size() || ck[j] < rk[i]) {
+            nk.push_back(ck[j]); nt.push_back(cc[j]); top_r = -1; top_c = (int64_t)j;
+            tstar = entered ? std::max(tstar, cf[j]) : cf[j];
+            entered = true;
+            j++;
+        } else { nk.push_back(rk[i]); nt.push_back(R.tot[i] + cc[j]); top_r = (int64_t)i++; top_c = (int64_t)j++; }
+    }
+    if (entered && P.positions && nk.back() != EMPTY_KEY) {
+        uint32_t part = 0;
+        if (top_c >= 0) {
+            const uint64_t f = cf[top_c], l = cl[top_c];
+            if (l <= tstar) part = cc[top_c];
+            else if (f > tstar) part = 0;
+            else if (f == tstar) part = P.mc;
+            else MG_TRY(P.recount(nk.back(), tstar, &part));
+        }
+        R.top_at_tstar = (top_r >= 0 ? R.tot[top_r] : 0) + part;
+    }
+    R.keys.swap(nk);
+    R.tot.swap(nt);
+    return MASHGPU_OK;
+}
+
+// The reference's counts: a full heap's top counts its occurrences up to t* only.
+static void unit_counts(const UnitSketch &R, uint32_t s, uint32_t *out)
+{
+    std::copy(R.tot.begin(), R.tot.end(), out);
+    if (R.keys.size() == s && R.keys.back() != EMPTY_KEY) out[s - 1] = R.top_at_tstar;
+}
+
+// Exact re-run of flagged unit u: the single-unit pass from 8x the survivor factor, uncapped, merged into an empty state.
+static int rerun_unit(UnitPass &P, const SketchStream &S, uint32_t u, uint64_t *d_out_hashes, uint32_t *d_out_counts, uint32_t *d_out_n)
+{
+    const uint32_t s = P.p->sketch_size;
+    P.ctx->exact_reruns++;
+    P.u = u;
+    P.lo = S.unit_start[u];
+    P.hi = S.unit_start[u + 1];
+    MG_TRY(P.scan(8.0 * SURVIVOR_FACTOR, EMPTY_KEY));
+    MG_TRY(P.finish());
+    UnitSketch R;
+    MG_TRY(unit_merge(P, R));
+    const uint32_t n = (uint32_t)R.keys.size();
+    std::vector<uint32_t> counts(n);
+    unit_counts(R, s, counts.data());
+    MG_CUDA(P.ctx, cudaMemcpyAsync(d_out_hashes + (uint64_t)u * s, R.keys.data(), n * 8ull, cudaMemcpyHostToDevice, P.st));
+    if (d_out_counts) MG_CUDA(P.ctx, cudaMemcpyAsync(d_out_counts + (uint64_t)u * s, counts.data(), n * 4ull, cudaMemcpyHostToDevice, P.st));
+    MG_CUDA(P.ctx, cudaMemcpyAsync(d_out_n + u, &n, 4, cudaMemcpyHostToDevice, P.st));
+    MG_CUDA(P.ctx, cudaStreamSynchronize(P.st));
+    return MASHGPU_OK;
 }
 
 // Core: sketch every unit of a device-resident stream.
@@ -568,18 +752,7 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
     MG_CUDA(ctx, cudaMemsetAsync(d_keys.p, 0xFF, slots * 8ull, st));
     MG_CUDA(ctx, cudaMemsetAsync(d_cnt.p, 0, slots * 4ull, st));
 
-    ScanArgs a;
-    memset(&a, 0, sizeof a);
-    a.stream = (const uint8_t *)S.d_stream;
-    a.codes = S.d_codes;
-    a.inval = S.d_inval;
-    a.stream_len = stream_len;
-    a.tile_begin = 0;
-    a.tile_end = ntiles;
-    a.seed = p->seed;
-    a.use64 = p->use64;
-    a.preserve_case = p->preserve_case;
-    fill_byte_lut(a, p);
+    ScanArgs a = scan_base(p, S.d_stream, stream_len, S.d_codes, S.d_inval);
     a.mode = probe ? SCAN_SCREEN : SCAN_SKETCH;
     a.unit_start = d_start.p;
     a.n_units = n_units;
@@ -592,7 +765,6 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
     a.unit_maxhash = d_maxhash.p;
     a.tab_first = d_first;
     a.tab_last = d_last;
-    a.only_unit = -1;
     a.min_copies = mc;
     if (probe) {
         a.ref_keys = probe->keys; a.ref_idx = probe->idx; a.ref_cnt = probe->cnt; a.ref_log2 = probe->log2cap; a.ref_hmax = probe->hmax;
@@ -674,8 +846,6 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
     }
     MG_CUDA(ctx, cudaMemcpyAsync(ctx->flags_pinned, d_flags.p, n_units * 4ull, cudaMemcpyDeviceToHost, st));
     t.d_qtarget = d_qtarget; t.d_qtstar = d_qtstar;
-    t.scan_args.resize(sizeof(ScanArgs));
-    memcpy(t.scan_args.data(), &a, sizeof(ScanArgs));
     t.active = true;
     return MASHGPU_OK;
 }
@@ -691,8 +861,6 @@ int sketch_stream_finalize(mashgpu_ctx *ctx, SketchTicket &t)
     cudaStream_t st = t.st;
     uint64_t *d_out_hashes = t.d_out_hashes; uint32_t *d_out_counts = t.d_out_counts, *d_out_n = t.d_out_n;
     uint64_t *d_qtarget = t.d_qtarget, *d_qtstar = t.d_qtstar;
-    ScanArgs a;
-    memcpy(&a, t.scan_args.data(), sizeof(ScanArgs));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     const uint32_t *h_flags = (const uint32_t *)ctx->flags_pinned;
     bool any_flag = false;
@@ -707,11 +875,21 @@ int sketch_stream_finalize(mashgpu_ctx *ctx, SketchTicket &t)
         MG_CUDA(ctx, cudaMemcpyAsync(h_qtstar.data(), d_qtstar, n_units * 8ull, cudaMemcpyDeviceToHost, st));
         MG_CUDA(ctx, cudaStreamSynchronize(st));
     }
+    // re-runs and recounts scan the pass's stream again, finding units through its device copy of unit_start
+    ScanArgs a = scan_base(p, S.d_stream, S.unit_start[n_units], S.d_codes, S.d_inval);
+    a.unit_start = static_cast<const uint64_t *>(ctx->sc_start.p);
+    a.n_units = n_units;
+    UnitPass pass;
+    uint64_t pass_bytes = 0, pass_peak = 0;
     for (uint32_t u = 0; u < n_units; u++) {
         if (h_flags[u] == 0) continue;
-        a.mode = SCAN_SKETCH;    // reference-table hits were already counted in the first pass
-        if (h_flags[u] & 7u) MG_TRY(rerun_unit(ctx, p, S, u, d_out_hashes, d_out_counts, d_out_n, st, a));
-        else MG_TRY(recount_hash(ctx, p, a, S.unit_start[u], h_qtstar[u], h_qtarget[u], d_out_counts + (uint64_t)u * s + s - 1, st));
+        if (h_flags[u] & 7u) {
+            if (!pass.ctx) {
+                MG_TRY(pass.open(ctx, p, st, d_out_counts != nullptr, &pass_bytes, &pass_peak));
+                pass.base = a;
+            }
+            MG_TRY(rerun_unit(pass, S, u, d_out_hashes, d_out_counts, d_out_n));
+        } else MG_TRY(recount_hash(ctx, p, a, S.unit_start[u], h_qtstar[u], h_qtarget[u], d_out_counts + (uint64_t)u * s + s - 1, st));
     }
     if (any_recount) MG_CUDA(ctx, cudaStreamSynchronize(st));
     return MASHGPU_OK;
@@ -1623,21 +1801,10 @@ struct mashgpu_reads_job {
 
 namespace mashgpu {
 
-static uint64_t reads_env(const char *name, uint64_t dflt, uint64_t lo)
+static uint64_t env_u64(const char *name, uint64_t dflt, uint64_t lo)
 {
     const char *env = getenv(name);
     return env ? std::max<uint64_t>(lo, strtoull(env, nullptr, 10)) : dflt;
-}
-
-template <typename T>
-static bool reads_alloc(mashgpu_reads_job *job, DevBuf<T> &b, size_t n)
-{
-    const size_t before = b.n * sizeof(T);
-    if (b.alloc(n) != cudaSuccess) return false;
-    job->dev_bytes += n * sizeof(T);
-    job->dev_bytes -= before;
-    job->ctx->reads_peak_bytes = std::max(job->ctx->reads_peak_bytes, job->dev_bytes);
-    return true;
 }
 
 // Pending tables for `extra` more entries at load <= 1/2 (grown on the device, before the replay launch that needs them).
@@ -1649,7 +1816,7 @@ static int reads_reserve_pending(mashgpu_reads_job *job, uint64_t pend_n, uint64
     if (need + 2 > job->cap_ph) {
         uint64_t cap = std::max<uint64_t>(2 * job->cap_ph, need + 2);
         DevBuf<uint64_t> nh;
-        if (!reads_alloc(job, nh, cap)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending heap of %llu)", (unsigned long long)cap);
+        if (!tracked_alloc(nh, cap, job->dev_bytes, ctx->reads_peak_bytes)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending heap of %llu)", (unsigned long long)cap);
         if (pend_n) MG_CUDA(ctx, cudaMemcpyAsync(nh.p, job->p_heap.p, pend_n * 8, cudaMemcpyDeviceToDevice, st));
         MG_CUDA(ctx, cudaStreamSynchronize(st));
         job->dev_bytes -= job->p_heap.n * 8;
@@ -1660,7 +1827,7 @@ static int reads_reserve_pending(mashgpu_reads_job *job, uint64_t pend_n, uint64
         uint64_t cap = std::max<uint64_t>(16, job->cap_p);
         while (cap < 2 * need + 16) cap <<= 1;
         DevBuf<uint64_t> nk; DevBuf<uint32_t> nc;
-        if (!reads_alloc(job, nk, cap) || !reads_alloc(job, nc, cap)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending map of %llu)", (unsigned long long)cap);
+        if (!tracked_alloc(nk, cap, job->dev_bytes, ctx->reads_peak_bytes) || !tracked_alloc(nc, cap, job->dev_bytes, ctx->reads_peak_bytes)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pending map of %llu)", (unsigned long long)cap);
         MG_CUDA(ctx, cudaMemsetAsync(nc.p, 0, cap * 4, st));
         if (job->cap_p) {
             ReplayMap from{job->p_key.p, job->p_cnt.p, job->cap_p - 1}, to{nk.p, nc.p, cap - 1};
@@ -1688,14 +1855,10 @@ static int reads_process_stage(mashgpu_reads_job *job)
     if (len == 0 || job->stopped) return MASHGPU_OK;
     MG_CUDA(ctx, cudaMemcpyAsync(job->d_stage.p, job->stage.h(), len, cudaMemcpyHostToDevice, st));
     if (n_rec) MG_CUDA(ctx, cudaMemcpyAsync(job->d_rec_end.p, job->stage.rec_end.data(), n_rec * 8, cudaMemcpyHostToDevice, st));
-    ScanArgs a;
-    memset(&a, 0, sizeof a);
-    a.stream = job->d_stage.p; a.stream_len = len;
+    ScanArgs a = scan_base(p, job->d_stage.p, len);
     a.tile_tmax = job->d_tmax.p;
-    a.seed = p->seed; a.use64 = p->use64; a.preserve_case = p->preserve_case;
-    fill_byte_lut(a, p);
-    a.mode = SCAN_EVENTS; a.only_unit = -1; a.min_copies = 1;
-    a.unit_start = nullptr; a.n_units = 1; a.unit_t = &job->d_state.p->gate_t;
+    a.mode = SCAN_EVENTS;
+    a.unit_t = &job->d_state.p->gate_t;
     a.ev_pos = job->ev_pos.p; a.ev_hash = job->ev_hash.p; a.ev_count = &job->d_state.p->ev_count; a.ev_capacity = job->ev_cap;
     const uint64_t ntiles = (len + SCAN_TILE - 1) / SCAN_TILE;
     const double space = p->use64 ? 18446744073709551616.0 : 4294967296.0;
@@ -1786,8 +1949,8 @@ extern "C" int mashgpu_reads_open(mashgpu_ctx *ctx, const mashgpu_sketch_params 
     job->s = params->sketch_size;
     job->m = std::max(1u, params->min_copies);
     job->k = (uint64_t)params->kmer_size;
-    const uint64_t stage_cap = reads_env("MASHGPU_READS_STAGE_BYTES", 128ull << 20, 4 * job->k + 64);
-    job->ev_cap = std::min<uint64_t>(reads_env("MASHGPU_READS_EVENT_CAP", 1ull << 21, SCAN_TILE), 1ull << 30);    // cub takes int counts
+    const uint64_t stage_cap = env_u64("MASHGPU_READS_STAGE_BYTES", 128ull << 20, 4 * job->k + 64);
+    job->ev_cap = std::min<uint64_t>(env_u64("MASHGPU_READS_EVENT_CAP", 1ull << 21, SCAN_TILE), 1ull << 30);    // cub takes int counts
     job->bloom_bits = params->bloom_bytes * 8;
     ctx->reads_peak_bytes = 0;
     cudaStream_t st = ctx->stream;
@@ -1799,12 +1962,13 @@ extern "C" int mashgpu_reads_open(mashgpu_ctx *ctx, const mashgpu_sketch_params 
                                     (int)job->ev_cap, 0, 64, st);
     if (job->stage.open(stage_cap, job->k, 1) != cudaSuccess || job->h_state.alloc(1) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory");
-    if (!reads_alloc(job, job->d_stage, ((stage_cap + 15) / 16) * 16 + 64) || !reads_alloc(job, job->d_rec_end, max_rec) ||
-        !reads_alloc(job, job->d_tmax, max_tiles) || !reads_alloc(job, job->ev_pos, job->ev_cap) || !reads_alloc(job, job->ev_hash, job->ev_cap) ||
-        !reads_alloc(job, job->ev_pos2, job->ev_cap) || !reads_alloc(job, job->ev_hash2, job->ev_cap) || (job->bloom_bits && !reads_alloc(job, job->ev_bit, job->ev_cap)) ||
-        !reads_alloc(job, job->sort_tmp, job->sort_tmp_bytes) || !reads_alloc(job, job->d_state, 1) || !reads_alloc(job, job->a_key, job->cap_a) ||
-        !reads_alloc(job, job->a_cnt, job->cap_a) || !reads_alloc(job, job->a_heap, job->s + 2) ||
-        (job->bloom_bits && !reads_alloc(job, job->bloom, (std::min(params->bloom_bytes, BLOOM_MAX_BYTES) + 3) / 4)))
+    auto alloc = [&](auto &b, size_t n) { return tracked_alloc(b, n, job->dev_bytes, ctx->reads_peak_bytes); };
+    if (!alloc(job->d_stage, ((stage_cap + 15) / 16) * 16 + 64) || !alloc(job->d_rec_end, max_rec) ||
+        !alloc(job->d_tmax, max_tiles) || !alloc(job->ev_pos, job->ev_cap) || !alloc(job->ev_hash, job->ev_cap) ||
+        !alloc(job->ev_pos2, job->ev_cap) || !alloc(job->ev_hash2, job->ev_cap) || (job->bloom_bits && !alloc(job->ev_bit, job->ev_cap)) ||
+        !alloc(job->sort_tmp, job->sort_tmp_bytes) || !alloc(job->d_state, 1) || !alloc(job->a_key, job->cap_a) ||
+        !alloc(job->a_cnt, job->cap_a) || !alloc(job->a_heap, job->s + 2) ||
+        (job->bloom_bits && !alloc(job->bloom, (std::min(params->bloom_bytes, BLOOM_MAX_BYTES) + 3) / 4)))
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (reads job)");
     MG_CUDA(ctx, cudaMemsetAsync(job->a_cnt.p, 0, job->cap_a * 4, st));
     if (job->bloom_bits) MG_CUDA(ctx, cudaMemsetAsync(job->bloom.p, 0, job->bloom.n * 4, st));
@@ -1882,28 +2046,9 @@ extern "C" int mashgpu_reads_close(mashgpu_reads_job *job)
 // ---------------------------------------------------------------------------------------------------------
 // Streaming unit job (mashgpu_unit_*, DESIGN.md 2.7): one sketchFile unit with minCov 1 and no Bloom filter, of any size, in device
 // memory fixed by the parameters.  The bottom-s of a set does not depend on order, so each stage of the stream is sketched on its
-// own -- the one-unit pass of sketch_stream_core, with the running s-th smallest hash as the threshold once s hashes are held --
-// and its bottom-s (count, first and last position of each hash) is merged into the running state: the bottom-s hashes, their
-// summed counts, and the current top's count at positions <= t* (tests/unit_stream_model.py restates the merge).
+// own by the single-unit pass, with the running s-th smallest hash as the cap of its threshold once s hashes are held, and its
+// bottom-s (count, first and last position of each hash) is merged into the running state (unit_merge).
 // ---------------------------------------------------------------------------------------------------------
-namespace mashgpu {
-
-// The stage's bottom-s, ascending, with the count and the global first / last position of each hash.
-__global__ void unit_emit_kernel(const uint64_t *sorted, uint32_t m, const uint64_t *keys, const uint32_t *cnt, const uint64_t *first,
-                                 const uint64_t *last, uint32_t log2cap, uint64_t base, uint64_t *c_key, uint32_t *c_cnt, uint64_t *c_first,
-                                 uint64_t *c_last)
-{
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const uint64_t key = sorted[i];
-    const int64_t slot = table_find(keys, log2cap, key);
-    c_key[i] = key;
-    c_cnt[i] = cnt[slot];
-    c_first[i] = base + first[slot];
-    c_last[i] = base + last[slot];
-}
-
-}  // namespace mashgpu
 
 struct mashgpu_unit_job {
     mashgpu_ctx *ctx = nullptr;
@@ -1912,205 +2057,30 @@ struct mashgpu_unit_job {
     mashgpu::RecordStage stage;                 // two pinned buffers: one fills while the other is copied
     mashgpu::DevBuf<uint8_t> d_stage[2];
     cudaEvent_t copied[2] = {nullptr, nullptr};
-    // the stage in flight: scanned (or being scanned), not merged yet
-    int pending = -1;                           // its buffer, -1 = none
-    uint64_t pend_len = 0, pend_base = 0;       // its length and the global stream position of its first byte
-    uint64_t pend_t = 0;                        // its threshold
-    uint32_t pend_lg = 0;                       // log2 of its table's capacity
-    double pend_factor = 0;                     // its plan_unit survivor factor
+    int pending = -1;                           // buffer of the stage in flight (scanned or being scanned, not merged), -1 = none
     uint64_t next_base = 0;                     // global stream position of the next stage's first byte
-    // candidate table of one stage, its compaction and sort
-    mashgpu::DevBuf<uint64_t> t_keys, t_first, t_last, comp, sorted, c_key, c_first, c_last, d_meta;   // d_meta: [threshold, 0]
-    mashgpu::DevBuf<uint32_t> t_cnt, c_cnt, d_small;       // d_small: [log2, flags, maxhash, recount]
-    mashgpu::DevBuf<unsigned long long> d_n;
-    mashgpu::DevBuf<uint8_t> sort_tmp;
-    size_t sort_tmp_bytes = 0;
-    uint32_t lg_cap = 0;                        // capacity of the table buffers
-    // running state
-    std::vector<uint64_t> keys;                 // bottom-s so far, ascending
-    std::vector<uint32_t> tot;                  // their counts summed over the stages
-    uint32_t top_at_tstar = 0;                  // the top's count at positions <= t*
+    mashgpu::UnitPass pass;                     // the stage in flight: unit 0 of its buffer, positions + its global start
+    mashgpu::UnitSketch sketch;                 // running state
     bool finished = false;
     uint64_t dev_bytes = 0;
 };
 
 namespace mashgpu {
 
-template <typename T>
-static bool unit_alloc(mashgpu_unit_job *job, DevBuf<T> &b, size_t n)
-{
-    const size_t before = b.n * sizeof(T);
-    if (b.alloc(n) != cudaSuccess) return false;
-    job->dev_bytes += n * sizeof(T);
-    job->dev_bytes -= before;
-    job->ctx->unit_peak_bytes = std::max(job->ctx->unit_peak_bytes, job->dev_bytes);
-    return true;
-}
-
-// Table, compaction and sort buffers for 2^lg slots (grown only by a re-run that needs a larger table).
-static int unit_reserve_table(mashgpu_unit_job *job, uint32_t lg)
-{
-    if (lg <= job->lg_cap) return MASHGPU_OK;
-    const uint64_t cap = 1ull << lg;
-    size_t tmp = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, tmp, (uint64_t *)nullptr, (uint64_t *)nullptr, (int)cap, 0, 64, job->ctx->stream);
-    if (!unit_alloc(job, job->t_keys, cap) || !unit_alloc(job, job->t_cnt, cap) || !unit_alloc(job, job->t_first, cap) ||
-        !unit_alloc(job, job->t_last, cap) || !unit_alloc(job, job->comp, cap) || !unit_alloc(job, job->sorted, cap) ||
-        !unit_alloc(job, job->sort_tmp, tmp))
-        return fail(job->ctx, MASHGPU_ERR_NOMEM, "out of device memory (unit job table of %llu slots)", (unsigned long long)cap);
-    job->sort_tmp_bytes = tmp;
-    job->lg_cap = lg;
-    return MASHGPU_OK;
-}
-
-// Threshold and table of the pending stage for a survivor factor; once s hashes are held nothing above the running top can enter.
-static int unit_plan(mashgpu_unit_job *job, double factor)
-{
-    plan_unit(&job->params, job->pend_len, factor, &job->pend_t, &job->pend_lg);
-    if (job->keys.size() == job->s) job->pend_t = std::min(job->pend_t, job->keys.back());
-    job->pend_factor = factor;
-    return unit_reserve_table(job, job->pend_lg);
-}
-
-static ScanArgs unit_scan_args(mashgpu_unit_job *job)
-{
-    const mashgpu_sketch_params *p = &job->params;
-    ScanArgs a;
-    memset(&a, 0, sizeof a);
-    a.stream = job->d_stage[job->pending].p;
-    a.stream_len = job->pend_len;
-    a.tile_begin = 0;
-    a.tile_end = (job->pend_len + SCAN_TILE - 1) / SCAN_TILE;
-    a.coarse_t = job->pend_t;
-    a.seed = p->seed; a.use64 = p->use64; a.preserve_case = p->preserve_case;
-    fill_byte_lut(a, p);
-    a.mode = SCAN_SKETCH;
-    a.unit_start = nullptr;          // one unit: the scan never looks a unit up
-    a.n_units = 1;
-    a.unit_t = job->d_meta.p;
-    a.tab_off = job->d_meta.p + 1;
-    a.tab_log2 = job->d_small.p;
-    a.unit_flags = job->d_small.p + 1;
-    a.unit_maxhash = job->d_small.p + 2;
-    a.tab_keys = job->t_keys.p; a.tab_cnt = job->t_cnt.p; a.tab_first = job->t_first.p; a.tab_last = job->t_last.p;
-    a.only_unit = -1;
-    a.min_copies = 1;
-    return a;
-}
-
-// Enqueue the scan of the pending stage into a cleared table (after its copy has landed).
-static int unit_scan(mashgpu_unit_job *job)
-{
-    mashgpu_ctx *ctx = job->ctx;
-    cudaStream_t st = ctx->stream;
-    const uint64_t cap = 1ull << job->pend_lg;
-    MG_CUDA(ctx, cudaMemsetAsync(job->t_keys.p, 0xFF, cap * 8, st));
-    MG_CUDA(ctx, cudaMemsetAsync(job->t_cnt.p, 0, cap * 4, st));
-    MG_CUDA(ctx, cudaMemsetAsync(job->t_first.p, 0xFF, cap * 8, st));
-    MG_CUDA(ctx, cudaMemsetAsync(job->t_last.p, 0, cap * 8, st));
-    const uint64_t meta[2] = {job->pend_t, 0};
-    const uint32_t small[4] = {job->pend_lg, 0, 0, 0};
-    MG_CUDA(ctx, cudaMemcpyAsync(job->d_meta.p, meta, sizeof meta, cudaMemcpyHostToDevice, st));
-    MG_CUDA(ctx, cudaMemcpyAsync(job->d_small.p, small, sizeof small, cudaMemcpyHostToDevice, st));
-    MG_CUDA(ctx, cudaStreamWaitEvent(st, job->copied[job->pending], 0));
-    return launch_scan(ctx, &job->params, unit_scan_args(job), st);
-}
-
-// Finish the pending stage: exactness guard (re-run with a larger threshold while its bytes are resident), its bottom-s, and the merge.
+// Finish the pending stage: exactness guard (re-scans while its bytes are resident), its bottom-s, and the merge.
 static int unit_complete(mashgpu_unit_job *job)
 {
     if (job->pending < 0) return MASHGPU_OK;
-    mashgpu_ctx *ctx = job->ctx;
-    cudaStream_t st = ctx->stream;
-    const uint32_t s = job->s;
-    uint32_t small[4];
-    unsigned long long n = 0;
-    for (;;) {
-        MG_CUDA(ctx, cudaMemcpyAsync(small, job->d_small.p, sizeof small, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-        bool rerun = (small[1] & 1u) != 0;                                          // table overflow
-        if (!rerun) {
-            const uint64_t cap = 1ull << job->pend_lg;
-            MG_CUDA(ctx, cudaMemsetAsync(job->d_n.p, 0, 8, st));
-            compact_table_kernel<<<(unsigned)((cap + 255) / 256), 256, 0, st>>>(job->t_keys.p, job->t_cnt.p, 1, cap, job->comp.p, job->d_n.p);
-            ctx->kernel_launches++;
-            MG_CUDA(ctx, cudaGetLastError());
-            MG_CUDA(ctx, cudaMemcpyAsync(&n, job->d_n.p, 8, cudaMemcpyDeviceToHost, st));
-            MG_CUDA(ctx, cudaStreamSynchronize(st));
-            // fewer than s survivors although k-mers were dropped: the stage's bottom-s may lie above the threshold -- unless the
-            // threshold is the running top, above which nothing can enter
-            const uint64_t total = n + (small[2] ? 1 : 0);
-            const bool capped = job->keys.size() == s && job->pend_t == job->keys.back();
-            rerun = total < s && job->pend_t != EMPTY_KEY && !capped;
-        }
-        if (!rerun) break;
-        ctx->exact_reruns++;
-        MG_TRY(unit_plan(job, job->pend_factor * 8.0));
-        MG_TRY(unit_scan(job));
-    }
-    const uint32_t m = (uint32_t)std::min<uint64_t>(n, s);
-    if (n) {
-        MG_CUDA(ctx, cub::DeviceRadixSort::SortKeys(job->sort_tmp.p, job->sort_tmp_bytes, job->comp.p, job->sorted.p, (int)n, 0, 64, st));
-        ctx->kernel_launches += 8;
-        unit_emit_kernel<<<(m + 255) / 256, 256, 0, st>>>(job->sorted.p, m, job->t_keys.p, job->t_cnt.p, job->t_first.p, job->t_last.p,
-                                                          job->pend_lg, job->pend_base, job->c_key.p, job->c_cnt.p, job->c_first.p, job->c_last.p);
-        ctx->kernel_launches++;
-        MG_CUDA(ctx, cudaGetLastError());
-    }
-    std::vector<uint64_t> ck(m + 1), cf(m + 1), cl(m + 1);
-    std::vector<uint32_t> cc(m + 1);
-    if (m) {
-        MG_CUDA(ctx, cudaMemcpyAsync(ck.data(), job->c_key.p, m * 8ull, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(cc.data(), job->c_cnt.p, m * 4ull, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(cf.data(), job->c_first.p, m * 8ull, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(cl.data(), job->c_last.p, m * 8ull, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    uint32_t nc = m;
-    if (small[2] && m < s) { ck[nc] = EMPTY_KEY; cc[nc] = small[2]; cf[nc] = cl[nc] = job->pend_base; nc++; }   // 2^64-1: not a table key
-    // merge: bottom-s of the union, counts summed; t* = the latest first occurrence among the hashes that entered in this stage
-    std::vector<uint64_t> nk; std::vector<uint32_t> nt;
-    nk.reserve(s); nt.reserve(s);
-    const std::vector<uint64_t> &rk = job->keys;
-    size_t i = 0, j = 0;
-    int64_t top_r = -1, top_c = -1;             // where the last emitted hash came from
-    bool entered = false;
-    uint64_t tstar = 0;
-    while (nk.size() < s && (i < rk.size() || j < nc)) {
-        if (j == nc || (i < rk.size() && rk[i] < ck[j])) { nk.push_back(rk[i]); nt.push_back(job->tot[i]); top_r = (int64_t)i++; top_c = -1; }
-        else if (i == rk.size() || ck[j] < rk[i]) {
-            nk.push_back(ck[j]); nt.push_back(cc[j]); top_r = -1; top_c = (int64_t)j;
-            tstar = entered ? std::max(tstar, cf[j]) : cf[j];
-            entered = true;
-            j++;
-        } else { nk.push_back(rk[i]); nt.push_back(job->tot[i] + cc[j]); top_r = (int64_t)i++; top_c = (int64_t)j++; }
-    }
-    if (entered && nk.back() != EMPTY_KEY) {
-        // the top's count at positions <= t*: its total before this stage plus its occurrences in the stage up to t*, which its first
-        // and last positions in the stage usually decide; otherwise count them over [stage start, t*] of the still-resident stage
-        uint32_t part = 0;
-        if (top_c >= 0) {
-            const uint64_t f = cf[top_c], l = cl[top_c];
-            if (l <= tstar) part = cc[top_c];
-            else if (f > tstar) part = 0;
-            else if (f == tstar) part = 1;
-            else {
-                MG_TRY(recount_hash(ctx, &job->params, unit_scan_args(job), 0, tstar - job->pend_base, nk.back(), job->d_small.p + 3, st));
-                MG_CUDA(ctx, cudaMemcpyAsync(&part, job->d_small.p + 3, 4, cudaMemcpyDeviceToHost, st));
-                MG_CUDA(ctx, cudaStreamSynchronize(st));
-            }
-        }
-        job->top_at_tstar = (top_r >= 0 ? job->tot[top_r] : 0) + part;
-    }
-    job->keys.swap(nk);
-    job->tot.swap(nt);
+    MG_TRY(job->pass.finish());
+    job->ctx->exact_reruns += job->pass.scans - 1;
+    MG_TRY(unit_merge(job->pass, job->sketch));
     job->pending = -1;
-    ctx->unit_stages++;
+    job->ctx->unit_stages++;
     return MASHGPU_OK;
 }
 
-// The current buffer is full (or the unit ends): copy it to the device, merge the stage before it (whose running top is this stage's
-// threshold), then enqueue this stage's scan.  The host fills the other buffer while the scan runs.
+// The current buffer is full (or the unit ends): copy it to the device, merge the stage before it (whose running top caps this
+// stage's threshold), then enqueue this stage's scan.  The host fills the other buffer while the scan runs.
 static int unit_process(mashgpu_unit_job *job)
 {
     mashgpu_ctx *ctx = job->ctx;
@@ -2121,11 +2091,14 @@ static int unit_process(mashgpu_unit_job *job)
     MG_CUDA(ctx, cudaEventRecord(job->copied[b], ctx->copy_stream));
     MG_TRY(unit_complete(job));
     job->pending = b;
-    job->pend_len = len;
-    job->pend_base = job->next_base;
+    UnitPass &P = job->pass;
+    P.base = scan_base(&job->params, job->d_stage[b].p, len);
+    P.hi = len;
+    P.pos_base = job->next_base;
     job->next_base += len - job->stage.carry.size();      // the next stage starts with the carried k-1 bases
-    MG_TRY(unit_plan(job, SURVIVOR_FACTOR));
-    return unit_scan(job);
+    const std::vector<uint64_t> &keys = job->sketch.keys;
+    MG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, job->copied[b], 0));
+    return P.scan(SURVIVOR_FACTOR, keys.size() == job->s ? keys.back() : EMPTY_KEY);
 }
 
 static int unit_flush(mashgpu_unit_job *job, bool record_continues)
@@ -2177,19 +2150,19 @@ extern "C" int mashgpu_unit_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *
     job->params = *params;
     job->s = params->sketch_size;
     const uint64_t k = (uint64_t)params->kmer_size;
-    const uint64_t stage_cap = reads_env("MASHGPU_UNIT_STAGE_BYTES", 128ull << 20, 4 * k + 64);
+    const uint64_t stage_cap = env_u64("MASHGPU_UNIT_STAGE_BYTES", 128ull << 20, 4 * k + 64);
     ctx->unit_peak_bytes = 0;
     if (job->stage.open(stage_cap, k, 2) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (unit job staging)");
     const uint64_t d_stage_bytes = ((stage_cap + 15) / 16) * 16 + 64;
-    if (!unit_alloc(job, job->d_stage[0], d_stage_bytes) || !unit_alloc(job, job->d_stage[1], d_stage_bytes) || !unit_alloc(job, job->d_meta, 2) ||
-        !unit_alloc(job, job->d_small, 4) || !unit_alloc(job, job->d_n, 1) || !unit_alloc(job, job->c_key, job->s) ||
-        !unit_alloc(job, job->c_cnt, job->s) || !unit_alloc(job, job->c_first, job->s) || !unit_alloc(job, job->c_last, job->s))
+    if (!tracked_alloc(job->d_stage[0], d_stage_bytes, job->dev_bytes, ctx->unit_peak_bytes) ||
+        !tracked_alloc(job->d_stage[1], d_stage_bytes, job->dev_bytes, ctx->unit_peak_bytes))
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (unit job)");
+    MG_TRY(job->pass.open(ctx, &job->params, ctx->stream, true, &job->dev_bytes, &ctx->unit_peak_bytes));
     // the table of any stage's first pass: a full stage, or a short one that plan_unit keeps whole (span <= 6 s)
     uint64_t t; uint32_t lg_full, lg_short;
     plan_unit(params, stage_cap, SURVIVOR_FACTOR, &t, &lg_full);
     plan_unit(params, std::min<uint64_t>(stage_cap, 2 * (uint64_t)(SURVIVOR_FACTOR * job->s) + 2), SURVIVOR_FACTOR, &t, &lg_short);
-    MG_TRY(unit_reserve_table(job, std::max(lg_full, lg_short)));
+    MG_TRY(job->pass.reserve(std::max(lg_full, lg_short)));
     MG_CUDA(ctx, cudaEventCreateWithFlags(&job->copied[0], cudaEventDisableTiming));
     MG_CUDA(ctx, cudaEventCreateWithFlags(&job->copied[1], cudaEventDisableTiming));
     *out = guard.release();
@@ -2220,13 +2193,10 @@ extern "C" int mashgpu_unit_finish(mashgpu_unit_job *job, uint64_t *out_hashes, 
         MG_TRY(unit_complete(job));
         job->finished = true;
     }
-    const size_t n = job->keys.size();
-    std::copy(job->keys.begin(), job->keys.end(), out_hashes);
-    if (out_counts) {
-        std::copy(job->tot.begin(), job->tot.end(), out_counts);
-        // the reference's top-of-heap quirk (quirk_kernel): a full heap's top counts its occurrences up to t* only
-        if (n == job->s && job->keys.back() != EMPTY_KEY) out_counts[n - 1] = job->top_at_tstar;
-    }
+    const std::vector<uint64_t> &keys = job->sketch.keys;
+    const size_t n = keys.size();
+    std::copy(keys.begin(), keys.end(), out_hashes);
+    if (out_counts) unit_counts(job->sketch, job->s, out_counts);
     *out_n = (uint32_t)n;
     *out_length = job->stage.bases;
     *out_records = job->stage.records;
@@ -2382,14 +2352,9 @@ extern "C" int mashgpu_hash_windows(mashgpu_ctx *ctx, const mashgpu_sketch_param
     MG_CUDA(ctx, cudaMemcpyAsync(d_seq.p, seq, len, cudaMemcpyHostToDevice, st));
     MG_CUDA(ctx, cudaMemsetAsync(d_valid.p, 0, len, st));
     MG_CUDA(ctx, cudaMemsetAsync(d_hash.p, 0, len * 8, st));
-    ScanArgs a;
-    memset(&a, 0, sizeof a);
-    a.stream = d_seq.p; a.stream_len = len;
-    a.tile_begin = 0; a.tile_end = (len + SCAN_TILE - 1) / SCAN_TILE;
+    ScanArgs a = scan_base(params, d_seq.p, len);
     a.coarse_t = EMPTY_KEY;
-    a.seed = params->seed; a.use64 = params->use64; a.preserve_case = params->preserve_case;
-    fill_byte_lut(a, params);
-    a.mode = SCAN_DUMP; a.only_unit = -1;
+    a.mode = SCAN_DUMP;
     a.out_hash = d_hash.p; a.out_valid = d_valid.p;
     MG_TRY(launch_scan(ctx, params, a, st));
     MG_CUDA(ctx, cudaMemcpyAsync(out_hash, d_hash.p, nwin * 8, cudaMemcpyDeviceToHost, st));

@@ -32,7 +32,8 @@ struct ScreenProbe {
 
 // One sketch_stream pass in flight: the kernels are enqueued by sketch_stream_enqueue and the per-unit status flags come back
 // into pinned memory; sketch_stream_finalize waits for them and re-runs flagged units exactly.  The stream data, the output
-// buffers and the context's scratch must stay untouched between the two calls (one ticket in flight per context).
+// buffers and the context's scratch (the re-runs find units through its copy of unit_start) must stay untouched between the two
+// calls (one ticket in flight per context).
 struct SketchTicket {
     bool active = false;
     mashgpu_sketch_params params{};
@@ -41,7 +42,6 @@ struct SketchTicket {
     uint64_t *d_out_hashes = nullptr; uint32_t *d_out_counts = nullptr, *d_out_n = nullptr;
     cudaStream_t st = nullptr;
     uint64_t *d_qtarget = nullptr, *d_qtstar = nullptr;
-    std::vector<uint8_t> scan_args;         // the ScanArgs of the pass (base of the re-runs), kept opaque here
 };
 
 // reads = the entry point is a reads-mode path (the only ones that take bloom_bytes)

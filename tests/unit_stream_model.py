@@ -6,6 +6,9 @@ count, first and last position, merged into the running set.  A stage changes th
 t* (the latest first occurrence among the set's hashes) then lies in that stage, and the top's count at positions <= t* is its
 total before the stage plus its occurrences in the stage up to t*.  The result must equal MinHashHeap with m = 1
 (reads_stream_model.ReferenceHeap) fed every hash in order, for any stage boundaries.
+
+`unit_merge` in sketch.cu is the device code's one copy of this rule: the unit job applies it per stage, and the exact re-run of a
+flagged unit applies it once, as a merge into an empty state (with m > 1, the promoting m-th occurrence stands for the first).
 """
 import numpy as np
 
