@@ -54,15 +54,10 @@ extern "C" void mashgpu_destroy(mashgpu_ctx *ctx)
     for (auto *list : {&ctx->scan_events, &ctx->dist_events, &ctx->tax_events})
         for (auto &ev : *list) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     for (int b = 0; b < 2; b++) {
-        if (ctx->pinned[b]) cudaFreeHost(ctx->pinned[b]);
-        if (ctx->pinned_sep[b]) cudaFreeHost(ctx->pinned_sep[b]);
         if (ctx->wave_copied[b]) cudaEventDestroy(ctx->wave_copied[b]);
-        if (ctx->pinned_codes[b]) cudaFreeHost(ctx->pinned_codes[b]);
         if (ctx->pack_copied[b]) cudaEventDestroy(ctx->pack_copied[b]);
-        if (ctx->scr_pinned[b]) cudaFreeHost(ctx->scr_pinned[b]);
     }
     if (ctx->pack_stream) cudaStreamDestroy(ctx->pack_stream);
-    if (ctx->flags_pinned) cudaFreeHost(ctx->flags_pinned);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     delete ctx;

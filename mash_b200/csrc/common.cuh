@@ -17,23 +17,24 @@ struct EventPair { cudaEvent_t a, b; };
 }  // namespace mashgpu
 
 namespace mashgpu {
-// grow-only device scratch owned by the context (no cudaMalloc/cudaFree on the hot path after warm-up)
-struct Scratch {
+// grow-only buffer owned by the context (no allocation on the hot path after warm-up); growing discards the contents
+template <cudaError_t (*Alloc)(void **, size_t), cudaError_t (*Free)(void *)>
+struct GrowBuf {
     void *p = nullptr;
     size_t bytes = 0;
-    ~Scratch() { if (p) cudaFree(p); }
+    ~GrowBuf() { if (p) Free(p); }
     template <typename T>
     T *get(size_t count)
     {
         size_t need = count * sizeof(T);
         if (need == 0) need = 16;
         if (need > bytes) {
-            if (p) cudaFree(p);
+            if (p) Free(p);
             p = nullptr; bytes = 0;
             size_t want = need + need / 8;
-            if (cudaMalloc(&p, want) != cudaSuccess) {
+            if (Alloc(&p, want) != cudaSuccess) {
                 cudaGetLastError();
-                if (cudaMalloc(&p, need) != cudaSuccess) { cudaGetLastError(); p = nullptr; return nullptr; }
+                if (Alloc(&p, need) != cudaSuccess) { cudaGetLastError(); p = nullptr; return nullptr; }
                 want = need;
             }
             bytes = want;
@@ -41,6 +42,8 @@ struct Scratch {
         return reinterpret_cast<T *>(p);
     }
 };
+using Scratch = GrowBuf<cudaMalloc, cudaFree>;              // device memory
+using PinnedScratch = GrowBuf<cudaMallocHost, cudaFreeHost>;  // page-locked host memory
 }  // namespace mashgpu
 
 struct mashgpu_ctx {
@@ -65,21 +68,16 @@ struct mashgpu_ctx {
     mashgpu::Scratch sc_wave[2], sc_inval[2], sc_runs[2], sc_out_hashes, sc_out_n, sc_out_counts;
     mashgpu::Scratch sc_sep[2], sc_codes[2];
     mashgpu::Scratch sc_big_units, sc_big_n, sc_big_off, sc_big_bounds, sc_big_comp, sc_big_sorted, sc_big_tmp;   // select of tables > 2^14 slots
-    void *pinned_sep[2] = {nullptr, nullptr};
-    void *pinned_codes[2] = {nullptr, nullptr};     // packed feed path: host code buffers
-    size_t pinned_codes_bytes[2] = {0, 0};
+    mashgpu::PinnedScratch pinned[2], pinned_sep[2];   // ASCII feed path: staged small records, separator list
+    mashgpu::PinnedScratch pinned_codes[2];         // packed feed path: host code buffers
     cudaEvent_t pack_copied[2] = {nullptr, nullptr};
-    void *flags_pinned = nullptr;                   // per-unit status flags of the sketch pass in flight (sketch.cu)
-    size_t flags_pinned_n = 0;
+    mashgpu::PinnedScratch flags_pinned;            // per-unit status flags of the sketch pass in flight (sketch.cu)
     cudaStream_t pack_stream = nullptr;             // packed uploads (next to the ASCII copies on copy_stream)
     // screen: chunk staging buffers and the finish() outputs outlive a job (cudaMalloc of a few hundred MB inside a timed pass cost
     // 1-50 ms depending on the box); scr_stage_owner = the job using the staging pair, others allocate their own
     mashgpu::Scratch scr_stage[2], scr_out;
     const void *scr_stage_owner = nullptr;
-    void *scr_pinned[2] = {nullptr, nullptr};       // packed host feed of screen: pinned codes + mask per slot (with scr_stage)
-    size_t scr_pinned_bytes[2] = {0, 0};
-    void *pinned[2] = {nullptr, nullptr};
-    size_t pinned_bytes[2] = {0, 0};
+    mashgpu::PinnedScratch scr_pinned[2];           // packed host feed of screen: pinned codes + mask per slot (with scr_stage)
     cudaEvent_t wave_copied[2] = {nullptr, nullptr};
 };
 

@@ -476,16 +476,8 @@ int screen_feed_host_packed(mashgpu_screen_job *job, const void *chunk, uint64_t
         ctx->scr_stage_owner = job;
         stage = ctx->scr_stage[b].get<uint8_t>(ctx->scr_stage[b].bytes < bytes ? bytes + (bytes >> 2) : bytes);
         if (!stage) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (chunk of %llu B)", (unsigned long long)len);
-        if (ctx->scr_pinned_bytes[b] < bytes) {
-            if (ctx->scr_pinned[b]) cudaFreeHost(ctx->scr_pinned[b]);
-            ctx->scr_pinned[b] = nullptr; ctx->scr_pinned_bytes[b] = 0;
-            if (cudaMallocHost(&ctx->scr_pinned[b], bytes + (bytes >> 2)) != cudaSuccess) {
-                cudaGetLastError();
-                return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (packed chunk of %llu B)", (unsigned long long)len);
-            }
-            ctx->scr_pinned_bytes[b] = bytes + (bytes >> 2);
-        }
-        h_codes = static_cast<uint64_t *>(ctx->scr_pinned[b]);
+        h_codes = ctx->scr_pinned[b].get<uint64_t>((bytes + 7) / 8);
+        if (!h_codes) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (packed chunk of %llu B)", (unsigned long long)len);
     } else {
         if (job->stage[b].n < bytes && job->stage[b].alloc(bytes + (bytes >> 2)) != cudaSuccess)
             return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (chunk of %llu B)", (unsigned long long)len);

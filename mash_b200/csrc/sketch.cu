@@ -837,14 +837,10 @@ int sketch_stream_enqueue(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, cons
         MG_CUDA(ctx, cudaGetLastError());
     }
 
-    if (ctx->flags_pinned_n < n_units) {          // one ticket in flight per context: its flags land in the context's pinned buffer
-        if (ctx->flags_pinned) cudaFreeHost(ctx->flags_pinned);
-        ctx->flags_pinned = nullptr; ctx->flags_pinned_n = 0;
-        const size_t want = (size_t)n_units + n_units / 4 + 64;
-        if (cudaMallocHost(&ctx->flags_pinned, want * 4) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (unit flags)");
-        ctx->flags_pinned_n = want;
-    }
-    MG_CUDA(ctx, cudaMemcpyAsync(ctx->flags_pinned, d_flags.p, n_units * 4ull, cudaMemcpyDeviceToHost, st));
+    // one ticket in flight per context: its flags land in the context's pinned buffer
+    uint32_t *h_flags = ctx->flags_pinned.get<uint32_t>(n_units);
+    if (!h_flags) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (unit flags)");
+    MG_CUDA(ctx, cudaMemcpyAsync(h_flags, d_flags.p, n_units * 4ull, cudaMemcpyDeviceToHost, st));
     t.d_qtarget = d_qtarget; t.d_qtstar = d_qtstar;
     t.active = true;
     return MASHGPU_OK;
@@ -862,7 +858,7 @@ int sketch_stream_finalize(mashgpu_ctx *ctx, SketchTicket &t)
     uint64_t *d_out_hashes = t.d_out_hashes; uint32_t *d_out_counts = t.d_out_counts, *d_out_n = t.d_out_n;
     uint64_t *d_qtarget = t.d_qtarget, *d_qtstar = t.d_qtstar;
     MG_CUDA(ctx, cudaStreamSynchronize(st));
-    const uint32_t *h_flags = (const uint32_t *)ctx->flags_pinned;
+    const uint32_t *h_flags = static_cast<const uint32_t *>(ctx->flags_pinned.p);
     bool any_flag = false;
     for (uint32_t u = 0; u < n_units; u++) any_flag |= h_flags[u] != 0;
     if (!any_flag) return MASHGPU_OK;
@@ -928,12 +924,6 @@ extern "C" int mashgpu_sketch_stream_dev(mashgpu_ctx *ctx, const mashgpu_sketch_
     return sketch_stream_core(ctx, params, S, d_out_hashes, d_out_counts, d_out_n, stream ? (cudaStream_t)stream : ctx->stream, nullptr);
 }
 
-namespace {
-
-struct Wave { uint64_t unit_begin, unit_end, rec_begin, rec_end, bytes; };
-
-}  // namespace
-
 namespace mashgpu {
 static int unit_stream_limit(mashgpu_ctx *ctx, uint64_t *limit);
 static int sketch_unit_streamed(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, uint64_t n_records, const char *const *seq,
@@ -947,102 +937,108 @@ constexpr uint64_t WAVE_BYTES = 1ull << 30;        // stream bytes per wave (the
 constexpr uint32_t SEP_LIST_MAX = 1u << 15;        // directly copied records per wave whose separators go through the list
 constexpr uint64_t DIRECT_COPY_MIN = 1ull << 18;   // records at least this long are copied straight from the caller's buffer
 
-}  // namespace
+// ---- the wave pieces of both batch calls (mashgpu_sketch_batch, mashgpu_sketch_batch_packed)
 
-extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
-                                    uint64_t n_records, const char *const *seq, const uint64_t *len,
-                                    const uint32_t *unit_of_record, uint64_t n_units,
-                                    uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length)
+// Waves are cut by stream bytes and by unit count (outputs and candidate tables grow with the number of units, not with their
+// length -- a multi-FASTA of millions of short records must not allocate units x s outputs at once).
+struct WaveLimits { uint64_t bytes, units; };
+
+WaveLimits wave_limits(uint32_t s)
 {
-    if (!ctx) return MASHGPU_ERR_INVALID;
-    MG_TRY(validate_sketch_params(ctx, params));
-    if (n_units == 0) return MASHGPU_OK;
-    if (!out_hashes || !out_n) return fail(ctx, MASHGPU_ERR_INVALID, "out_hashes/out_n is NULL");
-    if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
-    if (n_units > 0xFFFFFFF0ull) return fail(ctx, MASHGPU_ERR_INVALID, "too many units");
-    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    WaveLimits L{WAVE_BYTES, std::max<uint64_t>(64, (1ull << 28) / ((uint64_t)s * 8))};
+    if (const char *env = getenv("MASHGPU_WAVE_BYTES")) L.bytes = std::max<uint64_t>(1024, strtoull(env, nullptr, 10));      // tests: many waves from little data
+    if (const char *env = getenv("MASHGPU_WAVE_UNITS")) L.units = std::max<uint64_t>(1, strtoull(env, nullptr, 10));
+    return L;
+}
+
+// The call's host outputs, indexed by unit (out_counts may be NULL), and the device outputs of one wave (the context's scratch).
+struct WaveOut {
+    uint64_t *out_hashes; uint32_t *out_counts, *out_n;
+    uint64_t *d_hashes = nullptr; uint32_t *d_counts = nullptr, *d_n = nullptr;
+};
+
+int wave_outputs(mashgpu_ctx *ctx, uint32_t s, uint64_t max_units, WaveOut &o)
+{
+    o.d_hashes = ctx->sc_out_hashes.get<uint64_t>(max_units * s);
+    o.d_n = ctx->sc_out_n.get<uint32_t>(max_units);
+    o.d_counts = o.out_counts ? ctx->sc_out_counts.get<uint32_t>(max_units * s) : nullptr;
+    if (!o.d_hashes || !o.d_n || (o.out_counts && !o.d_counts)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (outputs)");
+    return MASHGPU_OK;
+}
+
+// Sketches the wave S -- units [u0, u0 + S.n_units) of the call -- on the compute stream, copies its sketches back and waits for them.
+int sketch_wave(mashgpu_ctx *ctx, const mashgpu_sketch_params *p, const SketchStream &S, uint64_t u0, const WaveOut &o)
+{
+    const uint64_t s = p->sketch_size, nu = S.n_units;
+    MG_TRY(sketch_stream_core(ctx, p, S, o.d_hashes, o.d_counts, o.d_n, ctx->stream, nullptr));
+    MG_CUDA(ctx, cudaMemcpyAsync(o.out_hashes + u0 * s, o.d_hashes, nu * s * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    MG_CUDA(ctx, cudaMemcpyAsync(o.out_n + u0, o.d_n, nu * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    if (o.out_counts) MG_CUDA(ctx, cudaMemcpyAsync(o.out_counts + u0 * s, o.d_counts, nu * s * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return MASHGPU_OK;
+}
+
+// Device slots for packed waves of up to max_len positions: 2-bit codes and the invalid-position mask, `groups` 32-position
+// groups each (tile-padded + halo: the scan kernel reads whole tiles without looking at the stream length).  Uploads go on
+// pack_stream and record pack_copied[b].
+struct PackedSlots { uint64_t groups = 0; uint64_t *d_codes[2] = {}; uint32_t *d_inval[2] = {}; };
+
+int packed_slots(mashgpu_ctx *ctx, int n_slots, uint64_t max_len, PackedSlots &P)
+{
+    P.groups = (max_len + SCAN_TILE - 1) / SCAN_TILE * (SCAN_TILE / 32) + 64;
+    for (int b = 0; b < n_slots; b++) {
+        P.d_codes[b] = ctx->sc_codes[b].get<uint64_t>(P.groups);
+        P.d_inval[b] = ctx->sc_inval[b].get<uint32_t>(P.groups);
+        if (!P.d_codes[b] || !P.d_inval[b]) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (packed stream of %llu groups)", (unsigned long long)P.groups);
+        if (!ctx->pack_copied[b]) MG_CUDA(ctx, cudaEventCreateWithFlags(&ctx->pack_copied[b], cudaEventDisableTiming));
+    }
+    if (n_slots && !ctx->pack_stream) MG_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
+    return MASHGPU_OK;
+}
+
+// Enqueues the upload of a packed wave into slot b: `groups` code words, then the mask -- zeroed, and the invalid runs set (they
+// must reach the end of the slot) by one apply_runs_kernel -- then records pack_copied[b].  The packer thread calls it too, so it
+// returns a bare code: the launching thread reports the failure and counts the launch.
+int upload_packed(mashgpu_ctx *ctx, const PackedSlots &P, int b, const uint64_t *h_codes, uint64_t groups, const std::vector<PackRun> &runs)
+{
+    cudaStream_t cs = ctx->pack_stream;
+    if (groups && cudaMemcpyAsync(P.d_codes[b], h_codes, groups * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
+    if (cudaMemsetAsync(P.d_inval[b], 0, P.groups * 4, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
+    PackRun *d_runs = ctx->sc_runs[b].get<PackRun>(runs.size());
+    if (!d_runs) return MASHGPU_ERR_NOMEM;
+    if (cudaMemcpyAsync(d_runs, runs.data(), runs.size() * sizeof(PackRun), cudaMemcpyHostToDevice, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
+    const uint64_t nr = runs.size();
+    const unsigned blocks = (unsigned)std::min<uint64_t>((nr * 32 + 255) / 256, (uint64_t)ctx->sm_count * 16);
+    apply_runs_kernel<<<std::max(1u, blocks), 256, 0, cs>>>(d_runs, nr, P.d_inval[b]);
+    if (cudaGetLastError() != cudaSuccess) return MASHGPU_ERR_CUDA;
+    if (cudaEventRecord(ctx->pack_copied[b], cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
+    return MASHGPU_OK;
+}
+
+// ---- mashgpu_sketch_batch
+
+struct Wave { uint64_t unit_begin, unit_end, bytes; };     // its records: unit_rec_begin[unit_begin] .. unit_rec_begin[unit_end]
+
+// Units [u0, u1) of a batch, none of them too large for the device, in waves.  Records, units and outputs are indexed as in the
+// call: unit u holds the records unit_rec_begin[u] .. unit_rec_begin[u + 1], unit_bytes[u] stream bytes.
+int sketch_units(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, const char *const *seq, const uint64_t *len,
+                 const uint64_t *unit_rec_begin, const uint64_t *unit_bytes, uint64_t u0, uint64_t u1,
+                 uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n)
+{
     const uint32_t s = params->sketch_size;
     const uint64_t k = (uint64_t)params->kmer_size;
-
-    // unit spans in the flat stream: kept records back to back, one separator byte after each
-    std::vector<uint64_t> unit_bytes(n_units, 0), unit_rec_begin(n_units + 1, 0);
-    {
-        uint64_t r = 0;
-        for (uint64_t u = 0; u < n_units; u++) {
-            unit_rec_begin[u] = r;
-            while (r < n_records && (unit_of_record ? unit_of_record[r] : r) == u) {
-                if (len[r] >= k) unit_bytes[u] += len[r] + 1;
-                r++;
-            }
-            if (r < n_records && unit_of_record && unit_of_record[r] < u)
-                return fail(ctx, MASHGPU_ERR_INVALID, "unit_of_record must be non-decreasing");
-        }
-        unit_rec_begin[n_units] = r;
-        if (r != n_records) return fail(ctx, MASHGPU_ERR_INVALID, "unit_of_record refers to units >= n_units or is not sorted");
-    }
-    if (out_length)
-        for (uint64_t u = 0; u < n_units; u++) {
-            uint64_t L = 0;
-            for (uint64_t r = unit_rec_begin[u]; r < unit_rec_begin[u + 1]; r++)
-                if (len[r] >= k) L += len[r];
-            out_length[u] = L;
-        }
-
-    // a unit whose stream does not fit on the device at once (the whole-set rule of mashgpu_sketch_reads) streams through a unit job
-    // fed from the caller's buffers; the runs of units between such units take the waves below (DESIGN.md 2.7)
-    if (params->min_copies <= 1) {
-        uint64_t limit = 0;
-        MG_TRY(unit_stream_limit(ctx, &limit));
-        bool any = false;
-        for (uint64_t u = 0; u < n_units; u++) any |= unit_bytes[u] > limit;
-        if (any) {
-            mashgpu_sketch_params q = *params;
-            q.target_cov = 0;                    // not a reads-mode setting: ignored here as in the waves
-            std::vector<uint32_t> uor;
-            for (uint64_t u0 = 0; u0 < n_units;) {
-                const uint64_t rb = unit_rec_begin[u0];
-                if (unit_bytes[u0] > limit) {
-                    MG_TRY(sketch_unit_streamed(ctx, &q, unit_rec_begin[u0 + 1] - rb, seq + rb, len + rb, out_hashes + u0 * s,
-                                                out_counts ? out_counts + u0 * s : nullptr, out_n + u0, out_length ? out_length + u0 : nullptr, nullptr));
-                    u0++;
-                    continue;
-                }
-                uint64_t u1 = u0 + 1;
-                while (u1 < n_units && unit_bytes[u1] <= limit) u1++;
-                const uint64_t re = unit_rec_begin[u1];
-                const uint32_t *sub = nullptr;
-                if (unit_of_record) {
-                    uor.resize(re - rb);
-                    for (uint64_t r = rb; r < re; r++) uor[r - rb] = unit_of_record[r] - (uint32_t)u0;
-                    sub = uor.data();
-                }
-                MG_TRY(mashgpu_sketch_batch(ctx, params, re - rb, seq + rb, len + rb, sub, u1 - u0, out_hashes + u0 * s,
-                                            out_counts ? out_counts + u0 * s : nullptr, out_n + u0, out_length ? out_length + u0 : nullptr));
-                u0 = u1;
-            }
-            return MASHGPU_OK;
-        }
-    }
-
-    // waves: cut by stream bytes and by unit count (outputs and candidate tables grow with the number of units, not with their
-    // length -- a multi-FASTA of millions of short records must not allocate units x s outputs at once)
-    uint64_t wave_units_max = std::max<uint64_t>(64, (1ull << 28) / ((uint64_t)s * 8));
-    uint64_t wave_bytes = WAVE_BYTES;
-    if (const char *env = getenv("MASHGPU_WAVE_BYTES")) wave_bytes = std::max<uint64_t>(1024, strtoull(env, nullptr, 10));      // tests: many waves from little data
-    if (const char *env = getenv("MASHGPU_WAVE_UNITS")) wave_units_max = std::max<uint64_t>(1, strtoull(env, nullptr, 10));
+    const WaveLimits lim = wave_limits(s);
     std::vector<Wave> waves;
     {
-        Wave w{0, 0, 0, 0, 0};
-        for (uint64_t u = 0; u < n_units; u++) {
-            if (w.unit_end > w.unit_begin && (w.bytes + unit_bytes[u] > wave_bytes || w.unit_end - w.unit_begin >= wave_units_max)) {
-                w.rec_end = unit_rec_begin[u];
+        Wave w{u0, u0, 0};
+        for (uint64_t u = u0; u < u1; u++) {
+            if (w.unit_end > w.unit_begin && (w.bytes + unit_bytes[u] > lim.bytes || w.unit_end - w.unit_begin >= lim.units)) {
                 waves.push_back(w);
-                w = Wave{u, u, unit_rec_begin[u], 0, 0};
+                w = Wave{u, u, 0};
             }
             w.unit_end = u + 1;
             w.bytes += unit_bytes[u];
         }
-        w.rec_end = n_records;
         waves.push_back(w);
     }
     const size_t n_waves = waves.size();
@@ -1066,7 +1062,7 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
             const Wave &w = waves[wi];
             bool ok = true;
             bool probed = false;
-            for (uint64_t r = w.rec_begin; r < w.rec_end && ok; r++) {
+            for (uint64_t r = unit_rec_begin[w.unit_begin]; r < unit_rec_begin[w.unit_end] && ok; r++) {
                 if (len[r] < k) continue;
                 if (len[r] < DIRECT_COPY_MIN) ok = false;
                 else if (!probed) {          // one probe per wave: callers allocate their records the same way
@@ -1084,10 +1080,8 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
     int threads = host_pack_threads();
     if ((feed & FEED_ASCII) && !getenv("MASHGPU_PACK_THREADS")) threads = std::max(1, threads - 1);
 
-    uint64_t *d_hashes = ctx->sc_out_hashes.get<uint64_t>(max_units * s);
-    uint32_t *d_n = ctx->sc_out_n.get<uint32_t>(max_units);
-    uint32_t *d_counts = out_counts ? ctx->sc_out_counts.get<uint32_t>(max_units * s) : nullptr;
-    if (!d_hashes || !d_n || (out_counts && !d_counts)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (outputs)");
+    WaveOut out{out_hashes, out_counts, out_n};
+    MG_TRY(wave_outputs(ctx, s, max_units, out));
 
     // ---- ASCII producer: two device wave buffers, copies on copy_stream
     struct AsciiSlot { int64_t wave = -1; uint8_t *d = nullptr; std::vector<uint64_t> unit_start; };
@@ -1105,23 +1099,15 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
         uint8_t *dst = aslot[b].d;
         // staging size: all small records of the wave
         uint64_t small_bytes = 0;
-        for (uint64_t r = w.rec_begin; r < w.rec_end; r++)
+        for (uint64_t r = unit_rec_begin[w.unit_begin]; r < unit_rec_begin[w.unit_end]; r++)
             if (len[r] >= k && len[r] < DIRECT_COPY_MIN) small_bytes += len[r] + 1;
-        if (ctx->pinned_bytes[b] < small_bytes) {
-            if (ctx->pinned[b]) cudaFreeHost(ctx->pinned[b]);
-            ctx->pinned[b] = nullptr; ctx->pinned_bytes[b] = 0;
-            if (cudaMallocHost(&ctx->pinned[b], small_bytes + small_bytes / 8) != cudaSuccess)
-                return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (%llu B)", (unsigned long long)small_bytes);
-            ctx->pinned_bytes[b] = small_bytes + small_bytes / 8;
-        }
-        uint8_t *stage = (uint8_t *)ctx->pinned[b];
+        uint8_t *stage = ctx->pinned[b].get<uint8_t>(small_bytes);
+        if (!stage) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (%llu B)", (unsigned long long)small_bytes);
         std::vector<uint64_t> &us = aslot[b].unit_start;
         us.assign(w.unit_end - w.unit_begin + 1, 0);
         // separator offsets of the directly copied records (pinned list -> device -> one kernel); list full: 1-byte memsets
-        if (!ctx->pinned_sep[b]) {
-            if (cudaMallocHost(&ctx->pinned_sep[b], SEP_LIST_MAX * 8) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (separator list)");
-        }
-        uint64_t *h_sep = (uint64_t *)ctx->pinned_sep[b];
+        uint64_t *h_sep = ctx->pinned_sep[b].get<uint64_t>(SEP_LIST_MAX);
+        if (!h_sep) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (separator list)");
         uint64_t *d_sep = ctx->sc_sep[b].get<uint64_t>(SEP_LIST_MAX);
         if (!d_sep) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (separator list)");
         uint32_t n_sep = 0;
@@ -1169,34 +1155,23 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
     // its upload (codes, invalid runs -> mask) on pack_stream, so a finished future means "event recorded"
     struct PackSlot {
         int64_t wave = -1;
-        uint64_t *h_codes = nullptr, *d_codes = nullptr; uint32_t *d_inval = nullptr;
+        uint64_t *h_codes = nullptr;
         std::vector<uint64_t> unit_start; std::vector<PackRun> runs; uint64_t len = 0;
     };
     PackSlot pslot[2];
     const int n_pslots = (feed & FEED_PACK) ? (n_waves > 1 ? 2 : 1) : 0;
-    const uint64_t max_tiles = (max_bytes + SCAN_TILE - 1) / SCAN_TILE;
-    const uint64_t groups_alloc = max_tiles * (SCAN_TILE / 32) + 64;       // tile-padded + halo
+    PackedSlots slots;
+    MG_TRY(packed_slots(ctx, n_pslots, max_bytes, slots));
     for (int b = 0; b < n_pslots; b++) {
-        pslot[b].d_codes = ctx->sc_codes[b].get<uint64_t>(groups_alloc);
-        pslot[b].d_inval = ctx->sc_inval[b].get<uint32_t>(groups_alloc);
-        if (!pslot[b].d_codes || !pslot[b].d_inval) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (packed stream of %llu groups)", (unsigned long long)groups_alloc);
-        if (ctx->pinned_codes_bytes[b] < groups_alloc * 8) {
-            if (ctx->pinned_codes[b]) cudaFreeHost(ctx->pinned_codes[b]);
-            ctx->pinned_codes[b] = nullptr; ctx->pinned_codes_bytes[b] = 0;
-            if (cudaMallocHost(&ctx->pinned_codes[b], groups_alloc * 8) != cudaSuccess)
-                return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (%llu B)", (unsigned long long)(groups_alloc * 8));
-            ctx->pinned_codes_bytes[b] = groups_alloc * 8;
-        }
-        pslot[b].h_codes = (uint64_t *)ctx->pinned_codes[b];
-        if (!ctx->pack_copied[b]) MG_CUDA(ctx, cudaEventCreateWithFlags(&ctx->pack_copied[b], cudaEventDisableTiming));
+        pslot[b].h_codes = ctx->pinned_codes[b].get<uint64_t>(slots.groups);
+        if (!pslot[b].h_codes) return fail(ctx, MASHGPU_ERR_NOMEM, "out of pinned host memory (%llu B)", (unsigned long long)(slots.groups * 8));
     }
-    if (n_pslots && !ctx->pack_stream) MG_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
     auto pack_job = [&](size_t wi, int b) -> int {
         cudaSetDevice(ctx->device);
         const Wave &w = waves[wi];
         PackSlot &P = pslot[b];
         std::vector<PackSegment> segs;
-        segs.reserve(w.rec_end - w.rec_begin);
+        segs.reserve(unit_rec_begin[w.unit_end] - unit_rec_begin[w.unit_begin]);
         P.unit_start.assign(w.unit_end - w.unit_begin + 1, 0);
         uint64_t off = 0;
         for (uint64_t u = w.unit_begin; u < w.unit_end; u++) {
@@ -1210,21 +1185,9 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
         P.unit_start[w.unit_end - w.unit_begin] = off;
         P.len = off;
         pack_stream(segs.data(), segs.size(), off, params->preserve_case, threads, P.h_codes, P.runs);
-        P.runs.push_back(PackRun{off, groups_alloc * 32 - off});      // everything from the end of the stream to the end of the allocation is invalid
-        // upload: codes, zeroed mask, runs -> mask
-        const uint64_t groups = (P.len + 31) / 32;
-        cudaStream_t cs = ctx->pack_stream;
-        if (groups && cudaMemcpyAsync(P.d_codes, P.h_codes, groups * 8, cudaMemcpyHostToDevice, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
-        if (cudaMemsetAsync(P.d_inval, 0, groups_alloc * 4, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
-        PackRun *d_runs = ctx->sc_runs[b].get<PackRun>(P.runs.size());
-        if (!d_runs) return MASHGPU_ERR_NOMEM;
-        if (cudaMemcpyAsync(d_runs, P.runs.data(), P.runs.size() * sizeof(PackRun), cudaMemcpyHostToDevice, cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
-        const uint64_t nr = P.runs.size();
-        const unsigned blocks = (unsigned)std::min<uint64_t>((nr * 32 + 255) / 256, (uint64_t)ctx->sm_count * 16);
-        apply_runs_kernel<<<std::max(1u, blocks), 256, 0, cs>>>(d_runs, nr, P.d_inval);
-        if (cudaGetLastError() != cudaSuccess) return MASHGPU_ERR_CUDA;
-        if (cudaEventRecord(ctx->pack_copied[b], cs) != cudaSuccess) return MASHGPU_ERR_CUDA;
-        return MASHGPU_OK;          // the upload is in flight: the slot is ready once the event has fired (its buffers are reused only after that)
+        P.runs.push_back(PackRun{off, slots.groups * 32 - off});      // everything from the end of the stream to the end of the allocation is invalid
+        // the upload is in flight when this returns: the slot is ready once the event has fired (its buffers are reused only after that)
+        return upload_packed(ctx, slots, b, P.h_codes, (P.len + 31) / 32, P.runs);
     };
 
     // ---- scheduler: both producers claim the next unclaimed wave they may take; this thread runs the kernels of whichever
@@ -1248,18 +1211,6 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
     int pstate[2] = {P_EMPTY, P_EMPTY};         // under `mu`
     int pack_rc = MASHGPU_OK;                   // under `mu`: first failure of the packer thread
     bool stop = false, packer_done = n_pslots == 0;
-    auto run_wave = [&](size_t wi, const SketchStream &S) -> int {
-        const Wave &w = waves[wi];
-        const uint64_t nu = w.unit_end - w.unit_begin;
-        int r = sketch_stream_core(ctx, params, S, d_hashes, d_counts, d_n, ctx->stream, nullptr);
-        if (r != MASHGPU_OK) return r;
-        MG_CUDA(ctx, cudaMemcpyAsync(out_hashes + w.unit_begin * s, d_hashes, nu * s * 8ull, cudaMemcpyDeviceToHost, ctx->stream));
-        MG_CUDA(ctx, cudaMemcpyAsync(out_n + w.unit_begin, d_n, nu * 4ull, cudaMemcpyDeviceToHost, ctx->stream));
-        if (out_counts)
-            MG_CUDA(ctx, cudaMemcpyAsync(out_counts + w.unit_begin * s, d_counts, nu * s * 4ull, cudaMemcpyDeviceToHost, ctx->stream));
-        MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        return MASHGPU_OK;
-    };
     // the packer thread: claims a wave whenever one of its two slots is empty, packs it on `threads` host threads, enqueues the
     // upload and moves on -- it never waits for this thread's kernels
     std::thread packer;
@@ -1324,18 +1275,20 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
         if (rc != MASHGPU_OK) break;
         if (ready_p >= 0) {
             PackSlot &P = pslot[ready_p];
+            const Wave &w = waves[P.wave];
             ctx->kernel_launches++;             // apply_runs_kernel of the upload
             SketchStream S;
-            S.d_codes = P.d_codes; S.d_inval = P.d_inval; S.unit_start = P.unit_start.data(); S.n_units = waves[P.wave].unit_end - waves[P.wave].unit_begin;
-            rc = run_wave((size_t)P.wave, S);
+            S.d_codes = slots.d_codes[ready_p]; S.d_inval = slots.d_inval[ready_p]; S.unit_start = P.unit_start.data(); S.n_units = w.unit_end - w.unit_begin;
+            rc = sketch_wave(ctx, params, S, w.unit_begin, out);
             { std::lock_guard<std::mutex> lock(mu); P.wave = -1; pstate[ready_p] = P_EMPTY; }
             cv.notify_all();
             done++;
         } else if (ready_a >= 0) {
             AsciiSlot &A = aslot[ready_a];
+            const Wave &w = waves[A.wave];
             SketchStream S;
-            S.d_stream = A.d; S.unit_start = A.unit_start.data(); S.n_units = waves[A.wave].unit_end - waves[A.wave].unit_begin;
-            rc = run_wave((size_t)A.wave, S);
+            S.d_stream = A.d; S.unit_start = A.unit_start.data(); S.n_units = w.unit_end - w.unit_begin;
+            rc = sketch_wave(ctx, params, S, w.unit_begin, out);
             A.wave = -1;
             done++;
         } else {
@@ -1359,6 +1312,69 @@ extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_param
     return rc;
 }
 
+}  // namespace
+
+extern "C" int mashgpu_sketch_batch(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
+                                    uint64_t n_records, const char *const *seq, const uint64_t *len,
+                                    const uint32_t *unit_of_record, uint64_t n_units,
+                                    uint64_t *out_hashes, uint32_t *out_counts, uint32_t *out_n, uint64_t *out_length)
+{
+    if (!ctx) return MASHGPU_ERR_INVALID;
+    MG_TRY(validate_sketch_params(ctx, params));
+    if (n_units == 0) return MASHGPU_OK;
+    if (!out_hashes || !out_n) return fail(ctx, MASHGPU_ERR_INVALID, "out_hashes/out_n is NULL");
+    if (n_records && (!seq || !len)) return fail(ctx, MASHGPU_ERR_INVALID, "seq/len is NULL");
+    if (n_units > 0xFFFFFFF0ull) return fail(ctx, MASHGPU_ERR_INVALID, "too many units");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    const uint32_t s = params->sketch_size;
+    const uint64_t k = (uint64_t)params->kmer_size;
+
+    // unit spans in the flat stream: kept records back to back, one separator byte after each
+    std::vector<uint64_t> unit_bytes(n_units, 0), unit_rec_begin(n_units + 1, 0);
+    {
+        uint64_t r = 0;
+        for (uint64_t u = 0; u < n_units; u++) {
+            unit_rec_begin[u] = r;
+            while (r < n_records && (unit_of_record ? unit_of_record[r] : r) == u) {
+                if (len[r] >= k) unit_bytes[u] += len[r] + 1;
+                r++;
+            }
+            if (r < n_records && unit_of_record && unit_of_record[r] < u)
+                return fail(ctx, MASHGPU_ERR_INVALID, "unit_of_record must be non-decreasing");
+        }
+        unit_rec_begin[n_units] = r;
+        if (r != n_records) return fail(ctx, MASHGPU_ERR_INVALID, "unit_of_record refers to units >= n_units or is not sorted");
+    }
+    if (out_length)
+        for (uint64_t u = 0; u < n_units; u++) {
+            uint64_t L = 0;
+            for (uint64_t r = unit_rec_begin[u]; r < unit_rec_begin[u + 1]; r++)
+                if (len[r] >= k) L += len[r];
+            out_length[u] = L;
+        }
+
+    // a unit whose stream does not fit on the device at once (the whole-set rule of mashgpu_sketch_reads) streams through a unit job
+    // fed from the caller's buffers; each run of units between such units takes the waves of sketch_units (DESIGN.md 2.7)
+    uint64_t limit = UINT64_MAX;
+    if (params->min_copies <= 1) MG_TRY(unit_stream_limit(ctx, &limit));
+    mashgpu_sketch_params q = *params;
+    q.target_cov = 0;                    // not a reads-mode setting: ignored here as in the waves
+    for (uint64_t u0 = 0; u0 < n_units;) {
+        if (unit_bytes[u0] > limit) {
+            const uint64_t rb = unit_rec_begin[u0];
+            MG_TRY(sketch_unit_streamed(ctx, &q, unit_rec_begin[u0 + 1] - rb, seq + rb, len + rb, out_hashes + u0 * s,
+                                        out_counts ? out_counts + u0 * s : nullptr, out_n + u0, out_length ? out_length + u0 : nullptr, nullptr));
+            u0++;
+            continue;
+        }
+        uint64_t u1 = u0 + 1;
+        while (u1 < n_units && unit_bytes[u1] <= limit) u1++;
+        MG_TRY(sketch_units(ctx, params, seq, len, unit_rec_begin.data(), unit_bytes.data(), u0, u1, out_hashes, out_counts, out_n));
+        u0 = u1;
+    }
+    return MASHGPU_OK;
+}
+
 extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
                                            const uint64_t *codes, uint64_t stream_len, const uint64_t *runs, uint64_t n_runs,
                                            const uint64_t *unit_start, uint64_t n_units,
@@ -1377,34 +1393,21 @@ extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketc
     const uint32_t s = params->sketch_size;
     // waves of whole units, each starting at the 32-position group that holds its first unit's first position
     struct PWave { uint64_t u0, u1, g0, g1; };      // units [u0, u1), groups [g0, g1)
-    uint64_t wave_units_max = std::max<uint64_t>(64, (1ull << 28) / ((uint64_t)s * 8));
-    uint64_t wave_bytes = WAVE_BYTES;
-    if (const char *env = getenv("MASHGPU_WAVE_BYTES")) wave_bytes = std::max<uint64_t>(1024, strtoull(env, nullptr, 10));
-    if (const char *env = getenv("MASHGPU_WAVE_UNITS")) wave_units_max = std::max<uint64_t>(1, strtoull(env, nullptr, 10));
+    const WaveLimits lim = wave_limits(s);
     std::vector<PWave> waves;
     for (uint64_t u = 0; u < n_units;) {
         uint64_t v = u + 1;
-        while (v < n_units && v - u < wave_units_max && unit_start[v + 1] - unit_start[u] <= wave_bytes) v++;
+        while (v < n_units && v - u < lim.units && unit_start[v + 1] - unit_start[u] <= lim.bytes) v++;
         waves.push_back(PWave{u, v, unit_start[u] / 32, (unit_start[v] + 31) / 32});
         u = v;
     }
     uint64_t max_groups = 1, max_units = 1;
     for (auto &w : waves) { max_groups = std::max(max_groups, w.g1 - w.g0); max_units = std::max(max_units, w.u1 - w.u0); }
-    const uint64_t max_tiles = (max_groups * 32 + SCAN_TILE - 1) / SCAN_TILE;
-    const uint64_t groups_alloc = max_tiles * (SCAN_TILE / 32) + 64;       // tile-padded + halo
     const int nbuf = waves.size() > 1 ? 2 : 1;
-    uint64_t *d_codes[2] = {nullptr, nullptr}; uint32_t *d_inval[2] = {nullptr, nullptr};
-    for (int b = 0; b < nbuf; b++) {
-        d_codes[b] = ctx->sc_codes[b].get<uint64_t>(groups_alloc);
-        d_inval[b] = ctx->sc_inval[b].get<uint32_t>(groups_alloc);
-        if (!d_codes[b] || !d_inval[b]) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (packed stream of %llu groups)", (unsigned long long)groups_alloc);
-        if (!ctx->pack_copied[b]) MG_CUDA(ctx, cudaEventCreateWithFlags(&ctx->pack_copied[b], cudaEventDisableTiming));
-    }
-    if (!ctx->pack_stream) MG_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
-    uint64_t *d_hashes = ctx->sc_out_hashes.get<uint64_t>(max_units * s);
-    uint32_t *d_n = ctx->sc_out_n.get<uint32_t>(max_units);
-    uint32_t *d_counts = out_counts ? ctx->sc_out_counts.get<uint32_t>(max_units * s) : nullptr;
-    if (!d_hashes || !d_n || (out_counts && !d_counts)) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (outputs)");
+    PackedSlots slots;
+    MG_TRY(packed_slots(ctx, nbuf, max_groups * 32, slots));
+    WaveOut out{out_hashes, out_counts, out_n};
+    MG_TRY(wave_outputs(ctx, s, max_units, out));
 
     std::vector<PackRun> wruns[2];
     std::vector<uint64_t> wstart[2];
@@ -1412,10 +1415,7 @@ extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketc
     auto upload = [&](size_t wi) -> int {
         const PWave &w = waves[wi];
         const int b = (int)(wi % nbuf);
-        cudaStream_t cs = ctx->pack_stream;
         const uint64_t p0 = w.g0 * 32, p1 = unit_start[w.u1];           // wave-local position = position - p0
-        MG_CUDA(ctx, cudaMemcpyAsync(d_codes[b], codes + w.g0, (w.g1 - w.g0) * 8, cudaMemcpyHostToDevice, cs));
-        MG_CUDA(ctx, cudaMemsetAsync(d_inval[b], 0, groups_alloc * 4, cs));
         std::vector<PackRun> &R = wruns[b];
         R.clear();
         if (unit_start[w.u0] > p0) R.push_back(PackRun{0, unit_start[w.u0] - p0});       // the tail of the previous unit in the first group
@@ -1424,15 +1424,10 @@ extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketc
             const uint64_t a = std::max(runs[2 * r], unit_start[w.u0]), e = std::min(runs[2 * r] + runs[2 * r + 1], p1);
             if (e > a) R.push_back(PackRun{a - p0, e - a});
         }
-        R.push_back(PackRun{p1 - p0, groups_alloc * 32 - (p1 - p0)});                   // everything past the wave's last unit
-        PackRun *d_runs = ctx->sc_runs[b].get<PackRun>(R.size());
-        if (!d_runs) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (invalid runs)");
-        MG_CUDA(ctx, cudaMemcpyAsync(d_runs, R.data(), R.size() * sizeof(PackRun), cudaMemcpyHostToDevice, cs));
-        const unsigned blocks = (unsigned)std::min<uint64_t>((R.size() * 32 + 255) / 256, (uint64_t)ctx->sm_count * 16);
-        apply_runs_kernel<<<std::max(1u, blocks), 256, 0, cs>>>(d_runs, R.size(), d_inval[b]);
-        ctx->kernel_launches++;
-        MG_CUDA(ctx, cudaGetLastError());
-        MG_CUDA(ctx, cudaEventRecord(ctx->pack_copied[b], cs));
+        R.push_back(PackRun{p1 - p0, slots.groups * 32 - (p1 - p0)});                  // everything past the wave's last unit
+        const int rc = upload_packed(ctx, slots, b, codes + w.g0, w.g1 - w.g0, R);
+        if (rc != MASHGPU_OK) return fail(ctx, rc, "packed upload failed");
+        ctx->kernel_launches++;             // apply_runs_kernel
         wstart[b].resize(w.u1 - w.u0 + 1);
         for (uint64_t u = w.u0; u <= w.u1; u++) wstart[b][u - w.u0] = unit_start[u] - p0;
         return MASHGPU_OK;
@@ -1449,15 +1444,9 @@ extern "C" int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketc
             if (rc != MASHGPU_OK) break;
         }
         MG_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->pack_copied[b], 0));
-        const uint64_t nu = w.u1 - w.u0;
         SketchStream S;
-        S.d_codes = d_codes[b]; S.d_inval = d_inval[b]; S.unit_start = wstart[b].data(); S.n_units = nu;
-        rc = sketch_stream_core(ctx, params, S, d_hashes, d_counts, d_n, ctx->stream, nullptr);
-        if (rc != MASHGPU_OK) break;
-        MG_CUDA(ctx, cudaMemcpyAsync(out_hashes + w.u0 * s, d_hashes, nu * s * 8ull, cudaMemcpyDeviceToHost, ctx->stream));
-        MG_CUDA(ctx, cudaMemcpyAsync(out_n + w.u0, d_n, nu * 4ull, cudaMemcpyDeviceToHost, ctx->stream));
-        if (out_counts) MG_CUDA(ctx, cudaMemcpyAsync(out_counts + w.u0 * s, d_counts, nu * s * 4ull, cudaMemcpyDeviceToHost, ctx->stream));
-        MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        S.d_codes = slots.d_codes[b]; S.d_inval = slots.d_inval[b]; S.unit_start = wstart[b].data(); S.n_units = w.u1 - w.u0;
+        rc = sketch_wave(ctx, params, S, w.u0, out);
     }
     cudaStreamSynchronize(ctx->pack_stream);
     return rc;
