@@ -306,6 +306,37 @@ int mashgpu_dist(mashgpu_ctx *ctx, const mashgpu_sketch_set *ref, const mashgpu_
                  uint32_t *numer, uint32_t *denom, double *distance, double *pvalue, uint8_t *pass);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * `mash within`: containment of query sketches in reference sketches, every pair (CommandContain.cpp:205-265).
+ * ------------------------------------------------------------------------------------------------------- */
+typedef struct mashgpu_within_job mashgpu_within_job;
+
+/* Uploads both sets (qry == NULL or qry == ref: every sketch of one set against every other and itself) and encodes them with
+ * the order-preserving 32-bit dictionary of mashgpu_dist_open.  Reference rows take part in full: unlike dist's rows they are not
+ * cut to a sketch size (containSketches walks min(|R|, |Q|) query hashes but as many reference hashes as it needs,
+ * CommandContain.cpp:231-258).  Each row r holds n_hashes[r] ascending distinct hashes; a row with n_hashes > stride is refused
+ * (MASHGPU_ERR_INVALID) before any work.  length is not read (NULL allowed).  max_error: the -e threshold of writeOutput
+ * (CommandContain.cpp:179-203), as the double the caller compares with -- the CLI passes (double)(float)e. */
+int mashgpu_within_open(mashgpu_ctx *ctx, const mashgpu_sketch_set *ref, const mashgpu_sketch_set *qry, double max_error,
+                        mashgpu_within_job **job);
+/* containSketches(ref r, query q) for queries [q_begin, q_begin + q_count) and every reference, pair (q, r) written at
+ * (q - q_begin) * n_ref + r (the query-major order of CommandContain.cpp:143-175):
+ *   common    shared hashes among the query hashes examined
+ *   examined  j, the query hashes examined: min(min(|R|, |Q|), #{query hashes <= the largest reference hash})
+ *   score     common / j (CommandContain.cpp:264); for j == 0 the x86 result of 0.0 / 0, a NaN with the sign bit set
+ *   error     1 / sqrt(j) (:262); +inf for j == 0
+ *   pass      error <= max_error (writeOutput, :189)
+ * score and error are bit-identical to the reference's.  Reference sketches of up to 1034 hashes run a tiled lockstep merge
+ * (32 references per shared-memory tile), larger ones a warp-per-pair merge.  Any output pointer may be NULL.  Host buffers;
+ * the device outputs are cut into chunks of 2^24 pairs. */
+int mashgpu_within_run(mashgpu_within_job *job, uint64_t q_begin, uint64_t q_count, uint32_t *common, uint32_t *examined,
+                       double *score, double *error, uint8_t *pass);
+/* Same with device output buffers, enqueued on `stream` (cudaStream_t, NULL = context stream); runs of one job may be in flight
+ * on several streams at once (the job keeps no per-run scratch). */
+int mashgpu_within_run_dev(mashgpu_within_job *job, uint64_t q_begin, uint64_t q_count, uint32_t *d_common, uint32_t *d_examined,
+                           double *d_score, double *d_error, uint8_t *d_pass, void *stream);
+int mashgpu_within_close(mashgpu_within_job *job);
+
+/* ---------------------------------------------------------------------------------------------------------
  * Hot path 3: screen (containment of reference sketches in a read stream).
  * ------------------------------------------------------------------------------------------------------- */
 typedef struct mashgpu_screen_job mashgpu_screen_job;

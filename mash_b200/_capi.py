@@ -118,6 +118,11 @@ def load_library():
     L.mashgpu_dist_prefilter_stats.argtypes = [C.c_void_p, u64p, u64p, C.POINTER(C.c_int)]
     L.mashgpu_dist_pair_stats.argtypes = [C.c_void_p, u64p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
+    L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
+    L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
+    L.mashgpu_within_run_dev.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p]
+    L.mashgpu_within_close.argtypes = [C.c_void_p]
     L.mashgpu_screen_open.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.POINTER(SketchSet), C.POINTER(C.c_void_p)]
     L.mashgpu_screen_feed.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     L.mashgpu_screen_feed_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
@@ -314,6 +319,11 @@ class Engine:
                   max_distance=1.0, max_pvalue=1.0):
         return DistJob(self, ref, ref_n, ref_len, qry, qry_n, qry_len, sketch_size, k, kmer_space, max_distance, max_pvalue)
 
+    def within_open(self, ref, ref_n, qry=None, qry_n=None, *, max_error=0.05):
+        """`mash within` job: containment of every query sketch in every reference sketch (qry None: the set against itself).
+        max_error is compared as a double; the CLI's -e is a float, so pass float32(e) to reproduce it."""
+        return WithinJob(self, ref, ref_n, qry, qry_n, max_error)
+
     def dist_open_encoded(self, d_rows, d_n_eff, d_length, n_rows, ref_begin, ref_count, *, sketch_size, k, kmer_space,
                           max_distance=1.0, max_pvalue=1.0, keepalive=None):
         """Job over dictionary-encoded rows in device memory (pointers); references = rows [ref_begin, ref_begin + ref_count)."""
@@ -441,6 +451,44 @@ class DistJob:
     def close(self):
         if self.h:
             self.eng.lib.mashgpu_dist_close(self.h)
+            self.h = None
+
+
+class WithinJob:
+    def __init__(self, eng, ref, ref_n, qry, qry_n, max_error):
+        self.eng = eng
+        self._ref = ref if isinstance(ref, _Set) else _Set(ref, ref_n)
+        self._qry = qry if (qry is None or isinstance(qry, _Set)) else _Set(qry, qry_n)
+        self.n_ref = int(self._ref.c.n)
+        self.n_qry = self.n_ref if self._qry is None else int(self._qry.c.n)
+        h = C.c_void_p()
+        eng._check(eng.lib.mashgpu_within_open(eng.h, C.byref(self._ref.c), C.byref(self._qry.c) if self._qry is not None else None,
+                                               float(max_error), C.byref(h)))
+        self.h = h
+
+    WITHIN_OUTPUTS = (("common", np.uint32, u32p), ("examined", np.uint32, u32p), ("score", np.float64, f64p), ("error", np.float64, f64p),
+                      ("pass", np.uint8, u8p))
+
+    def run(self, q_begin, q_count, outputs=("common", "examined", "score", "error", "pass")):
+        """(q_count, n_ref) arrays of the named outputs; the others are passed as NULL."""
+        n = q_count * self.n_ref
+        unknown = set(outputs) - {name for name, _, _ in self.WITHIN_OUTPUTS}
+        if unknown:
+            raise ValueError(f"unknown within outputs {sorted(unknown)}")
+        arrs = {name: np.zeros(n, dt) for name, dt, _ in self.WITHIN_OUTPUTS if name in outputs}
+        ptrs = [_p(arrs[name], pt) if name in arrs else None for name, _, pt in self.WITHIN_OUTPUTS]
+        self.eng._check(self.eng.lib.mashgpu_within_run(self.h, q_begin, q_count, *ptrs))
+        out = {name: a.reshape(q_count, self.n_ref) for name, a in arrs.items()}
+        if "pass" in out:
+            out["pass"] = out["pass"].astype(bool)
+        return out
+
+    def run_dev(self, q_begin, q_count, d_common=None, d_examined=None, d_score=None, d_error=None, d_pass=None, stream=None):
+        self.eng._check(self.eng.lib.mashgpu_within_run_dev(self.h, q_begin, q_count, d_common, d_examined, d_score, d_error, d_pass, stream))
+
+    def close(self):
+        if self.h:
+            self.eng.lib.mashgpu_within_close(self.h)
             self.h = None
 
 

@@ -29,16 +29,10 @@
 
 #include "common.cuh"
 #include "binom.cuh"
+#include "dict.cuh"
 #include "dist_filter.cuh"
 
 namespace mashgpu {
-
-constexpr uint32_t RANK_PAD = 0xFFFFFFFFu;
-constexpr int DIST_WARPS = 12;
-constexpr int DIST_ILP = 2;
-constexpr int DIST_THREADS = DIST_WARPS * 32;
-constexpr int DIST_TILE_R = 32;
-static_assert(DIST_TILE_R * 4 == 128, "the merge step's PTX hard-codes the 128-byte stride of the interleaved reference tile");
 
 struct FixEntry;
 struct DistArgs {
@@ -86,13 +80,6 @@ __device__ __forceinline__ void dist_list_append(const DistArgs &a, uint64_t o, 
     if (at < a.list_capacity) {
         a.list_idx[at] = o; a.list_numer[at] = common; a.list_denom[at] = denom; a.list_distance[at] = dist; a.list_pvalue[at] = p;
     }
-}
-
-__device__ __forceinline__ uint32_t lds32(uint32_t addr)
-{
-    uint32_t v;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr));
-    return v;
 }
 
 // distance of compareSketches (CommandDistance.cpp:387-407)
@@ -162,18 +149,7 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
     }
 }
 
-// The query rows are staged by the TMA engine (cp.async.bulk global -> shared, completion on a per-warp mbarrier).  A row of
-// P ranks starts at a 4-byte aligned address (pitch P words), the bulk copy needs 16: the copy covers the 16-byte aligned
-// span around the row and the merge starts `skew` bytes into the warp's buffer.
-__host__ __device__ __forceinline__ uint32_t dist_qpitch(uint32_t P) { return (P + 4u + 3u) & ~3u; }
-
-// Dynamic shared memory of dist_kernel for rows of P ranks: the reference tile, the query buffers and the mbarriers.  Sketch
-// sizes for which it exceeds 227 KB are not tiled.
-inline size_t dist_smem_bytes(uint32_t P)
-{
-    return ((((size_t)P * DIST_TILE_R + 3) & ~(size_t)3) + (size_t)DIST_WARPS * DIST_ILP * dist_qpitch(P)) * 4 + DIST_WARPS * 8;
-}
-
+// (query rows staged by TMA, dist_qpitch / dist_smem_bytes: dict.cuh)
 __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
 {
     extern __shared__ __align__(16) uint32_t smem[];
@@ -840,15 +816,9 @@ struct mashgpu_dist_job {
     ~mashgpu_dist_job() { if (flag_event) cudaEventDestroy(flag_event); }
 };
 
-namespace {
+namespace mashgpu {
 
-// device copies of a sketch set's arrays (uploaded when the set lives in host memory)
-struct SetOnDevice {
-    const uint64_t *hashes = nullptr; const uint32_t *n_hashes = nullptr; const uint64_t *length = nullptr;
-    DevBuf<uint64_t> h, l; DevBuf<uint32_t> n;
-};
-
-int stage_set(mashgpu_ctx *ctx, const mashgpu_sketch_set *s, SetOnDevice &d, cudaStream_t st, bool want_length = true)
+int stage_set(mashgpu_ctx *ctx, const mashgpu_sketch_set *s, SetOnDevice &d, cudaStream_t st, bool want_length)
 {
     if (s->on_device) { d.hashes = s->hashes; d.n_hashes = s->n_hashes; d.length = s->length; return MASHGPU_OK; }
     if (d.h.alloc(s->n * s->stride) != cudaSuccess || d.n.alloc(s->n) != cudaSuccess || (want_length && d.l.alloc(s->n) != cudaSuccess))
@@ -860,17 +830,13 @@ int stage_set(mashgpu_ctx *ctx, const mashgpu_sketch_set *s, SetOnDevice &d, cud
     return MASHGPU_OK;
 }
 
-int check_set(mashgpu_ctx *ctx, const mashgpu_sketch_set *s, const char *what, bool want_length = true)
+int check_set(mashgpu_ctx *ctx, const mashgpu_sketch_set *s, const char *what, bool want_length)
 {
     if (!s) return fail(ctx, MASHGPU_ERR_INVALID, "%s set is NULL", what);
     if (s->n && (!s->hashes || !s->n_hashes || (want_length && !s->length))) return fail(ctx, MASHGPU_ERR_INVALID, "%s set has NULL arrays", what);
     return MASHGPU_OK;
 }
 
-inline unsigned blocks_for(uint64_t n, unsigned tb = 256) { return (unsigned)std::max<uint64_t>(1, (n + tb - 1) / tb); }
-
-// Valid hashes of a device-resident set -> keys[out0 ...] / slots[out0 ...] (compacted, row order); n_eff[row0 + row] filled.
-// Returns the number of entries through *n_out (synchronises the stream once to read it).
 int dict_gather(mashgpu_ctx *ctx, const SetOnDevice &d, uint64_t n_rows, uint64_t stride, uint32_t P, uint64_t row0, uint32_t *n_eff,
                 uint64_t out0, uint64_t *keys, uint32_t *slots, uint64_t *n_out, cudaStream_t st)
 {
@@ -895,8 +861,6 @@ int dict_gather(mashgpu_ctx *ctx, const SetOnDevice &d, uint64_t n_rows, uint64_
     return MASHGPU_OK;
 }
 
-// out[vals[t]] = rank of keys[t] among the distinct keys (keys in any order; `keys` and `vals` are clobbered).
-// *n_distinct is read back (synchronises the stream).
 int dict_rank(mashgpu_ctx *ctx, uint64_t *keys, uint32_t *vals, uint64_t n, uint32_t *out, uint64_t *n_distinct, cudaStream_t st)
 {
     *n_distinct = 0;
@@ -925,6 +889,27 @@ int dict_rank(mashgpu_ctx *ctx, uint64_t *keys, uint32_t *vals, uint64_t n, uint
     *n_distinct = nd;
     return MASHGPU_OK;
 }
+
+int encode_rows(mashgpu_ctx *ctx, const SetOnDevice &ref, uint64_t n_ref, uint64_t ref_stride, const SetOnDevice *qry, uint64_t n_qry,
+                uint64_t qry_stride, uint32_t P, uint32_t *ranks, uint32_t *n_eff, cudaStream_t st)
+{
+    const uint64_t rows = n_ref + (qry ? n_qry : 0), total = rows * P;
+    if (rows == 0) return MASHGPU_OK;
+    DevBuf<uint64_t> keys; DevBuf<uint32_t> slots;
+    if (keys.alloc(total) != cudaSuccess || slots.alloc(total) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (dictionary scratch for %llu hashes)", (unsigned long long)total);
+    uint64_t n_r = 0, n_q = 0, n_distinct = 0;
+    MG_TRY(dict_gather(ctx, ref, n_ref, ref_stride, P, 0, n_eff, 0, keys.p, slots.p, &n_r, st));
+    if (qry) MG_TRY(dict_gather(ctx, *qry, n_qry, qry_stride, P, n_ref, n_eff, n_r, keys.p, slots.p, &n_q, st));
+    MG_CUDA(ctx, cudaMemsetAsync(ranks, 0xFF, total * 4, st));                  // padding code everywhere, then the real ranks
+    MG_TRY(dict_rank(ctx, keys.p, slots.p, n_r + n_q, ranks, &n_distinct, st));
+    if (n_distinct >= 0xFFFFFFFFull) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "more than 2^32 - 1 distinct hashes");
+    return MASHGPU_OK;
+}
+
+}  // namespace mashgpu
+
+namespace {
 
 // distance LUT, binomial table, kernel attributes and the environment switches: everything of a job but the rank rows
 int dist_job_tables(mashgpu_ctx *ctx, mashgpu_dist_job *job, cudaStream_t st)
@@ -1016,16 +1001,9 @@ extern "C" int mashgpu_dist_open(mashgpu_ctx *ctx, const mashgpu_sketch_set *ref
     job->d_ranks = job->ranks.p; job->d_n_eff = job->n_eff.p; job->d_lens = job->lens.p;
     job->ref_row0 = 0; job->qry_row0 = self ? 0 : job->n_ref;
     if (rows) {
-        DevBuf<uint64_t> keys; DevBuf<uint32_t> slots;
-        if (keys.alloc(total) != cudaSuccess || slots.alloc(total) != cudaSuccess)
-            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (dictionary scratch for %llu hashes)", (unsigned long long)total);
-        uint64_t n_r = 0, n_q = 0, n_distinct = 0;
-        if (trace) fprintf(stderr, "[mashgpu] dist_open: staging + 5 allocations (%.0f MB) %.2f ms\n", total * 16e-6, now() - t_open);
-        MG_TRY(dict_gather(ctx, dr, job->n_ref, ref->stride, P, 0, job->n_eff.p, 0, keys.p, slots.p, &n_r, st));
-        if (!self) MG_TRY(dict_gather(ctx, dq, job->n_qry, qry->stride, P, job->n_ref, job->n_eff.p, n_r, keys.p, slots.p, &n_q, st));
-        MG_CUDA(ctx, cudaMemsetAsync(job->ranks.p, 0xFF, total * 4, st));                  // padding code everywhere, then the real ranks
-        MG_TRY(dict_rank(ctx, keys.p, slots.p, n_r + n_q, job->ranks.p, &n_distinct, st));
-        if (n_distinct >= 0xFFFFFFFFull) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "more than 2^32 - 1 distinct hashes");
+        if (trace) fprintf(stderr, "[mashgpu] dist_open: staging + rank rows (%.0f MB) %.2f ms\n", total * 4e-6, now() - t_open);
+        MG_TRY(encode_rows(ctx, dr, job->n_ref, ref->stride, self ? nullptr : &dq, job->n_qry, self ? 0 : qry->stride, P, job->ranks.p,
+                           job->n_eff.p, st));
         MG_CUDA(ctx, cudaMemcpyAsync(job->lens.p, dr.length, job->n_ref * 8, cudaMemcpyDeviceToDevice, st));
         if (!self && job->n_qry)
             MG_CUDA(ctx, cudaMemcpyAsync(job->lens.p + job->n_ref, dq.length, job->n_qry * 8, cudaMemcpyDeviceToDevice, st));

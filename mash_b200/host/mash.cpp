@@ -1,9 +1,9 @@
-// mash.cpp -- thin command-line front end over the host shim: `mash sketch | dist | triangle | screen | taxscreen | info | paste`.
-// Mirrors the reference's command drivers (CommandSketch.cpp:36-169, CommandDistance.cpp:44-304,
-// CommandTriangle.cpp:45-214, CommandScreen.cpp:54-461, CommandTaxScreen.cpp:57-480, CommandInfo.cpp:222-299): same option
-// identifiers and defaults (Command.cpp:165-200), same stdout formats (iostream default precision), same ordering contracts.
-// It exists so that the reference's `make test` flow can be replayed against the GPU engine; help text, `bounds`,
-// `within` and `find` are out of scope.
+// mash.cpp -- thin command-line front end over the host shim: `mash sketch | dist | triangle | within | screen | taxscreen | info |
+// paste`.  Mirrors the reference's command drivers (CommandSketch.cpp:36-169, CommandDistance.cpp:44-304,
+// CommandTriangle.cpp:45-214, CommandContain.cpp:33-203, CommandScreen.cpp:54-461, CommandTaxScreen.cpp:57-480,
+// CommandInfo.cpp:222-299): same option identifiers and defaults (Command.cpp:165-200), same stdout formats (iostream default
+// precision), same ordering contracts.  It exists so that the reference's `make test` flow can be replayed against the GPU engine;
+// help text, `bounds` and `find` are out of scope.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -390,6 +390,81 @@ int runDist(int argc, const char **argv)
         mashgpu_dist_close(job);
     }
     if (w.warningCount > 0 && !parameters.reads) warnKmerSize(parameters, w.lengthMax, w.lengthMaxName, w.randomChance, w.kMin, w.warningCount);
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- within
+int runWithin(int argc, const char **argv)   // reference CommandContain.cpp:33-203
+{
+    Command c;
+    c.add("help", Option(Option::Boolean, "h", ""));
+    c.add("list", Option(Option::Boolean, "l", ""));
+    c.add("errorThreshold", Option(Option::Number, "e", "0.05"));
+    c.useSketchOptions();
+    if (c.parse(argc, argv)) return 1;
+    if (c.arguments.size() < 2 || c.opt("help").active) { cerr << "usage: mash within [options] <reference> <query> [<query>] ..." << endl; return 0; }
+    const float errorMax = c.opt("errorThreshold").number;      // writeOutput takes it as a float (:179)
+    Sketch::Parameters parameters;
+    if (sketchParameterSetup(parameters, c)) return 1;
+    Sketch sketchRef;
+    const string &fileReference = c.arguments[0];
+    bool isSketch = hasSuffix(fileReference, suffixSketch);
+    if (isSketch) {
+        // no dash before the identifier here (unlike dist); -a and -z are reported and ignored (:60-82)
+        for (const char *o : {"kmer", "noncanonical", "protein", "alphabet"})
+            if (c.opt(o).active) {
+                cerr << "ERROR: The option " << c.opt(o).identifier << " cannot be used when a sketch is provided; it is inherited from the sketch." << endl;
+                if (!strcmp(o, "kmer") || !strcmp(o, "noncanonical")) return 1;
+            }
+    } else {
+        cerr << "Sketching " << fileReference << " (provide sketch file made with \"mash sketch\" to skip)...";
+    }
+    vector<string> refArgVector(1, fileReference);
+    sketchRef.initFromFiles(refArgVector, parameters);
+    if (isSketch) {
+        parameters.minHashesPerWindow = sketchRef.getMinHashesPerWindow();
+        parameters.kmerSize = sketchRef.getKmerSize();
+        parameters.noncanonical = sketchRef.getNoncanonical();
+        parameters.preserveCase = sketchRef.getPreserveCase();
+        parameters.seed = sketchRef.getHashSeed();
+        string alphabet;
+        sketchRef.getAlphabetAsString(alphabet);
+        setAlphabetFromString(parameters, alphabet.c_str());
+    } else {
+        cerr << "done.\n";
+    }
+    vector<string> queryFiles;
+    for (size_t i = 1; i < c.arguments.size(); i++) { if (c.opt("list").active) splitFile(c.arguments[i], queryFiles); else queryFiles.push_back(c.arguments[i]); }
+    Sketch sketchQuery;
+    sketchQuery.initFromFiles(queryFiles, parameters, 0, true, true);      // contain: a query .msh with a smaller s is used, not skipped
+
+    // With no reference sketch the reference divides by zero (iFloor, :137); here nothing is printed.
+    const uint64_t nRef = sketchRef.getReferenceCount(), nQry = sketchQuery.getReferenceCount();
+    if (nRef && nQry) {
+        mashgpu_sketch_set setRef, setQry;
+        vector<uint64_t> hR, lR, hQ, lQ; vector<uint32_t> nR, nQ;
+        sketchRef.toSketchSet(setRef, hR, nR, lR);
+        sketchQuery.toSketchSet(setQry, hQ, nQ, lQ);
+        mashgpu_within_job *job = 0;
+        if (mashgpu_within_open(gpuContext(), &setRef, &setQry, (double)errorMax, &job) != MASHGPU_OK) gpuFail();
+        const uint64_t rows = std::max<uint64_t>(1, (1ull << 24) / nRef);
+        vector<double> score, error; vector<uint8_t> pass;
+        const uint64_t cap = std::min(rows, nQry) * nRef;
+        score.resize(cap); error.resize(cap); pass.resize(cap);
+        for (uint64_t q = 0; q < nQry; q += rows) {
+            const uint64_t r = std::min(rows, nQry - q);
+            if (mashgpu_within_run(job, q, r, nullptr, nullptr, score.data(), error.data(), pass.data()) != MASHGPU_OK) gpuFail();
+            mashhost::writeRows(r, parameters.parallelism, nRef, [&](uint64_t i, mashhost::OutBuf &o) {   // == writeOutput, :179-203
+                for (uint64_t j = 0; j < nRef; j++) {
+                    const size_t k = i * nRef + j;
+                    if (!pass[k]) continue;
+                    o.dbl(score[k]); o.ch('\t'); o.dbl(error[k]); o.ch('\t');
+                    o.str(sketchRef.getReference(j).name); o.ch('\t'); o.str(sketchQuery.getReference(q + i).name); o.ch('\n');
+                }
+            });
+        }
+        mashgpu_within_close(job);
+    }
     return 0;
 }
 
@@ -903,6 +978,7 @@ static int runCommand(int argc, const char **argv)
     if (cmd == "sketch") return runSketch(argc - 2, argv + 2);
     if (cmd == "dist") return runDist(argc - 2, argv + 2);
     if (cmd == "triangle") return runTriangle(argc - 2, argv + 2);
+    if (cmd == "within") return runWithin(argc - 2, argv + 2);
     if (cmd == "screen") return runScreen(argc - 2, argv + 2);
     if (cmd == "taxscreen") return runTaxScreen(argc - 2, argv + 2);
     if (cmd == "tax-dump") return runTaxDump(argc - 2, argv + 2);
@@ -917,7 +993,7 @@ static int runCommand(int argc, const char **argv)
 int main(int argc, const char **argv)
 {
     if (argc < 2) {
-        cerr << "usage: mash <sketch|dist|triangle|screen|taxscreen|info|paste> ...   (H100 engine; see INTEGRATION.md)" << endl;
+        cerr << "usage: mash <sketch|dist|triangle|within|screen|taxscreen|info|paste> ...   (H100 engine; see INTEGRATION.md)" << endl;
         return 0;
     }
     const int rc = runCommand(argc, argv);
