@@ -265,6 +265,39 @@ int mashgpu_dist_prefilter_stats(mashgpu_dist_job *job, uint64_t *combos_probed,
  * *pairs_merged_from_lists: pairs that took this path since the job was opened.  Synchronises the device. */
 int mashgpu_dist_pair_stats(mashgpu_dist_job *job, uint64_t *pairs_merged_from_lists);
 
+/* Best hits: the n_best nearest references of every query, selected on the device (no counterpart in the reference, whose
+ * users pipe `mash dist` into sort; `mash dist -B`).  A HIT of query q is a reference r whose pair (q, r) has pass == 1 in
+ * mashgpu_dist_run (so max_distance, max_pvalue and mashgpu_dist_set_triangle apply unchanged) and numer > 0.  Pairs without a
+ * shared hash all sit at distance 1 and p-value 1 and are left out on purpose; so is the pair of two EMPTY sketches, which has
+ * numer == denom == 0 and distance 0.  The best list of q is its hits ordered by (distance ascending as a double, reference
+ * index ascending), cut to n_best: the first n_best rows of a stable sort of q's row of the dense grid once the rows with
+ * numer == 0 or pass == 0 are dropped.  numer, denom, distance and pvalue of a hit are bit-identical to what
+ * mashgpu_dist_run returns for the pair from the same job.
+ * Row (q - q_begin) of ref / numer / denom / distance / pvalue holds n_best entries in rank order, n_hits[q - q_begin] of them
+ * valid (the entries past them are zero); n_total (may be NULL) is the number of hits the query has in all.  ref is relative
+ * to the job's references (to ref_begin for mashgpu_dist_open_encoded), like the column of the grid.
+ * 1 <= n_best <= 1024: 0 is MASHGPU_ERR_INVALID, more MASHGPU_ERR_UNSUPPORTED, both before any work.  In a self comparison
+ * every non-empty sketch is its own nearest hit: ask for n_best + 1.
+ * The output is q_count x n_best entries instead of q_count x n_ref, so a search of a large collection runs at the speed of
+ * the kernels, not of the link to the host.  Works on every kind of job and every merge path.  Host buffers. */
+int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count, uint32_t n_best,
+                          uint32_t *n_hits, uint32_t *n_total, uint32_t *ref, uint32_t *numer, uint32_t *denom, double *distance,
+                          double *pvalue);
+/* Same with device output buffers and a stream (NULL = context stream); entries past n_hits are zero here too.  The hits are
+ * captured in a bounded candidate buffer, block of queries by block, and the call reads the candidate count of every block on
+ * the host (it synchronises `stream`, as mashgpu_dist_run_list does): a block whose hits exceed the buffer is discarded and run
+ * again as two halves, so no hit is ever dropped.  The rule of mashgpu_dist_run_dev holds: one run of a job in flight. */
+int mashgpu_dist_run_best_dev(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count, uint32_t n_best,
+                              uint32_t *d_n_hits, uint32_t *d_n_total, uint32_t *d_ref, uint32_t *d_numer, uint32_t *d_denom,
+                              double *d_distance, double *d_pvalue, void *stream);
+/* Capacity of the candidate buffer in entries (32 bytes each, held twice).  Default 2^25; never below the number of references,
+ * so that the hits of one query always fit (smaller values are raised to it, 0 restores the default), and below 2^32. */
+int mashgpu_dist_set_best_capacity(mashgpu_dist_job *job, uint64_t entries);
+/* Counters of the best runs since the job was opened: blocks of queries run (the re-runs of split blocks included), blocks
+ * discarded and split because their hits exceeded the candidate buffer, hits captured by the blocks that were kept, and, when
+ * mashgpu_set_timing is on, the device time of grouping and selection.  Any pointer may be NULL. */
+int mashgpu_dist_best_stats(mashgpu_dist_job *job, uint64_t *blocks_run, uint64_t *blocks_split, uint64_t *candidates, double *select_ms);
+
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE
  * instead (a sample sort): a rank sorts only its own rows' hashes, the sorted keys are cut at G-1 splitters, every rank

@@ -117,6 +117,11 @@ def load_library():
     L.mashgpu_dist_set_triangle.argtypes = [C.c_void_p, C.c_int]
     L.mashgpu_dist_prefilter_stats.argtypes = [C.c_void_p, u64p, u64p, C.POINTER(C.c_int)]
     L.mashgpu_dist_pair_stats.argtypes = [C.c_void_p, u64p]
+    L.mashgpu_dist_run_best.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, u32p, u32p, u32p, u32p, u32p, f64p, f64p]
+    L.mashgpu_dist_run_best_dev.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.mashgpu_dist_set_best_capacity.argtypes = [C.c_void_p, C.c_uint64]
+    L.mashgpu_dist_best_stats.argtypes = [C.c_void_p, u64p, u64p, u64p, f64p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
     L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
@@ -432,6 +437,31 @@ class DistJob:
 
     def run_dev(self, q_begin, q_count, d_numer=None, d_denom=None, d_distance=None, d_pvalue=None, d_pass=None, stream=None):
         self.eng._check(self.eng.lib.mashgpu_dist_run_dev(self.h, q_begin, q_count, d_numer, d_denom, d_distance, d_pvalue, d_pass, stream))
+
+    def run_best(self, q_begin, q_count, n_best):
+        """The n_best nearest references of every query among its hits (pass and numer > 0), by (distance, reference index).
+        Returns n_hits, n_total of shape (q_count,) and ref, numer, denom, distance, pvalue of shape (q_count, n_best) in rank
+        order; entries past n_hits are zero."""
+        shp = (q_count, max(0, min(int(n_best), 1024)))        # an n_best out of range is refused by the library
+        n_hits = np.zeros(q_count, np.uint32); n_total = np.zeros(q_count, np.uint32)
+        ref = np.zeros(shp, np.uint32); numer = np.zeros(shp, np.uint32); denom = np.zeros(shp, np.uint32)
+        dist = np.zeros(shp, np.float64); pv = np.zeros(shp, np.float64)
+        self.eng._check(self.eng.lib.mashgpu_dist_run_best(self.h, q_begin, q_count, n_best, _p(n_hits, u32p), _p(n_total, u32p), _p(ref, u32p),
+                                                           _p(numer, u32p), _p(denom, u32p), _p(dist, f64p), _p(pv, f64p)))
+        return {"n_hits": n_hits, "n_total": n_total, "ref": ref, "numer": numer, "denom": denom, "distance": dist, "pvalue": pv}
+
+    def run_best_dev(self, q_begin, q_count, n_best, d_n_hits, d_n_total, d_ref, d_numer, d_denom, d_distance, d_pvalue, stream=None):
+        self.eng._check(self.eng.lib.mashgpu_dist_run_best_dev(self.h, q_begin, q_count, n_best, d_n_hits, d_n_total, d_ref, d_numer, d_denom,
+                                                               d_distance, d_pvalue, stream))
+
+    def set_best_capacity(self, entries):
+        """Candidate buffer of run_best in entries (0 = default); values below n_ref are raised to it."""
+        self.eng._check(self.eng.lib.mashgpu_dist_set_best_capacity(self.h, int(entries)))
+
+    def best_stats(self):
+        blocks = C.c_uint64(0); splits = C.c_uint64(0); cands = C.c_uint64(0); ms = C.c_double(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_best_stats(self.h, C.byref(blocks), C.byref(splits), C.byref(cands), C.byref(ms)))
+        return {"blocks_run": blocks.value, "blocks_split": splits.value, "candidates": cands.value, "select_ms": ms.value}
 
     def set_prefilter(self, mode):
         """-1 = auto (default), 0 = merge every pair, 1 = always probe the reference tiles first."""

@@ -18,6 +18,8 @@
 //   dist_kernel        the merge, on the tiles' work lists (or on every pair when the prefilter is off)
 //   dist_fix_kernel    p-value / pass flag / pass-list entry of the pairs with shared hashes, evaluated densely
 // Results are identical with and without the prefilter (tests/test_gpu_dist_prefilter.py).
+// A best run (mashgpu_dist_run_best, DESIGN.md 3.7) runs the same kernels with no dense output: the two places that know a pair's
+// final pass flag, dist_emit and dist_fix_kernel, capture the hits, and dist_best.cuh selects the N nearest of every query.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -31,6 +33,7 @@
 #include "binom.cuh"
 #include "dict.cuh"
 #include "dist_filter.cuh"
+#include "dist_best.cuh"
 
 namespace mashgpu {
 
@@ -70,6 +73,7 @@ struct DistArgs {
     int pair_dense;             // dist_pair_kernel enumerates every pair of the run itself (sketch sizes beyond the tiled merge)
     // deferred p-values (dist_fix_kernel): pairs with shared hashes whose binomial tail is evaluated in a dense second pass
     struct FixEntry *fix_list; unsigned long long *fix_count; uint64_t fix_capacity;
+    BestCapture best;           // best runs: hits (pass, common > 0) are captured here; every dense output and the pass list are NULL then
 };
 
 struct FixEntry { uint64_t o; uint32_t common, denom; };
@@ -126,6 +130,7 @@ __device__ __forceinline__ void dist_emit(const DistArgs &a, uint32_t q, uint32_
     if (a.distance) a.distance[o] = dist;
     if (deferred) return;
     if (a.list_idx && pass) dist_list_append(a, o, common, denom, dist, p);
+    if (a.best.cand && pass && common) dist_best_append(a.best, q - a.q_begin, r, common, denom, dist, p);
     if (a.pvalue) a.pvalue[o] = p;
     if (a.pass) a.pass[o] = pass ? 1 : 0;
 }
@@ -140,9 +145,10 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
         const uint32_t q = a.q_begin + (uint32_t)(e.o / a.n_ref), r = (uint32_t)(e.o % a.n_ref);
         const double p = mash_pvalue(e.common, a.ref_len[r], a.qry_len[q], a.kmer_space, e.denom, &a.binom);
         const bool pass = !(a.max_pvalue >= 0 && p > a.max_pvalue);
-        if (a.list_idx && pass) {
+        if ((a.list_idx || a.best.cand) && pass) {
             const double dist = (e.denom == a.S) ? a.dist_lut[e.common] : mash_distance(e.common, e.denom, a.kmer_size);
-            dist_list_append(a, e.o, e.common, e.denom, dist, p);
+            if (a.list_idx) dist_list_append(a, e.o, e.common, e.denom, dist, p);
+            else dist_best_append(a.best, q - a.q_begin, r, e.common, e.denom, dist, p);      // queued pairs share a hash
         }
         if (a.pvalue) a.pvalue[e.o] = p;
         if (a.pass) a.pass[e.o] = pass ? 1 : 0;
@@ -484,7 +490,9 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
         } else if (mine && !((mask >> lane) & 1u)) {
             // empty intersection: the merge would take min(s', |A| + |B|) union steps and count nothing
             const uint32_t denom = min(a.S, nA + nB_all);
-            if (denom == a.S && a.list_idx && pass_const == 0) {
+            if (a.best.cand) {
+                // best run: a pair without a shared hash is not a hit, whatever its denominator
+            } else if (denom == a.S && a.list_idx && pass_const == 0) {
                 // filtered run (-d / -v) and distance 1 / p-value 1 does not pass: nothing to write for this pair
             } else if (denom == a.S && !a.list_idx) {
                 const uint64_t o = (uint64_t)(q - a.q_begin) * a.n_ref + r;
@@ -795,6 +803,16 @@ struct mashgpu_dist_job {
     // grow-only buffers of mashgpu_dist_run_list (no cudaMalloc per call after the first)
     DevBuf<uint64_t> l_idx, s_idx; DevBuf<uint32_t> l_n, l_d, l_order, s_order, o_n, o_d; DevBuf<double> l_D, l_P, o_D, o_P;
     DevBuf<unsigned long long> l_cnt; DevBuf<uint8_t> l_tmp;
+    // best hits (mashgpu_dist_run_best_dev): capture target of the next run, grow-only buffers, counters since the job was opened
+    BestCapture best{};
+    uint64_t best_capacity = 0;         // mashgpu_dist_set_best_capacity; 0 = default
+    DevBuf<BestCand> b_cand, b_grouped;
+    DevBuf<uint32_t> b_q;               // per query of a block: hits, segment offset, scatter cursor
+    DevBuf<unsigned long long> b_cnt;
+    DevBuf<uint8_t> b_tmp;
+    uint64_t best_blocks = 0, best_splits = 0, best_candidates = 0;
+    double best_select_ms = 0;
+    std::vector<EventPair> best_events;
     // prefilter (dist_probe_kernel): -1 = auto (on; switched off when most combinations turn out to share hashes), 0 = off, 1 = on
     int prefilter_mode = -1;
     bool triangle = false;
@@ -1241,6 +1259,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     a.triangle = job->triangle ? 1 : 0;
     a.tri_r0 = job->self ? 0u : (uint32_t)job->ref_row0;
     a.pair_list = nullptr; a.pair_count = nullptr; a.pair_full = nullptr; a.pair_capacity = 0; a.pair_total = nullptr; a.pair_max = 0; a.pair_dense = 0;
+    a.best = job->best;
     {   // queue for the deferred p-values: 1/16 of the pairs (at least 2^20); beyond that dist_emit evaluates in place
         const uint64_t pairs = q_count * job->n_ref;
         const uint64_t cap = std::min<uint64_t>(pairs, std::max<uint64_t>(1ull << 20, pairs / 16));
@@ -1461,11 +1480,150 @@ extern "C" int mashgpu_dist_run_list(mashgpu_dist_job *job, uint64_t q_begin, ui
     return MASHGPU_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Best hits (DESIGN.md 3.7)
+// ---------------------------------------------------------------------------------------------------------
+constexpr uint64_t BEST_DEFAULT_CAPACITY = 1ull << 25;      // candidates: 1 GiB of capture buffer and 1 GiB of grouped copy
+constexpr uint64_t BEST_BLOCK_PAIRS = 1ull << 31;           // pairs of a starting block: bounds the work lists and queues of one run
+constexpr uint64_t BEST_HOST_ENTRIES = 1ull << 24;          // q x n_best entries per device output chunk of the host call
+
+extern "C" int mashgpu_dist_set_best_capacity(mashgpu_dist_job *job, uint64_t entries)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    job->best_capacity = std::min<uint64_t>(entries, 0xFFFFFFFFull);       // segment offsets are 32-bit
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_best_stats(mashgpu_dist_job *job, uint64_t *blocks_run, uint64_t *blocks_split, uint64_t *candidates, double *select_ms)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    cudaSetDevice(job->ctx->device);
+    for (auto &ev : job->best_events) {
+        cudaEventSynchronize(ev.b);
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, ev.a, ev.b) == cudaSuccess) job->best_select_ms += ms;
+        cudaEventDestroy(ev.a);
+        cudaEventDestroy(ev.b);
+    }
+    job->best_events.clear();
+    if (blocks_run) *blocks_run = job->best_blocks;
+    if (blocks_split) *blocks_split = job->best_splits;
+    if (candidates) *candidates = job->best_candidates;
+    if (select_ms) *select_ms = job->best_select_ms;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_run_best_dev(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count, uint32_t n_best,
+                                         uint32_t *d_n_hits, uint32_t *d_n_total, uint32_t *d_ref, uint32_t *d_numer, uint32_t *d_denom,
+                                         double *d_distance, double *d_pvalue, void *stream)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (n_best == 0) return fail(ctx, MASHGPU_ERR_INVALID, "n_best must be at least 1");
+    if (n_best > BEST_MAX_N) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "n_best %u exceeds %u", n_best, BEST_MAX_N);
+    if (q_begin + q_count > job->n_qry) return fail(ctx, MASHGPU_ERR_INVALID, "query range [%llu, %llu) exceeds %llu", (unsigned long long)q_begin, (unsigned long long)(q_begin + q_count), (unsigned long long)job->n_qry);
+    if (q_count == 0) return MASHGPU_OK;
+    if (!d_n_hits || !d_ref || !d_numer || !d_denom || !d_distance || !d_pvalue) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    const uint64_t n_ref = job->n_ref;
+    if (n_ref == 0) {       // no reference, no hit
+        const uint64_t e = q_count * n_best;
+        MG_CUDA(ctx, cudaMemsetAsync(d_n_hits, 0, q_count * 4, st));
+        if (d_n_total) MG_CUDA(ctx, cudaMemsetAsync(d_n_total, 0, q_count * 4, st));
+        MG_CUDA(ctx, cudaMemsetAsync(d_ref, 0, e * 4, st)); MG_CUDA(ctx, cudaMemsetAsync(d_numer, 0, e * 4, st)); MG_CUDA(ctx, cudaMemsetAsync(d_denom, 0, e * 4, st));
+        MG_CUDA(ctx, cudaMemsetAsync(d_distance, 0, e * 8, st)); MG_CUDA(ctx, cudaMemsetAsync(d_pvalue, 0, e * 8, st));
+        return MASHGPU_OK;
+    }
+    // never below n_ref: a block of one query always fits, which is where the halving below ends
+    const uint64_t capacity = std::max<uint64_t>(n_ref, job->best_capacity ? job->best_capacity : BEST_DEFAULT_CAPACITY);
+    const uint64_t block0 = std::max<uint64_t>(1, BEST_BLOCK_PAIRS / n_ref);
+    uint32_t kw = 1;
+    while (kw < n_best) kw <<= 1;
+    mashgpu_dist_job &J = *job;
+    // blocks still to run, next one last; a block whose candidates overflow the buffer is replaced by its two halves
+    std::vector<std::pair<uint64_t, uint64_t>> todo;
+    for (uint64_t q = (q_count + block0 - 1) / block0; q-- > 0;) todo.push_back({q * block0, std::min(block0, q_count - q * block0)});
+    while (!todo.empty()) {
+        const uint64_t b0 = todo.back().first, bn = todo.back().second;
+        todo.pop_back();
+        const uint64_t cap = std::min(capacity, bn * n_ref);        // a block has at most bn * n_ref hits
+        if (J.b_cand.reserve(cap) != cudaSuccess || J.b_grouped.reserve(cap) != cudaSuccess || J.b_q.reserve(3 * bn) != cudaSuccess || J.b_cnt.reserve(1) != cudaSuccess)
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (best-hit candidates: %llu entries)", (unsigned long long)cap);
+        uint32_t *qcnt = J.b_q.p, *qoff = qcnt + bn, *cursor = qoff + bn;
+        MG_CUDA(ctx, cudaMemsetAsync(J.b_cnt.p, 0, 8, st));
+        MG_CUDA(ctx, cudaMemsetAsync(qcnt, 0, 3 * bn * 4, st));
+        job->best = BestCapture{J.b_cand.p, J.b_cnt.p, cap, qcnt};
+        const int rc = mashgpu_dist_run_dev(job, q_begin + b0, bn, nullptr, nullptr, nullptr, nullptr, nullptr, st);
+        job->best = BestCapture{};
+        MG_TRY(rc);
+        unsigned long long n = 0;
+        MG_CUDA(ctx, cudaMemcpyAsync(&n, J.b_cnt.p, 8, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        job->best_blocks++;
+        if (n > cap) {      // bn >= 2 here: one query has at most n_ref <= cap hits
+            job->best_splits++;
+            todo.push_back({b0 + bn / 2, bn - bn / 2});
+            todo.push_back({b0, bn / 2});
+            continue;
+        }
+        job->best_candidates += n;
+        time_begin(ctx, job->best_events, st);
+        size_t tb = 0;
+        cub::DeviceScan::ExclusiveSum(nullptr, tb, qcnt, qoff, (int)bn, st);
+        if (J.b_tmp.reserve(tb) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (scan scratch)");
+        MG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(J.b_tmp.p, tb, qcnt, qoff, (int)bn, st));
+        if (n) best_scatter_kernel<<<blocks_for(n), 256, 0, st>>>(J.b_cand.p, n, qoff, cursor, J.b_grouped.p);
+        const BestOut o{d_n_hits + b0, d_n_total ? d_n_total + b0 : nullptr, d_ref + b0 * n_best, d_numer + b0 * n_best, d_denom + b0 * n_best,
+                        d_distance + b0 * n_best, d_pvalue + b0 * n_best};
+        dist_best_kernel<<<blocks_for(bn, BEST_WARPS), BEST_THREADS, 0, st>>>(J.b_grouped.p, qoff, qcnt, (uint32_t)bn, n_best, kw, o);
+        MG_CUDA(ctx, cudaGetLastError());
+        time_end(ctx, job->best_events, st);
+        ctx->kernel_launches += 4;
+    }
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count, uint32_t n_best,
+                                     uint32_t *n_hits, uint32_t *n_total, uint32_t *ref, uint32_t *numer, uint32_t *denom, double *distance, double *pvalue)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (n_best == 0) return fail(ctx, MASHGPU_ERR_INVALID, "n_best must be at least 1");
+    if (n_best > BEST_MAX_N) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "n_best %u exceeds %u", n_best, BEST_MAX_N);
+    if (q_begin + q_count > job->n_qry) return fail(ctx, MASHGPU_ERR_INVALID, "query range exceeds query count");
+    if (q_count == 0) return MASHGPU_OK;
+    if (!n_hits || !ref || !numer || !denom || !distance || !pvalue) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    // bound the device outputs: chunks of queries (each is cut into blocks by the device call)
+    const uint64_t q_chunk = std::min<uint64_t>(q_count, std::max<uint64_t>(1, BEST_HOST_ENTRIES / n_best));
+    const uint64_t e_chunk = q_chunk * n_best;
+    DevBuf<uint32_t> dh, dt, dr, dn, dd; DevBuf<double> dD, dP;
+    if (dh.alloc(q_chunk) != cudaSuccess || dt.alloc(q_chunk) != cudaSuccess || dr.alloc(e_chunk) != cudaSuccess || dn.alloc(e_chunk) != cudaSuccess ||
+        dd.alloc(e_chunk) != cudaSuccess || dD.alloc(e_chunk) != cudaSuccess || dP.alloc(e_chunk) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (best-hit outputs)");
+    for (uint64_t q = 0; q < q_count; q += q_chunk) {
+        const uint64_t qc = std::min(q_chunk, q_count - q), e = qc * n_best, o = q * n_best;
+        MG_TRY(mashgpu_dist_run_best_dev(job, q_begin + q, qc, n_best, dh.p, dt.p, dr.p, dn.p, dd.p, dD.p, dP.p, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(n_hits + q, dh.p, qc * 4, cudaMemcpyDeviceToHost, st));
+        if (n_total) MG_CUDA(ctx, cudaMemcpyAsync(n_total + q, dt.p, qc * 4, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(ref + o, dr.p, e * 4, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(numer + o, dn.p, e * 4, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(denom + o, dd.p, e * 4, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(distance + o, dD.p, e * 8, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(pvalue + o, dP.p, e * 8, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+    }
+    return MASHGPU_OK;
+}
+
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)
 {
     if (!job) return MASHGPU_ERR_INVALID;
     cudaSetDevice(job->ctx->device);
     cudaStreamSynchronize(job->ctx->stream);
+    for (auto &ev : job->best_events) { cudaEventDestroy(ev.a); cudaEventDestroy(ev.b); }
     delete job;
     return MASHGPU_OK;
 }

@@ -273,6 +273,29 @@ struct PairBlock {
     void resize(size_t n) { numer.resize(n); denom.resize(n); distance.resize(n); pValue.resize(n); pass.resize(n); }
 };
 
+// `mash dist -B`: per query its nBest nearest references that share a hash with it, nearest first, in the five columns of writeOutput.
+// The engine selects on the device and returns rows x nBest entries, so the blocks are sized by that and not by rows x nRef.
+static void writeBestHits(mashgpu_dist_job *job, uint32_t nBest, const Sketch &sketchRef, const Sketch &sketchQuery, bool comment, int threads)
+{
+    const uint64_t nQry = sketchQuery.getReferenceCount();
+    const uint64_t rows = std::min<uint64_t>(nQry, std::max<uint64_t>(1, (1ull << 22) / nBest));
+    vector<uint32_t> hits(rows), ref(rows * nBest), numer(rows * nBest), denom(rows * nBest);
+    vector<double> distance(rows * nBest), pValue(rows * nBest);
+    for (uint64_t q = 0; q < nQry; q += rows) {
+        const uint64_t r = std::min(rows, nQry - q);
+        if (mashgpu_dist_run_best(job, q, r, nBest, hits.data(), 0, ref.data(), numer.data(), denom.data(), distance.data(), pValue.data()) != MASHGPU_OK) gpuFail();
+        mashhost::writeRows(r, threads, nBest, [&](uint64_t i, mashhost::OutBuf &o) {
+            for (uint64_t e = i * nBest; e < i * nBest + hits[i]; e++) {
+                o.str(sketchRef.getReference(ref[e]).name);
+                if (comment) { o.ch(':'); o.str(sketchRef.getReference(ref[e]).comment); }
+                o.ch('\t'); o.str(sketchQuery.getReference(q + i).name);
+                if (comment) { o.ch(':'); o.str(sketchQuery.getReference(q + i).comment); }
+                o.ch('\t'); o.dbl(distance[e]); o.ch('\t'); o.dbl(pValue[e]); o.ch('\t'); o.u64(numer[e]); o.ch('/'); o.u64(denom[e]); o.ch('\n');
+            }
+        });
+    }
+}
+
 int runDist(int argc, const char **argv)
 {
     Command c;
@@ -282,10 +305,17 @@ int runDist(int argc, const char **argv)
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.add("comment", Option(Option::Boolean, "C", ""));
+    c.add("best", Option(Option::Integer, "B", "", 1, 1024));      // not an option of the reference: its users pipe into sort
     c.useSketchOptions();
     if (c.parse(argc, argv)) return 1;
-    if (c.arguments.size() < 2 || c.opt("help").active) { cerr << "usage: mash dist [options] <reference> <query> [<query>] ..." << endl; return 0; }
+    if (c.arguments.size() < 2 || c.opt("help").active) {
+        cerr << "usage: mash dist [options] <reference> <query> [<query>] ..." << endl
+             << "  -B <int>  Best hits: per query only its <int> nearest references that share a hash with it, nearest first (1-1024; not with -t)." << endl;
+        return 0;
+    }
     bool table = c.opt("table").active, comment = c.opt("comment").active;
+    const uint32_t nBest = c.opt("best").active ? (uint32_t)c.opt("best").number : 0;
+    if (nBest && table) { cerr << "ERROR: The option -B cannot be used with -t (a table has one column per reference)." << endl; return 1; }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number;
     Sketch::Parameters parameters;
     if (sketchParameterSetup(parameters, c)) return 1;
@@ -341,16 +371,18 @@ int runDist(int argc, const char **argv)
         sketchQuery.toSketchSet(setQry, hQ, nQ, lQ);
         mashgpu_dist_job *job = 0;
         if (mashgpu_dist_open(gpuContext(), &setRef, &setQry, &dp, &job) != MASHGPU_OK) gpuFail();
+        if (nBest) writeBestHits(job, nBest, sketchRef, sketchQuery, comment, parameters.parallelism);
+        const uint64_t nDense = nBest ? 0 : nQry;       // queries still to be printed pair by pair
         uint64_t rows = std::max<uint64_t>(1, (1ull << 24) / nRef);
         PairBlock out;
-        out.resize(std::min(rows, nQry) * nRef);
+        out.resize(std::min(rows, nDense) * nRef);
         // with -d / -v filters only the passing pairs are needed (writeOutput prints nothing else): ask the engine for the
         // compacted pass-list, already in query-major order, instead of the dense grid
         const bool filtered = !table && (distanceMax < 1.0 || pValueMax < 1.0);
         const uint64_t listCapacity = 1ull << 22;
         vector<uint64_t> lIdx; vector<uint32_t> lNumer, lDenom; vector<double> lDist, lP;
         if (filtered) { lIdx.resize(listCapacity); lNumer.resize(listCapacity); lDenom.resize(listCapacity); lDist.resize(listCapacity); lP.resize(listCapacity); }
-        for (uint64_t q = 0; q < nQry; q += rows) {
+        for (uint64_t q = 0; q < nDense; q += rows) {
             uint64_t r = std::min(rows, nQry - q);
             if (filtered) {
                 uint64_t nPass = 0;

@@ -50,6 +50,53 @@ def exchange_query_tiles(hashes, n_hashes, lengths, counts=None, group=None):
     return torch.cat(out_h), torch.cat(out_n), torch.cat(out_l), counts
 
 
+BEST_INT_KEYS = ("n_hits", "n_total", "ref", "numer", "denom")
+BEST_LIST_KEYS = ("ref", "numer", "denom", "distance", "pvalue")
+
+
+def merge_best_lists(parts, n_best):
+    """Best lists of several reference shards (dicts as DistJob.run_best returns them, as tensors, `ref` already global, the same Q
+    and n_best in each) -> the best lists over all of them: hits ordered by (distance ascending, reference ascending), cut to
+    n_best; entries past n_hits are zero.  n_total is the sum over the shards."""
+    hits = torch.stack([p["n_hits"] for p in parts])                                    # (shards, Q)
+    cols = {k: torch.cat([p[k] for p in parts], dim=1) for k in BEST_LIST_KEYS}         # (Q, shards * n_best)
+    q, dev = hits.shape[1], hits.device
+    rank = torch.arange(n_best, device=dev)
+    valid = (rank.view(1, 1, -1) < hits.permute(1, 0).unsqueeze(2)).reshape(q, -1)
+    # stable sort by reference, then by distance: ties in distance stay in reference order; invalid entries go last
+    key_ref = torch.where(valid, cols["ref"], torch.full_like(cols["ref"], torch.iinfo(torch.int64).max))
+    order = torch.sort(key_ref, dim=1, stable=True).indices
+    key_d = torch.where(valid, cols["distance"], torch.full_like(cols["distance"], float("inf"))).gather(1, order)
+    order = order.gather(1, torch.sort(key_d, dim=1, stable=True).indices)[:, :n_best]
+    n_hits = torch.clamp(hits.sum(0), max=n_best)
+    keep = rank.view(1, -1) < n_hits.view(-1, 1)
+    out = {k: torch.where(keep, v.gather(1, order), torch.zeros_like(v[:, :n_best])) for k, v in cols.items()}
+    out["n_hits"] = n_hits
+    out["n_total"] = torch.stack([p["n_total"] for p in parts]).sum(0)
+    return out
+
+
+def merge_best(local, ref_begin, n_best, group=None):
+    """Global best hits from per-shard ones.  With the reference axis sharded, DistJob.run_best on a rank yields each query's best
+    list over that rank's references only; the union of the per-shard top n_best contains the global top n_best, so merging them
+    under the same order rule (with GLOBAL reference indices) is exact.
+
+    local: what run_best returned on this rank (numpy arrays or tensors; the same Q and n_best on every rank); ref_begin: global
+    index of this rank's reference 0.  Returns the merged dict on every rank, as tensors on the device of the inputs (integers as
+    int64)."""
+    world = td.get_world_size(group)
+    mine = {k: torch.as_tensor(v) for k, v in local.items()}
+    mine = {k: v.to(torch.int64 if k in BEST_INT_KEYS else torch.float64).contiguous() for k, v in mine.items()}
+    mine["ref"] = mine["ref"] + int(ref_begin)
+    parts = [dict() for _ in range(world)]
+    for k, v in mine.items():
+        got = [torch.empty_like(v) for _ in range(world)]
+        td.all_gather(got, v, group=group)
+        for r in range(world):
+            parts[r][k] = got[r]
+    return merge_best_lists(parts, n_best)
+
+
 class DictOps:
     """The four device steps of the sharded dictionary build, on torch tensors (C ABI: mashgpu_dict_*).  The CPU tests pass
     a stand-in with the same methods to exercise the exchange protocol under gloo."""
