@@ -13,7 +13,7 @@ struct u64x2 { uint32_t lo, hi; };
 // The hot loop is bound by the ALU pipe (SHF/LOP3/IADD3/PRMT).  Moving 64-bit adds, shifts, rotates or the PRMT selector
 // shift onto the FMA pipe through opaque power-of-two IMADs made the k=21 scan slower on B200 and on H100 (IMAD.WIDE/IMAD.HI
 // cost more issue slots than the SHF/IADD3 they replace); the scan uses the FMA pipe only where an add can ride on a
-// multiply-add that is there anyway (fmix_hi).
+// multiply-add that is there anyway (block 0's seed in murmur3_body).
 
 __device__ __forceinline__ u64x2 mul_const(u64x2 a, uint64_t c)
 {
@@ -54,6 +54,19 @@ __device__ __forceinline__ u64x2 mul5_add(u64x2 a, uint32_t c)
     return r;
 }
 
+// a * 5 + c, c a 64-bit value (block 0's h1 step with the seed folded into its addend, see murmur3_body): one IMAD.WIDE
+// with the register pair c as its addend, and one IMAD for the high word.  c passes through an empty asm: otherwise the
+// compiler factors the 5 back out of a * 5 + seed * 5 and adds the seed again.
+__device__ __forceinline__ u64x2 mul5_add64(u64x2 a, u64x2 c)
+{
+    uint64_t cc = ((uint64_t)c.hi << 32) | c.lo;
+    asm("" : "+l"(cc));
+    const uint64_t t = (uint64_t)a.lo * 5u + cc;
+    u64x2 r{(uint32_t)t, (uint32_t)(t >> 32)};
+    asm("mad.lo.u32 %0, %1, 5, %0;" : "+r"(r.hi) : "r"(a.hi));
+    return r;
+}
+
 __device__ __forceinline__ uint32_t shr1(uint32_t x) { return x >> 1; }
 
 __device__ __forceinline__ u64x2 fmix(u64x2 k)
@@ -66,17 +79,20 @@ __device__ __forceinline__ u64x2 fmix(u64x2 k)
     return k;
 }
 
-// high word of fmix(k), plus `add` (the final `k ^= k >> 33` only changes the low word).  The addend enters the first
-// multiply-add (IMAD.HI), so summing two of these and a constant stays on the FMA pipe.
-__device__ __forceinline__ uint32_t fmix_hi(u64x2 k, uint32_t add)
+// High word of fmix(k), on the FMA pipe alone (the final `k ^= k >> 33` only changes the low word): hi32(k.lo * c_lo) as
+// an IMAD.HI with a zero addend (the zero register pair, no move), then + k.lo * c_hi + k.hi * c_lo.  A nonzero 32-bit
+// addend would need a register pair {0, add}, which ptxas builds with IMAD.MOVs before every call.
+__device__ __forceinline__ uint32_t fmix_hi(u64x2 k)
 {
     k.lo ^= shr1(k.hi);
     k = mul_const(k, 0xff51afd7ed558ccdULL);
     k.lo ^= shr1(k.hi);
     constexpr uint64_t c = 0xc4ceb9fe1a85ec53ULL;
-    uint32_t r;
-    asm("mad.hi.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(k.lo), "n"((uint32_t)c), "r"(add));
-    return r + k.lo * (uint32_t)(c >> 32) + k.hi * (uint32_t)c;
+    uint32_t r = (uint32_t)(((uint64_t)k.lo * (uint32_t)c) >> 32);
+    // the two low products as a chain of multiply-adds on r (in C they are summed first, and the sum added with an IMAD.IADD)
+    asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(r) : "r"(k.lo), "n"((uint32_t)(c >> 32)));
+    asm("mad.lo.u32 %0, %1, %2, %0;" : "+r"(r) : "r"(k.hi), "n"((uint32_t)c));
+    return r;
 }
 
 // k1 of the tail block, rotl31(t * c1) * c2, where t holds the tail's (at most 8) bytes; when the tail has 8 bytes or fewer,
@@ -98,11 +114,16 @@ __device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t s
     constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
     constexpr int NB = K / 16, TAIL = K & 15;
     u64x2 h1{seed, 0u}, h2{seed, 0u};
+    // block 0 adds h2 while it is still the seed: (r + seed) * 5 + C = r * 5 + (seed * 5 + C) mod 2^64, so the seed rides
+    // on the multiply-add's addend (a loop invariant of the scan kernels) instead of a 64-bit add per hash
+    const uint64_t s5 = (uint64_t)seed * 5u + 0x52dce729u;
 #pragma unroll
     for (int b = 0; b < NB; b++) {
         u64x2 k1{a[4 * b], a[4 * b + 1]}, k2{a[4 * b + 2], a[4 * b + 3]};
         k1 = mul_const(k1, c1); k1 = rotl<31>(k1); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
-        h1 = rotl<27>(h1); h1 = add64(h1, h2); h1 = mul5_add(h1, 0x52dce729u);
+        h1 = rotl<27>(h1);
+        if (b == 0) h1 = mul5_add64(h1, u64x2{(uint32_t)s5, (uint32_t)(s5 >> 32)});
+        else { h1 = add64(h1, h2); h1 = mul5_add(h1, 0x52dce729u); }
         k2 = mul_const(k2, c2); k2 = rotl<33>(k2); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
         h2 = rotl<31>(h2); h2 = add64(h2, h1); h2 = mul5_add(h2, 0x38495ab5u);
     }
@@ -139,15 +160,14 @@ __device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t se
 //   H <= T  implies  X <= T + 1
 // (carry 0: X = H + 1 <= T + 1;  carry 1: X = H), so `X <= T + 1` (or anything, when T = 2^32 - 1) never rejects a hash
 // whose high word is <= T.  It lets through at most the one extra high word T + 1 and X = 0 (high words summing to
-// 2^32 - 1); the slow path recomputes the exact hash.  tests/test_scan_filter_model.py models this predicate.
+// 2^32 - 1); the slow path recomputes the exact hash.  tests/test_scan_filter_model.py models this predicate.  The two
+// high words and the 1 are summed by one three-input IADD3.
 template <int K, int NA, bool K1_GIVEN = false>
 __device__ __forceinline__ uint32_t murmur3_h1_filter(const uint32_t (&a)[NA], uint32_t seed, u64x2 k1_tail = u64x2{0u, 0u})
 {
     u64x2 h1, h2;
     murmur3_body<K, NA, K1_GIVEN>(a, seed, h1, h2, k1_tail);
-    uint32_t one;    // opaque, so that ptxas keeps the +1 as the IMAD.HI addend rather than a separate add on the ALU pipe
-    asm("mov.u32 %0, 1;" : "=r"(one));
-    return fmix_hi(h2, fmix_hi(h1, one));
+    return fmix_hi(h1) + fmix_hi(h2) + 1u;
 }
 
 // threshold for murmur3_h1_filter's word, from the exact high-word threshold T = tmax >> 32: T + 1, saturated at 2^32 - 1

@@ -648,6 +648,18 @@ __device__ __forceinline__ uint32_t ascii8_to_word(uint32_t lo, uint32_t hi, uin
     return __byte_perm(x0, x1, 0x6420) | (__byte_perm(x0, x1, 0x7531) << 4);
 }
 
+// 8 ASCII bytes -> one nibble word of the codes ((u >> 1) ^ (u >> 2)) & 3 alone (fold only touches bit 5, so the codes come
+// from the raw bytes), and into `diff` the bits in which the upper-cased bytes differ from the ACGT bytes of their codes,
+// rebuilt by PRMT from `pool`.  A byte is in the alphabet exactly when it equals the ACGT byte of its own code, so `diff`
+// stays 0 exactly when all 8 bytes are, and then the word is what ascii8_to_word gives.
+__device__ __forceinline__ uint32_t ascii8_to_code_word(uint32_t lo, uint32_t hi, uint32_t fold, uint32_t pool, uint32_t &diff)
+{
+    const uint32_t x0 = ((lo >> 1) ^ (lo >> 2)) & 0x03030303u, x1 = ((hi >> 1) ^ (hi >> 2)) & 0x03030303u;
+    const uint32_t w = __byte_perm(x0, x1, 0x6420) | (__byte_perm(x0, x1, 0x7531) << 4);
+    diff |= (prmt(pool, 0, w) ^ (lo & fold)) | (prmt(pool, 0, w >> 16) ^ (hi & fold));
+    return w;
+}
+
 // the nibble word of the 8 bytes at stream offset `off`, with the bytes at or past stream_len made separators
 __device__ __forceinline__ uint32_t clip_word(uint32_t w, uint64_t off, uint64_t stream_len)
 {
@@ -817,8 +829,18 @@ scan_kernel(const __grid_constant__ ScanArgs a)
     const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(smr), 0);
     const uint32_t land = (uint32_t)__cvta_generic_to_shared(land_all[FULL ? 0 : warp]);
     const uint32_t fold = a.preserve_case ? 0xFFFFFFFFu : 0xDFDFDFDFu;
-    uint32_t pool;   // bytes 'A','C','G','T' for PRMT; opaque to the compiler so that it stays in one register
-    asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
+    // the bytes 'A','C','G','T' for PRMT.  Filter-word kernels: each lane reads the pool back from its own word of the warp's
+    // tile (word 2 lane, which only this lane stages later), so that ptxas keeps it in one register for the whole kernel.  A
+    // constant, even through a shuffle or %laneid arithmetic, is rebuilt before every PRMT instead (an IMAD.U32 each).  The
+    // FULL kernels keep the constant.
+    uint32_t pool;
+    if (FULL) {
+        asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
+    } else {
+        const uint32_t at = (uint32_t)__cvta_generic_to_shared(sm) + 8u * lane;
+        asm volatile("st.shared.u32 [%0], %1;" :: "r"(at), "r"(0x54474341u) : "memory");
+        asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(pool) : "r"(at) : "memory");
+    }
 
     const uint64_t wt_begin = a.tile_begin * (SCAN_TILE / SCAN_WARP_TILE);
     const uint64_t wt_end = a.tile_end * (SCAN_TILE / SCAN_WARP_TILE);
@@ -883,16 +905,29 @@ scan_kernel(const __grid_constant__ ScanArgs a)
                     make_uint4(nibble_reverse(e1.w) ^ 0x33333333u, nibble_reverse(e1.z) ^ 0x33333333u, nibble_reverse(e1.y) ^ 0x33333333u, nibble_reverse(e1.x) ^ 0x33333333u);
             }
         } else if constexpr (!FULL) {
-            uint32_t w0 = ascii8_to_word(q0.x, q0.y, fold), w1 = ascii8_to_word(q0.z, q0.w, fold);
-            uint32_t w2 = ascii8_to_word(q1.x, q1.y, fold), w3 = ascii8_to_word(q1.z, q1.w, fold);
-            uint32_t w4 = ascii8_to_word(q2.x, q2.y, fold);
-            if (base + 16ull * SCAN_WARP_VECS > a.stream_len) {   // warp-uniform: only the last tile of a launch
-                const uint64_t o0 = base + 16ull * lane, o1 = o0 + 16ull * 32;
-                w0 = clip_word(w0, o0, a.stream_len);
-                w1 = clip_word(w1, o0 + 8, a.stream_len);
-                w2 = clip_word(w2, o1, a.stream_len);
-                w3 = clip_word(w3, o1 + 8, a.stream_len);
-                w4 = clip_word(w4, base + 16ull * 64 + 8ull * hw, a.stream_len);
+            // A tile of ACGT bytes alone (upper-cased unless preserve_case), halo included, is converted to codes only and
+            // checked with one vote.  A tile with any other byte (N, IUPAC codes, a record separator, lower case under
+            // preserve_case) is converted again with the validity test, as is the last tile of a launch, which reaches
+            // past stream_len (warp-uniform); bit 3 of a nibble marks a base outside the alphabet as before.
+            const bool ragged = base + 16ull * SCAN_WARP_VECS > a.stream_len;
+            uint32_t w0, w1, w2, w3, w4, diff = 0;
+            if (!ragged) {
+                w0 = ascii8_to_code_word(q0.x, q0.y, fold, pool, diff); w1 = ascii8_to_code_word(q0.z, q0.w, fold, pool, diff);
+                w2 = ascii8_to_code_word(q1.x, q1.y, fold, pool, diff); w3 = ascii8_to_code_word(q1.z, q1.w, fold, pool, diff);
+                w4 = ascii8_to_code_word(q2.x, q2.y, fold, pool, diff);
+            }
+            if (ragged || __any_sync(0xFFFFFFFFu, diff != 0)) {
+                w0 = ascii8_to_word(q0.x, q0.y, fold), w1 = ascii8_to_word(q0.z, q0.w, fold);
+                w2 = ascii8_to_word(q1.x, q1.y, fold), w3 = ascii8_to_word(q1.z, q1.w, fold);
+                w4 = ascii8_to_word(q2.x, q2.y, fold);
+                if (ragged) {
+                    const uint64_t o0 = base + 16ull * lane, o1 = o0 + 16ull * 32;
+                    w0 = clip_word(w0, o0, a.stream_len);
+                    w1 = clip_word(w1, o0 + 8, a.stream_len);
+                    w2 = clip_word(w2, o1, a.stream_len);
+                    w3 = clip_word(w3, o1 + 8, a.stream_len);
+                    w4 = clip_word(w4, base + 16ull * 64 + 8ull * hw, a.stream_len);
+                }
             }
             stage_words<CANON>(sm, smr, lane, hw, w0, w1, w2, w3, w4);
         } else {
