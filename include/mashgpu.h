@@ -186,6 +186,13 @@ int mashgpu_sketch_batch_packed(mashgpu_ctx *ctx, const mashgpu_sketch_params *p
 int mashgpu_hash_windows(mashgpu_ctx *ctx, const mashgpu_sketch_params *params,
                          const char *seq, uint64_t len, uint64_t *out_hash, uint8_t *out_valid);
 
+/* Six-frame translation of one chunk, as the translated screen runs it: d_out receives the peptides of forward frames 0, 1, 2
+ * and then of reverse-complement frames 0, 1, 2, frame f holding (len - f) / 3 amino acids followed by one 0 byte, a stop or a
+ * codon with a byte outside {A,C,G,T} written as 0 -- 6 + 2 * sum_f (len - f) / 3 bytes in all.  Device buffers: d_seq must be
+ * readable up to len rounded up to 16 when it is 16-byte aligned (the kernel then loads whole vectors).  Runs on the context's
+ * stream and returns once the output is written.  Diagnostic/test entry point of the translation kernel. */
+int mashgpu_translate6(mashgpu_ctx *ctx, const void *d_seq, uint64_t len, int preserve_case, uint8_t *d_out);
+
 /* ---------------------------------------------------------------------------------------------------------
  * Hot path 2: all-pairs sketch comparison.
  * ------------------------------------------------------------------------------------------------------- */
@@ -395,7 +402,8 @@ int mashgpu_screen_open(mashgpu_ctx *ctx, const mashgpu_sketch_params *params, c
  * caller's buffer may be reused; results are complete at mashgpu_screen_finish.  (MASHGPU_SCREEN_HOST_PACK=1: the chunk is 2-bit
  * packed on the host threads and uploaded with an invalid-position mask instead of as ASCII.) */
 int mashgpu_screen_feed(mashgpu_screen_job *job, const char *chunk, uint64_t len);
-/* Same for a chunk already in device memory (readable up to len rounded up to 16). */
+/* Same for a chunk already in device memory (readable up to len rounded up to 16), at any address: an untranslated job
+ * scans a chunk that is not 16-byte aligned from an aligned device copy. */
 int mashgpu_screen_feed_dev(mashgpu_screen_job *job, const void *d_chunk, uint64_t len);
 /* Reduce (CommandScreen.cpp:288-355, 409-455): per reference sketch i the number of its hashes seen at least
  * once (shared), the median multiplicity depths[shared/2], identity (estimateIdentity, :463-482) and p-value

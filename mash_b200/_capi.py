@@ -108,6 +108,7 @@ def load_library():
     L.mashgpu_sketch_batch_packed.argtypes = [C.c_void_p, C.POINTER(SketchParams), u64p, C.c_uint64, u64p, C.c_uint64, u64p, C.c_uint64, u64p, u32p, u32p]
     L.mashgpu_host_pack.argtypes = [C.POINTER(SketchParams), C.c_uint64, C.c_void_p, u64p, C.c_int, u64p, u64p, C.c_uint64, u64p]
     L.mashgpu_hash_windows.argtypes = [C.c_void_p, C.POINTER(SketchParams), C.c_void_p, C.c_uint64, u64p, u8p]
+    L.mashgpu_translate6.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p]
     L.mashgpu_dist_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), C.POINTER(C.c_void_p)]
     L.mashgpu_dist_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_dist_run_dev.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -308,6 +309,11 @@ class Engine:
         v = np.zeros(max(1, n), np.uint8)
         self._check(self.lib.mashgpu_hash_windows(self.h, C.byref(p), b.ctypes.data, b.size, _p(h, u64p), _p(v, u8p)))
         return h[:n], v[:n].astype(bool)
+
+    def translate6(self, d_seq_ptr, length, preserve_case, d_out_ptr):
+        """Six-frame translation of `length` bases at device address d_seq_ptr into translated_length(length) bytes at
+        d_out_ptr: the six peptides, each followed by a 0 byte, stops and unknown codons as 0."""
+        self._check(self.lib.mashgpu_translate6(self.h, d_seq_ptr, length, int(preserve_case), d_out_ptr))
 
     # ---- hot path 2 ----------------------------------------------------------------------------------------
     def dist(self, ref, ref_n, ref_len, qry=None, qry_n=None, qry_len=None, *, sketch_size, k, kmer_space,

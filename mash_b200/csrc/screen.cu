@@ -555,6 +555,14 @@ extern "C" int mashgpu_screen_feed_dev(mashgpu_screen_job *job, const void *d_ch
     if (!d_chunk) return fail(ctx, MASHGPU_ERR_INVALID, "chunk is NULL");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     MG_TRY(screen_collect(job));
+    if (!job->translate && ((uintptr_t)d_chunk & 15)) {
+        // the scan kernels load their stream as aligned 16-byte vectors: a chunk at any other address is scanned from an aligned
+        // copy (a translated job reads the chunk with byte loads and scans its own peptide buffer)
+        if (job->stage[0].reserve((len + 15) / 16 * 16) != cudaSuccess)
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (chunk of %llu B)", (unsigned long long)len);
+        MG_CUDA(ctx, cudaMemcpyAsync(job->stage[0].p, d_chunk, len, cudaMemcpyDeviceToDevice, ctx->stream));
+        d_chunk = job->stage[0].p;
+    }
     MG_TRY(screen_enqueue(job, 0, d_chunk, len));
     return screen_collect(job);          // the caller's device buffer is free again when this returns
 }

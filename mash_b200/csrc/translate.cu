@@ -125,12 +125,11 @@ __global__ void __launch_bounds__(TR_THREADS) translate6_kernel(const uint8_t *_
 
 int translate_enqueue(mashgpu_ctx *ctx, const void *d_chunk, uint64_t len, int preserve_case, uint8_t *d_pep, cudaStream_t st)
 {
-    if (len == 0) return MASHGPU_OK;
     TrFrames fr;
     uint64_t o = 0;
     for (int f = 0; f < 3; f++) fr.n[f] = len > (uint64_t)f ? (len - f) / 3 : 0;
     for (int s = 0; s < 6; s++) { fr.base[s] = o; o += fr.n[s % 3] + 1; }
-    const uint64_t blocks = (len + TR_CTA_BASES - 1) / TR_CTA_BASES;
+    const uint64_t blocks = len ? (len + TR_CTA_BASES - 1) / TR_CTA_BASES : 1;      // an empty chunk still gets its six terminators
     if (blocks > 0x7FFFFFFFull) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "chunk of %llu bases too large to translate", (unsigned long long)len);
     const int aligned = ((uintptr_t)d_chunk & 15) == 0;
     time_begin(ctx, ctx->translate_events, st);
@@ -143,3 +142,15 @@ int translate_enqueue(mashgpu_ctx *ctx, const void *d_chunk, uint64_t len, int p
 }
 
 }  // namespace mashgpu
+
+using namespace mashgpu;
+
+extern "C" int mashgpu_translate6(mashgpu_ctx *ctx, const void *d_seq, uint64_t len, int preserve_case, uint8_t *d_out)
+{
+    if (!ctx) return MASHGPU_ERR_INVALID;
+    if (!d_seq || !d_out) return fail(ctx, MASHGPU_ERR_INVALID, "NULL argument");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    MG_TRY(translate_enqueue(ctx, d_seq, len, preserve_case, d_out, ctx->stream));
+    MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return MASHGPU_OK;
+}

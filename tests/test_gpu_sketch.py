@@ -165,8 +165,13 @@ def synth_protein(seed, n):
     return a[rng.choice(a.size, n, p=w / w.sum())]
 
 
-@pytest.mark.parametrize("k,alphabet,preserve_case", [(9, PROTEIN, False), (7, PROTEIN, False), (9, PROTEIN, True), (21, "ACGTN", False),
-                                                       (12, "ACGU", False), (32, PROTEIN, False), (1, "AB", False), (5, "acgt", True)])
+_BYTE_CASES = [(9, PROTEIN, False), (7, PROTEIN, False), (9, PROTEIN, True), (21, "ACGTN", False),
+               (12, "ACGU", False), (32, PROTEIN, False), (1, "AB", False), (5, "acgt", True)]
+# every k of the byte kernel with the protein alphabet (64-bit hashes from k = 8) and a 5-letter one (from k = 14), both case modes
+_BYTE_CASES += [c for c in ((k, a, pc) for a in (PROTEIN, "ACGTN") for pc in (False, True) for k in range(1, 33)) if c not in _BYTE_CASES]
+
+
+@pytest.mark.parametrize("k,alphabet,preserve_case", _BYTE_CASES)
 def test_byte_alphabets_every_window(gpu, oracle, k, alphabet, preserve_case):
     # `mash sketch -a` (protein, k=9) and `-z <alphabet>`: non-canonical, any byte alphabet (sketchParameterSetup.cpp:79-95)
     p = gpu.params(k=k, s=100, alphabet=alphabet, noncanonical=True, preserve_case=preserve_case)
