@@ -383,6 +383,21 @@ class Engine:
         return {f: getattr(st, f) for f, _ in Stats._fields_}
 
 
+def _run_grid(job, fn, what, table, q_begin, q_count, outputs):
+    """A host run of a pair grid: (q_count, n_ref) arrays of the named outputs of `table` ((name, dtype, pointer type) in the C
+    argument order); the others are passed as NULL. `pass` comes back as bool."""
+    unknown = set(outputs) - {name for name, _, _ in table}
+    if unknown:
+        raise ValueError(f"unknown {what} outputs {sorted(unknown)}")
+    arrs = {name: np.zeros(q_count * job.n_ref, dt) for name, dt, _ in table if name in outputs}
+    ptrs = [_p(arrs[name], pt) if name in arrs else None for name, _, pt in table]
+    job.eng._check(fn(job.h, q_begin, q_count, *ptrs))
+    out = {name: a.reshape(q_count, job.n_ref) for name, a in arrs.items()}
+    if "pass" in out:
+        out["pass"] = out["pass"].astype(bool)
+    return out
+
+
 class DistJob:
     def __init__(self, eng, ref, ref_n, ref_len, qry, qry_n, qry_len, sketch_size, k, kmer_space, max_distance, max_pvalue):
         self.eng = eng
@@ -419,18 +434,7 @@ class DistJob:
 
     def run(self, q_begin, q_count, outputs=("numer", "denom", "distance", "pvalue", "pass")):
         """(q_count, n_ref) arrays of the named outputs; the others are passed as NULL (neither copied back nor allocated)."""
-        n = q_count * self.n_ref
-        unknown = set(outputs) - {name for name, _, _ in self.DIST_OUTPUTS}
-        if unknown:
-            raise ValueError(f"unknown dist outputs {sorted(unknown)}")
-        arrs = {name: np.zeros(n, dt) for name, dt, _ in self.DIST_OUTPUTS if name in outputs}
-        ptrs = [_p(arrs[name], pt) if name in arrs else None for name, _, pt in self.DIST_OUTPUTS]
-        self.eng._check(self.eng.lib.mashgpu_dist_run(self.h, q_begin, q_count, *ptrs))
-        shp = (q_count, self.n_ref)
-        out = {name: a.reshape(shp) for name, a in arrs.items()}
-        if "pass" in out:
-            out["pass"] = out["pass"].astype(bool)
-        return out
+        return _run_grid(self, self.eng.lib.mashgpu_dist_run, "dist", self.DIST_OUTPUTS, q_begin, q_count, outputs)
 
     def run_list(self, q_begin, q_count, capacity):
         """Passing pairs only, sorted by pair index. Returns (n_pass, dict of arrays) -- arrays empty when n_pass > capacity."""
@@ -507,17 +511,7 @@ class WithinJob:
 
     def run(self, q_begin, q_count, outputs=("common", "examined", "score", "error", "pass")):
         """(q_count, n_ref) arrays of the named outputs; the others are passed as NULL."""
-        n = q_count * self.n_ref
-        unknown = set(outputs) - {name for name, _, _ in self.WITHIN_OUTPUTS}
-        if unknown:
-            raise ValueError(f"unknown within outputs {sorted(unknown)}")
-        arrs = {name: np.zeros(n, dt) for name, dt, _ in self.WITHIN_OUTPUTS if name in outputs}
-        ptrs = [_p(arrs[name], pt) if name in arrs else None for name, _, pt in self.WITHIN_OUTPUTS]
-        self.eng._check(self.eng.lib.mashgpu_within_run(self.h, q_begin, q_count, *ptrs))
-        out = {name: a.reshape(q_count, self.n_ref) for name, a in arrs.items()}
-        if "pass" in out:
-            out["pass"] = out["pass"].astype(bool)
-        return out
+        return _run_grid(self, self.eng.lib.mashgpu_within_run, "within", self.WITHIN_OUTPUTS, q_begin, q_count, outputs)
 
     def run_dev(self, q_begin, q_count, d_common=None, d_examined=None, d_score=None, d_error=None, d_pass=None, stream=None):
         self.eng._check(self.eng.lib.mashgpu_within_run_dev(self.h, q_begin, q_count, d_common, d_examined, d_score, d_error, d_pass, stream))

@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
     }
 }
 
-// (query rows staged by TMA, dist_qpitch / dist_smem_bytes: dict.cuh)
+// (reference tile and query rows: stage_ref_tile / bulk_span / bulk_copy_wait, layout: dist_qpitch / dist_smem_bytes, all in dict.cuh)
 __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
 {
     extern __shared__ __align__(16) uint32_t smem[];
@@ -174,21 +174,14 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
     const uint32_t *my_list = a.use_qlist ? a.qlist + (uint64_t)blockIdx.x * a.qlist_stride : nullptr;
     if ((uint64_t)blockIdx.y * a.q_per_cta >= n_items) return;          // nothing to do: do not even stage the tile
 
-    // stage the reference tile, interleaved: element i of reference (r0+l) at s_ref[i*32 + l]
-    {
-        const uint32_t *row = a.ranks + (a.ref_row0 + (r_ok ? r : r0)) * (uint64_t)a.P;
-        for (uint32_t i = warp; i < a.P; i += DIST_WARPS) s_ref[i * DIST_TILE_R + lane] = r_ok ? row[i] : RANK_PAD;
-    }
+    stage_ref_tile(s_ref, a.ranks, a.ref_row0, a.P, r0, a.n_ref);
     __syncthreads();
     const uint32_t nA = r_ok ? a.ref_n[r] : 0;
     const uint64_t lenA = r_ok ? a.ref_len[r] : 1;
     const uint32_t sref_base = (uint32_t)__cvta_generic_to_shared(s_ref) + lane * 4;
     uint32_t *my_q = s_qry + (size_t)warp * DIST_ILP * qpitch;
-    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(s_bar + warp);
+    const uint32_t bar = warp_bar_init(s_bar + warp);
     uint32_t phase = 0;
-    if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
 
     for (uint64_t it_lo = (uint64_t)blockIdx.y * a.q_per_cta; it_lo < n_items; it_lo += (uint64_t)gridDim.y * a.q_per_cta) {
     const uint32_t it_hi = (uint32_t)min((uint64_t)n_items, it_lo + a.q_per_cta);
@@ -203,40 +196,21 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) dist_kernel(const DistArgs a)
             all_skipped &= qs[c] == 0xFFFFFFFFu;
         }
         if (all_skipped) continue;                      // warp-uniform
-        // load DIST_ILP query rows into this warp's buffers, one bulk copy per row
+        // load DIST_ILP query rows into this warp's buffers; a skipped one is padding (the merge still takes its S steps)
         uint32_t skew[DIST_ILP], bytes[DIST_ILP], total = 0;
         const uint32_t *src[DIST_ILP];
 #pragma unroll
         for (int c = 0; c < DIST_ILP; c++) {
             skew[c] = 0; bytes[c] = 0; src[c] = nullptr;
             if (qs[c] != 0xFFFFFFFFu) {
-                const uintptr_t row = (uintptr_t)(a.ranks + (a.qry_row0 + qs[c]) * (uint64_t)a.P);
-                const uintptr_t lo = row & ~(uintptr_t)15, hi = (row + (uintptr_t)a.P * 4 + 15) & ~(uintptr_t)15;
-                skew[c] = (uint32_t)(row - lo);
-                src[c] = reinterpret_cast<const uint32_t *>(lo);
-                bytes[c] = (uint32_t)(hi - lo);
+                bytes[c] = bulk_span(a.ranks + (a.qry_row0 + qs[c]) * (uint64_t)a.P, a.P, src[c], skew[c]);
                 total += bytes[c];
             } else {
                 uint32_t *dst = my_q + (size_t)c * qpitch;
                 for (uint32_t i = lane; i < a.P; i += 32) dst[i] = RANK_PAD;
             }
         }
-        __syncwarp();
-        if (lane == 0 && total) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // the lanes' reads of the previous rows precede the async writes
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(total) : "memory");
-#pragma unroll
-            for (int c = 0; c < DIST_ILP; c++)
-                if (bytes[c])
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 :: "r"((uint32_t)__cvta_generic_to_shared(my_q + (size_t)c * qpitch)), "l"(src[c]), "r"(bytes[c]), "r"(bar) : "memory");
-        }
-        if (total) {
-            asm volatile("{\n\t.reg .pred p;\n\tDIST_BULK_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra DIST_BULK_WAIT;\n\t}"
-                         :: "r"(bar), "r"(phase) : "memory");
-            phase ^= 1;
-        }
-        __syncwarp();
+        bulk_copy_wait(src, bytes, total, my_q, qpitch, bar, phase);
         uint32_t pa[DIST_ILP], pb[DIST_ILP], va[DIST_ILP], vb[DIST_ILP], pb0[DIST_ILP];
 #pragma unroll
         for (int c = 0; c < DIST_ILP; c++) {
@@ -546,11 +520,8 @@ __global__ void __launch_bounds__(PAIR_WARPS_MAX * 32) dist_pair_kernel(const Di
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
     uint32_t *bufA = smem + (size_t)warp * 2 * row_pitch, *bufB = bufA + row_pitch;
     uint64_t *s_bar = reinterpret_cast<uint64_t *>(smem + (size_t)warps * 2 * row_pitch);
-    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(s_bar + warp);
+    const uint32_t bar = warp_bar_init(s_bar + warp);
     uint32_t phase = 0;
-    if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
     uint64_t total;
     if (a.pair_dense) total = (uint64_t)a.q_count * a.n_ref;
     else {
@@ -570,26 +541,14 @@ __global__ void __launch_bounds__(PAIR_WARPS_MAX * 32) dist_pair_kernel(const Di
             q = e.x; r = e.y;
         }
         const uint32_t nA = min(a.ref_n[r], a.S), nB = min(a.qry_n[q], a.S);
-        // stage both rows with one bulk copy each (16-byte aligned span around the first n elements), then the sentinels
-        const uintptr_t rowA = (uintptr_t)(a.ranks + (a.ref_row0 + r) * (uint64_t)a.P), rowB = (uintptr_t)(a.ranks + (a.qry_row0 + q) * (uint64_t)a.P);
-        const uintptr_t loA = rowA & ~(uintptr_t)15, loB = rowB & ~(uintptr_t)15;
-        const uint32_t bytesA = nA ? (uint32_t)(((rowA + (uintptr_t)nA * 4 + 15) & ~(uintptr_t)15) - loA) : 0;
-        const uint32_t bytesB = nB ? (uint32_t)(((rowB + (uintptr_t)nB * 4 + 15) & ~(uintptr_t)15) - loB) : 0;
-        uint32_t *sA = bufA + (rowA - loA) / 4, *sB = bufB + (rowB - loB) / 4;
-        __syncwarp();                                        // the previous pair's reads of the buffers are done
-        if (bytesA + bytesB) {
-            if (lane == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytesA + bytesB) : "memory");
-                if (bytesA) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                         :: "r"((uint32_t)__cvta_generic_to_shared(bufA)), "l"(loA), "r"(bytesA), "r"(bar) : "memory");
-                if (bytesB) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                         :: "r"((uint32_t)__cvta_generic_to_shared(bufB)), "l"(loB), "r"(bytesB), "r"(bar) : "memory");
-            }
-            asm volatile("{\n\t.reg .pred p;\n\tPAIR_BULK_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra PAIR_BULK_WAIT;\n\t}"
-                         :: "r"(bar), "r"(phase) : "memory");
-            phase ^= 1;
-        }
+        // stage both rows cut to their first n elements (bufB = bufA + row_pitch), then the sentinels
+        const uint32_t *src[2];
+        uint32_t skew[2];
+        const uint32_t spanA = bulk_span(a.ranks + (a.ref_row0 + r) * (uint64_t)a.P, nA, src[0], skew[0]);
+        const uint32_t spanB = bulk_span(a.ranks + (a.qry_row0 + q) * (uint64_t)a.P, nB, src[1], skew[1]);
+        const uint32_t bytes[2] = {nA ? spanA : 0u, nB ? spanB : 0u};
+        bulk_copy_wait(src, bytes, bytes[0] + bytes[1], bufA, row_pitch, bar, phase);
+        uint32_t *sA = bufA + skew[0] / 4, *sB = bufB + skew[1] / 4;
         if (lane == 0) { sA[nA] = RANK_PAD; sB[nB] = RANK_PAD; }
         __syncwarp();
         uint32_t i0 = 0, i1 = nA, j0 = 0, j1 = nB;          // the segment still to be resolved
@@ -797,14 +756,10 @@ struct mashgpu_dist_job {
     DevBuf<double> lut, binom_m;
     DevBuf<int> binom_e;
     bool tiled = true;
-    // pass-list target of the next run (set by mashgpu_dist_run_list only)
-    uint64_t *list_idx = nullptr; uint32_t *list_numer = nullptr, *list_denom = nullptr; double *list_distance = nullptr, *list_pvalue = nullptr;
-    unsigned long long *list_count = nullptr; uint64_t list_capacity = 0;
     // grow-only buffers of mashgpu_dist_run_list (no cudaMalloc per call after the first)
     DevBuf<uint64_t> l_idx, s_idx; DevBuf<uint32_t> l_n, l_d, l_order, s_order, o_n, o_d; DevBuf<double> l_D, l_P, o_D, o_P;
     DevBuf<unsigned long long> l_cnt; DevBuf<uint8_t> l_tmp;
-    // best hits (mashgpu_dist_run_best_dev): capture target of the next run, grow-only buffers, counters since the job was opened
-    BestCapture best{};
+    // best hits (mashgpu_dist_run_best_dev): grow-only buffers, counters since the job was opened
     uint64_t best_capacity = 0;         // mashgpu_dist_set_best_capacity; 0 = default
     DevBuf<BestCand> b_cand, b_grouped;
     DevBuf<uint32_t> b_q;               // per query of a block: hits, segment offset, scatter cursor
@@ -1233,17 +1188,13 @@ extern "C" int mashgpu_dist_pair_stats(mashgpu_dist_job *job, uint64_t *pairs_me
     return MASHGPU_OK;
 }
 
-extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count,
-                                    uint32_t *d_numer, uint32_t *d_denom, double *d_distance, double *d_pvalue, uint8_t *d_pass,
-                                    void *stream)
+namespace {
+
+// The arguments of a run of queries [q_begin, q_begin + q_count): the job's tables and rows, the range and the triangle.  Every
+// output field is NULL; the caller sets the run's target (dense outputs, pass list or best-hit capture) before dist_enqueue.
+DistArgs dist_args(const mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count)
 {
-    if (!job) return MASHGPU_ERR_INVALID;
-    mashgpu_ctx *ctx = job->ctx;
-    if (q_begin + q_count > job->n_qry) return fail(ctx, MASHGPU_ERR_INVALID, "query range [%llu, %llu) exceeds %llu", (unsigned long long)q_begin, (unsigned long long)(q_begin + q_count), (unsigned long long)job->n_qry);
-    if (q_count == 0 || job->n_ref == 0) return MASHGPU_OK;
-    MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
-    DistArgs a;
+    DistArgs a{};
     a.ranks = job->d_ranks; a.P = job->P; a.S = (uint32_t)job->params.sketch_size;
     a.ref_n = job->d_n_eff + job->ref_row0; a.ref_len = job->d_lens + job->ref_row0; a.ref_row0 = job->ref_row0;
     a.qry_n = job->d_n_eff + job->qry_row0; a.qry_len = job->d_lens + job->qry_row0; a.qry_row0 = job->qry_row0;
@@ -1252,14 +1203,17 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     a.max_distance = job->params.max_distance; a.max_pvalue = job->params.max_pvalue;
     a.dist_lut = job->lut.p;
     a.binom.mant = job->binom_m.p; a.binom.expo = job->binom_e.p; a.binom.n0 = job->params.sketch_size;
-    a.numer = d_numer; a.denom = d_denom; a.distance = d_distance; a.pvalue = d_pvalue; a.pass = d_pass;
-    a.list_idx = job->list_idx; a.list_numer = job->list_numer; a.list_denom = job->list_denom; a.list_distance = job->list_distance;
-    a.list_pvalue = job->list_pvalue; a.list_count = job->list_count; a.list_capacity = job->list_capacity;
-    a.qlist = nullptr; a.qcount = nullptr; a.qlist_stride = 0; a.flag_total = nullptr; a.use_qlist = 0; a.q_per_cta = 0;
     a.triangle = job->triangle ? 1 : 0;
     a.tri_r0 = job->self ? 0u : (uint32_t)job->ref_row0;
-    a.pair_list = nullptr; a.pair_count = nullptr; a.pair_full = nullptr; a.pair_capacity = 0; a.pair_total = nullptr; a.pair_max = 0; a.pair_dense = 0;
-    a.best = job->best;
+    return a;
+}
+
+// Enqueues a run on `st` (a.q_count >= 1, n_ref >= 1, the device current): the merge path for the job (prefilter and pair list,
+// dense tiles, warp per pair or one thread per pair), the p-value pass, the launch counters and the prefilter's flag snapshot.
+int dist_enqueue(mashgpu_dist_job *job, DistArgs a, cudaStream_t st)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    const uint64_t q_count = a.q_count;
     {   // queue for the deferred p-values: 1/16 of the pairs (at least 2^20); beyond that dist_emit evaluates in place
         const uint64_t pairs = q_count * job->n_ref;
         const uint64_t cap = std::min<uint64_t>(pairs, std::max<uint64_t>(1ull << 20, pairs / 16));
@@ -1308,7 +1262,6 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     const uint32_t r_tiles = (uint32_t)((job->n_ref + DIST_TILE_R - 1) / DIST_TILE_R);
     const uint32_t round = DIST_WARPS * DIST_ILP;
     const size_t smem = dist_smem_bytes(a.P);
-    a.qlist = nullptr; a.qcount = nullptr; a.qlist_stride = 0; a.flag_total = nullptr; a.use_qlist = 0;
     dist_collect_flags(job);
     const bool prefilter = job->prefilter_mode > 0 || (job->prefilter_mode < 0 && !job->auto_off);
     if (prefilter) {
@@ -1369,13 +1322,7 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
         ctx->dist_launches += 2;
         return MASHGPU_OK;
     }
-    // slice the query range so that about 2 waves of CTAs cover the machine, at least one full round of warps each
-    uint32_t want_slices = std::max(1u, (uint32_t)(2 * ctx->sm_count + r_tiles - 1) / r_tiles);
-    uint32_t q_per_cta = (uint32_t)((q_count + want_slices - 1) / want_slices);
-    q_per_cta = std::max(round, ((q_per_cta + round - 1) / round) * round);
-    const uint32_t slices = (uint32_t)((q_count + q_per_cta - 1) / q_per_cta);
-    a.q_per_cta = q_per_cta;
-    dim3 grid(r_tiles, slices);
+    const dim3 grid = dense_grid(r_tiles, q_count, ctx->sm_count, a.q_per_cta);
     time_begin(ctx, ctx->dist_events, st);
     dist_kernel<<<grid, DIST_THREADS, smem, st>>>(a);
     MG_CUDA(ctx, cudaGetLastError());
@@ -1386,6 +1333,22 @@ extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uin
     return MASHGPU_OK;
 }
 
+}  // namespace
+
+extern "C" int mashgpu_dist_run_dev(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count,
+                                    uint32_t *d_numer, uint32_t *d_denom, double *d_distance, double *d_pvalue, uint8_t *d_pass,
+                                    void *stream)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (q_begin + q_count > job->n_qry) return fail(ctx, MASHGPU_ERR_INVALID, "query range [%llu, %llu) exceeds %llu", (unsigned long long)q_begin, (unsigned long long)(q_begin + q_count), (unsigned long long)job->n_qry);
+    if (q_count == 0 || job->n_ref == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    DistArgs a = dist_args(job, q_begin, q_count);
+    a.numer = d_numer; a.denom = d_denom; a.distance = d_distance; a.pvalue = d_pvalue; a.pass = d_pass;
+    return dist_enqueue(job, a, stream ? (cudaStream_t)stream : ctx->stream);
+}
+
 extern "C" int mashgpu_dist_run(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count,
                                 uint32_t *numer, uint32_t *denom, double *distance, double *pvalue, uint8_t *pass)
 {
@@ -1394,38 +1357,14 @@ extern "C" int mashgpu_dist_run(mashgpu_dist_job *job, uint64_t q_begin, uint64_
     if (q_begin + q_count > job->n_qry) return fail(ctx, MASHGPU_ERR_INVALID, "query range exceeds query count");
     if (q_count == 0 || job->n_ref == 0) return MASHGPU_OK;
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    // bound the device output tile: chunks of queries
+    // bound the device outputs: chunks of queries, 128 Mi pairs (~3.2 GB of outputs) per launch
     const uint64_t n_ref = job->n_ref;
-    const uint64_t max_pairs = 1ull << 27;     // 128 Mi pairs (~3.2 GB of outputs) per launch
-    uint64_t q_chunk = std::max<uint64_t>(1, max_pairs / n_ref);
-    q_chunk = std::min(q_chunk, q_count);
-    const uint64_t pairs = q_chunk * n_ref;
-    DevBuf<uint32_t> dn, dd; DevBuf<double> dD, dP; DevBuf<uint8_t> dpass;
-    if ((numer && dn.alloc(pairs) != cudaSuccess) || (denom && dd.alloc(pairs) != cudaSuccess) || (distance && dD.alloc(pairs) != cudaSuccess) ||
-        (pvalue && dP.alloc(pairs) != cudaSuccess) || (pass && dpass.alloc(pairs) != cudaSuccess))
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pair outputs)");
-    cudaStream_t st = ctx->stream;
-    for (uint64_t q = 0; q < q_count; q += q_chunk) {
-        const uint64_t qc = std::min(q_chunk, q_count - q);
-        if (job->triangle) {        // pairs on or above the diagonal are not written by the kernels: hand zeros back for them
-            const uint64_t np0 = qc * n_ref;
-            if (numer) MG_CUDA(ctx, cudaMemsetAsync(dn.p, 0, np0 * 4, st));
-            if (denom) MG_CUDA(ctx, cudaMemsetAsync(dd.p, 0, np0 * 4, st));
-            if (distance) MG_CUDA(ctx, cudaMemsetAsync(dD.p, 0, np0 * 8, st));
-            if (pvalue) MG_CUDA(ctx, cudaMemsetAsync(dP.p, 0, np0 * 8, st));
-            if (pass) MG_CUDA(ctx, cudaMemsetAsync(dpass.p, 0, np0, st));
-        }
-        MG_TRY(mashgpu_dist_run_dev(job, q_begin + q, qc, numer ? dn.p : nullptr, denom ? dd.p : nullptr, distance ? dD.p : nullptr,
-                                    pvalue ? dP.p : nullptr, pass ? dpass.p : nullptr, st));
-        const uint64_t np = qc * n_ref, o = q * n_ref;
-        if (numer) MG_CUDA(ctx, cudaMemcpyAsync(numer + o, dn.p, np * 4, cudaMemcpyDeviceToHost, st));
-        if (denom) MG_CUDA(ctx, cudaMemcpyAsync(denom + o, dd.p, np * 4, cudaMemcpyDeviceToHost, st));
-        if (distance) MG_CUDA(ctx, cudaMemcpyAsync(distance + o, dD.p, np * 8, cudaMemcpyDeviceToHost, st));
-        if (pvalue) MG_CUDA(ctx, cudaMemcpyAsync(pvalue + o, dP.p, np * 8, cudaMemcpyDeviceToHost, st));
-        if (pass) MG_CUDA(ctx, cudaMemcpyAsync(pass + o, dpass.p, np, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    return MASHGPU_OK;
+    const uint64_t q_chunk = std::min(q_count, std::max<uint64_t>(1, (1ull << 27) / n_ref));
+    const HostOut out[] = {{numer, 4 * n_ref}, {denom, 4 * n_ref}, {distance, 8 * n_ref}, {pvalue, 8 * n_ref}, {pass, n_ref}};
+    // pairs on or above the diagonal of a triangle run are not written by the kernels: hand zeros back for them
+    return run_host_chunks(ctx, out, q_count, q_chunk, job->triangle, "pair outputs", [&](uint64_t q, uint64_t qc, void *const *d) {
+        return mashgpu_dist_run_dev(job, q_begin + q, qc, (uint32_t *)d[0], (uint32_t *)d[1], (double *)d[2], (double *)d[3], (uint8_t *)d[4], ctx->stream);
+    });
 }
 
 extern "C" int mashgpu_dist_run_list(mashgpu_dist_job *job, uint64_t q_begin, uint64_t q_count, uint64_t capacity,
@@ -1449,11 +1388,10 @@ extern "C" int mashgpu_dist_run_list(mashgpu_dist_job *job, uint64_t q_begin, ui
         J.l_cnt.reserve(1) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pass list of %llu entries)", (unsigned long long)cap);
     MG_CUDA(ctx, cudaMemsetAsync(J.l_cnt.p, 0, 8, st));
-    job->list_idx = J.l_idx.p; job->list_numer = J.l_n.p; job->list_denom = J.l_d.p; job->list_distance = J.l_D.p; job->list_pvalue = J.l_P.p;
-    job->list_count = J.l_cnt.p; job->list_capacity = capacity;
-    int rc = mashgpu_dist_run_dev(job, q_begin, q_count, nullptr, nullptr, nullptr, nullptr, nullptr, st);
-    job->list_idx = nullptr; job->list_numer = job->list_denom = nullptr; job->list_distance = job->list_pvalue = nullptr; job->list_count = nullptr; job->list_capacity = 0;
-    MG_TRY(rc);
+    DistArgs a = dist_args(job, q_begin, q_count);
+    a.list_idx = J.l_idx.p; a.list_numer = J.l_n.p; a.list_denom = J.l_d.p; a.list_distance = J.l_D.p; a.list_pvalue = J.l_P.p;
+    a.list_count = J.l_cnt.p; a.list_capacity = capacity;
+    MG_TRY(dist_enqueue(job, a, st));
     unsigned long long n = 0;
     MG_CUDA(ctx, cudaMemcpyAsync(&n, J.l_cnt.p, 8, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
@@ -1553,10 +1491,9 @@ extern "C" int mashgpu_dist_run_best_dev(mashgpu_dist_job *job, uint64_t q_begin
         uint32_t *qcnt = J.b_q.p, *qoff = qcnt + bn, *cursor = qoff + bn;
         MG_CUDA(ctx, cudaMemsetAsync(J.b_cnt.p, 0, 8, st));
         MG_CUDA(ctx, cudaMemsetAsync(qcnt, 0, 3 * bn * 4, st));
-        job->best = BestCapture{J.b_cand.p, J.b_cnt.p, cap, qcnt};
-        const int rc = mashgpu_dist_run_dev(job, q_begin + b0, bn, nullptr, nullptr, nullptr, nullptr, nullptr, st);
-        job->best = BestCapture{};
-        MG_TRY(rc);
+        DistArgs a = dist_args(job, q_begin + b0, bn);
+        a.best = BestCapture{J.b_cand.p, J.b_cnt.p, cap, qcnt};
+        MG_TRY(dist_enqueue(job, a, st));
         unsigned long long n = 0;
         MG_CUDA(ctx, cudaMemcpyAsync(&n, J.b_cnt.p, 8, cudaMemcpyDeviceToHost, st));
         MG_CUDA(ctx, cudaStreamSynchronize(st));
@@ -1595,27 +1532,14 @@ extern "C" int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, ui
     if (q_count == 0) return MASHGPU_OK;
     if (!n_hits || !ref || !numer || !denom || !distance || !pvalue) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
     // bound the device outputs: chunks of queries (each is cut into blocks by the device call)
     const uint64_t q_chunk = std::min<uint64_t>(q_count, std::max<uint64_t>(1, BEST_HOST_ENTRIES / n_best));
-    const uint64_t e_chunk = q_chunk * n_best;
-    DevBuf<uint32_t> dh, dt, dr, dn, dd; DevBuf<double> dD, dP;
-    if (dh.alloc(q_chunk) != cudaSuccess || dt.alloc(q_chunk) != cudaSuccess || dr.alloc(e_chunk) != cudaSuccess || dn.alloc(e_chunk) != cudaSuccess ||
-        dd.alloc(e_chunk) != cudaSuccess || dD.alloc(e_chunk) != cudaSuccess || dP.alloc(e_chunk) != cudaSuccess)
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (best-hit outputs)");
-    for (uint64_t q = 0; q < q_count; q += q_chunk) {
-        const uint64_t qc = std::min(q_chunk, q_count - q), e = qc * n_best, o = q * n_best;
-        MG_TRY(mashgpu_dist_run_best_dev(job, q_begin + q, qc, n_best, dh.p, dt.p, dr.p, dn.p, dd.p, dD.p, dP.p, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(n_hits + q, dh.p, qc * 4, cudaMemcpyDeviceToHost, st));
-        if (n_total) MG_CUDA(ctx, cudaMemcpyAsync(n_total + q, dt.p, qc * 4, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(ref + o, dr.p, e * 4, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(numer + o, dn.p, e * 4, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(denom + o, dd.p, e * 4, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(distance + o, dD.p, e * 8, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaMemcpyAsync(pvalue + o, dP.p, e * 8, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    return MASHGPU_OK;
+    const uint64_t e4 = 4ull * n_best, e8 = 8ull * n_best;
+    const HostOut out[] = {{n_hits, 4}, {n_total, 4}, {ref, e4}, {numer, e4}, {denom, e4}, {distance, e8}, {pvalue, e8}};
+    return run_host_chunks(ctx, out, q_count, q_chunk, false, "best-hit outputs", [&](uint64_t q, uint64_t qc, void *const *d) {
+        return mashgpu_dist_run_best_dev(job, q_begin + q, qc, n_best, (uint32_t *)d[0], (uint32_t *)d[1], (uint32_t *)d[2], (uint32_t *)d[3],
+                                         (uint32_t *)d[4], (double *)d[5], (double *)d[6], ctx->stream);
+    });
 }
 
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)

@@ -52,7 +52,7 @@ __device__ __forceinline__ void within_emit(const WithinArgs &a, uint32_t q, uin
     if (a.pass) a.pass[o] = error <= a.max_error ? 1 : 0;
 }
 
-// Tiled lockstep kernel.  The reference tile and the query staging are dist_kernel's (dist.cu); the step is the reference's loop
+// Tiled lockstep kernel.  The reference tile and the query staging are dist_kernel's (dict.cuh); the step is the reference's loop
 // with its two stop conditions as per-lane predicates: a lane whose pair has stopped keeps issuing the step with everything
 // predicated off until the whole warp is done (a vote every 8 steps).  A lane stops at the end of R (i == |R|, its pointer reaches
 // the tile slot after its last rank) or once j reaches denom.
@@ -69,20 +69,14 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) within_kernel(const WithinArg
     const bool r_ok = r < a.n_ref;
     if ((uint64_t)blockIdx.y * a.q_per_cta >= a.q_count) return;
 
-    {   // element i of reference (r0+l) at s_ref[i*32 + l]
-        const uint32_t *row = a.ranks + (a.ref_row0 + (r_ok ? r : r0)) * (uint64_t)a.P;
-        for (uint32_t i = warp; i < a.P; i += DIST_WARPS) s_ref[i * DIST_TILE_R + lane] = r_ok ? row[i] : RANK_PAD;
-    }
+    stage_ref_tile(s_ref, a.ranks, a.ref_row0, a.P, r0, a.n_ref);
     __syncthreads();
     const uint32_t nR = r_ok ? a.ref_n[r] : 0;
     const uint32_t sref_base = (uint32_t)__cvta_generic_to_shared(s_ref) + lane * 4;
     const uint32_t sref_end = sref_base + nR * (DIST_TILE_R * 4);
     uint32_t *my_q = s_qry + (size_t)warp * DIST_ILP * qpitch;
-    const uint32_t bar = (uint32_t)__cvta_generic_to_shared(s_bar + warp);
+    const uint32_t bar = warp_bar_init(s_bar + warp);
     uint32_t phase = 0;
-    if (lane == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
 
     const uint32_t q_lo = a.q_begin + blockIdx.y * a.q_per_cta;
     const uint32_t q_hi = (uint32_t)min((uint64_t)a.q_begin + a.q_count, (uint64_t)q_lo + a.q_per_cta);
@@ -93,28 +87,12 @@ __global__ void __launch_bounds__(DIST_THREADS, 1) within_kernel(const WithinArg
         for (int c = 0; c < DIST_ILP; c++) {
             skew[c] = 0; bytes[c] = 0; src[c] = nullptr;
             if (qb + c < q_hi) {
-                const uintptr_t row = (uintptr_t)(a.ranks + (a.qry_row0 + qb + c) * (uint64_t)a.P);
-                const uintptr_t lo = row & ~(uintptr_t)15, hi = (row + (uintptr_t)a.P * 4 + 15) & ~(uintptr_t)15;
-                skew[c] = (uint32_t)(row - lo);
-                src[c] = reinterpret_cast<const uint32_t *>(lo);
-                bytes[c] = (uint32_t)(hi - lo);
+                bytes[c] = bulk_span(a.ranks + (a.qry_row0 + qb + c) * (uint64_t)a.P, a.P, src[c], skew[c]);
                 total += bytes[c];
             }
         }
-        __syncwarp();
-        if (lane == 0) {
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // the lanes' reads of the previous rows precede the async writes
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(total) : "memory");
-#pragma unroll
-            for (int c = 0; c < DIST_ILP; c++)
-                if (bytes[c])
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 :: "r"((uint32_t)__cvta_generic_to_shared(my_q + (size_t)c * qpitch)), "l"(src[c]), "r"(bytes[c]), "r"(bar) : "memory");
-        }
-        asm volatile("{\n\t.reg .pred p;\n\tWITHIN_BULK_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra WITHIN_BULK_WAIT;\n\t}"
-                     :: "r"(bar), "r"(phase) : "memory");
-        phase ^= 1;
-        __syncwarp();
+        __builtin_assume(total != 0);          // slot 0 holds query qb < q_hi
+        bulk_copy_wait(src, bytes, total, my_q, qpitch, bar, phase);
         uint32_t pa[DIST_ILP], pb[DIST_ILP], pb0[DIST_ILP], pb_end[DIST_ILP], va[DIST_ILP], vb[DIST_ILP], common[DIST_ILP];
 #pragma unroll
         for (int c = 0; c < DIST_ILP; c++) {
@@ -296,21 +274,15 @@ extern "C" int mashgpu_within_run_dev(mashgpu_within_job *job, uint64_t q_begin,
     if (q_count == 0 || job->n_ref == 0) return MASHGPU_OK;
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
-    WithinArgs a;
+    WithinArgs a{};
     a.ranks = job->ranks.p; a.P = job->P;
     a.ref_n = job->n_eff.p; a.qry_n = job->n_eff.p + job->qry_row0; a.ref_row0 = 0; a.qry_row0 = job->qry_row0;
-    a.n_ref = (uint32_t)job->n_ref; a.q_begin = (uint32_t)q_begin; a.q_count = (uint32_t)q_count; a.q_per_cta = 0;
+    a.n_ref = (uint32_t)job->n_ref; a.q_begin = (uint32_t)q_begin; a.q_count = (uint32_t)q_count;
     a.max_error = job->max_error;
     a.common = d_common; a.examined = d_examined; a.score = d_score; a.error = d_error; a.pass = d_pass;
     time_begin(ctx, ctx->dist_events, st);
     if (job->tiled) {
-        // slice the query range so that about 2 waves of CTAs cover the machine, at least one full round of warps each
-        const uint32_t r_tiles = (uint32_t)((job->n_ref + DIST_TILE_R - 1) / DIST_TILE_R), round = DIST_WARPS * DIST_ILP;
-        const uint32_t want_slices = std::max(1u, (uint32_t)(2 * ctx->sm_count + r_tiles - 1) / r_tiles);
-        uint32_t q_per_cta = (uint32_t)((q_count + want_slices - 1) / want_slices);
-        q_per_cta = std::max(round, ((q_per_cta + round - 1) / round) * round);
-        a.q_per_cta = q_per_cta;
-        const dim3 grid(r_tiles, (uint32_t)((q_count + q_per_cta - 1) / q_per_cta));
+        const dim3 grid = dense_grid((uint32_t)((job->n_ref + DIST_TILE_R - 1) / DIST_TILE_R), q_count, ctx->sm_count, a.q_per_cta);
         within_kernel<<<grid, DIST_THREADS, dist_smem_bytes(a.P), st>>>(a);
     } else {
         within_pair_kernel<<<ctx->sm_count * 8, WPAIR_WARPS * 32, 0, st>>>(a);
@@ -333,24 +305,11 @@ extern "C" int mashgpu_within_run(mashgpu_within_job *job, uint64_t q_begin, uin
     // bound the device outputs: chunks of queries
     const uint64_t n_ref = job->n_ref;
     const uint64_t q_chunk = std::min(q_count, std::max<uint64_t>(1, WITHIN_CHUNK_PAIRS / n_ref));
-    const uint64_t pairs = q_chunk * n_ref;
-    DevBuf<uint32_t> dc, dx; DevBuf<double> ds, de; DevBuf<uint8_t> dp;
-    if ((common && dc.alloc(pairs) != cudaSuccess) || (examined && dx.alloc(pairs) != cudaSuccess) || (score && ds.alloc(pairs) != cudaSuccess) ||
-        (error && de.alloc(pairs) != cudaSuccess) || (pass && dp.alloc(pairs) != cudaSuccess))
-        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (pair outputs)");
-    cudaStream_t st = ctx->stream;
-    for (uint64_t q = 0; q < q_count; q += q_chunk) {
-        const uint64_t qc = std::min(q_chunk, q_count - q), np = qc * n_ref, o = q * n_ref;
-        MG_TRY(mashgpu_within_run_dev(job, q_begin + q, qc, common ? dc.p : nullptr, examined ? dx.p : nullptr, score ? ds.p : nullptr,
-                                      error ? de.p : nullptr, pass ? dp.p : nullptr, st));
-        if (common) MG_CUDA(ctx, cudaMemcpyAsync(common + o, dc.p, np * 4, cudaMemcpyDeviceToHost, st));
-        if (examined) MG_CUDA(ctx, cudaMemcpyAsync(examined + o, dx.p, np * 4, cudaMemcpyDeviceToHost, st));
-        if (score) MG_CUDA(ctx, cudaMemcpyAsync(score + o, ds.p, np * 8, cudaMemcpyDeviceToHost, st));
-        if (error) MG_CUDA(ctx, cudaMemcpyAsync(error + o, de.p, np * 8, cudaMemcpyDeviceToHost, st));
-        if (pass) MG_CUDA(ctx, cudaMemcpyAsync(pass + o, dp.p, np, cudaMemcpyDeviceToHost, st));
-        MG_CUDA(ctx, cudaStreamSynchronize(st));
-    }
-    return MASHGPU_OK;
+    const HostOut out[] = {{common, 4 * n_ref}, {examined, 4 * n_ref}, {score, 8 * n_ref}, {error, 8 * n_ref}, {pass, n_ref}};
+    return run_host_chunks(ctx, out, q_count, q_chunk, false, "pair outputs", [&](uint64_t q, uint64_t qc, void *const *d) {
+        return mashgpu_within_run_dev(job, q_begin + q, qc, (uint32_t *)d[0], (uint32_t *)d[1], (double *)d[2], (double *)d[3], (uint8_t *)d[4],
+                                      ctx->stream);
+    });
 }
 
 extern "C" int mashgpu_within_close(mashgpu_within_job *job)

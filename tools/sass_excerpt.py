@@ -20,6 +20,8 @@ KERNELS = {
     "dist_kernel": "_ZN7mashgpu11dist_kernelENS_8DistArgsE",
     "dist_probe_kernel": "_ZN7mashgpu17dist_probe_kernelENS_8DistArgsE",
     "dist_pair_kernel": "_ZN7mashgpu16dist_pair_kernelENS_8DistArgs",
+    "within_kernel": "_ZN7mashgpu13within_kernelENS_10WithinArgsE",
+    "within_pair_kernel": "_ZN7mashgpu18within_pair_kernelENS_10WithinArgsE",
 }
 PIPES = {
     "ALU (SHF/LOP3/IADD3/PRMT/ISETP/SEL/...)": ("SHF", "LOP3", "IADD3", "IADD", "PRMT", "ISETP", "SEL", "LEA", "MOV", "PLOP3", "HSETP2", "VOTE", "POPC", "FLO", "BREV", "IABS", "IMNMX", "VIMNMX", "LOP"),
