@@ -305,6 +305,19 @@ int mashgpu_dist_set_best_capacity(mashgpu_dist_job *job, uint64_t entries);
  * mashgpu_set_timing is on, the device time of grouping and selection.  Any pointer may be NULL. */
 int mashgpu_dist_best_stats(mashgpu_dist_job *job, uint64_t *blocks_run, uint64_t *blocks_split, uint64_t *candidates, double *select_ms);
 
+/* Connected components of the passing pairs that share a hash (DESIGN.md 3.8); no counterpart in the reference.
+ * Self jobs (qry == NULL) and encoded jobs only; the pairs are enumerated in the lower triangle whatever
+ * mashgpu_dist_set_triangle says.  labels[i] = smallest index of sketch i's component, n_qry entries.
+ * The component graph has one vertex per query row and an edge {q, r'} for every pair (q, r) of the lower triangle with
+ * pass == 1 in mashgpu_dist_run and numer > 0 (the hit rule of mashgpu_dist_run_best: max_distance and max_pvalue apply, two
+ * empty sketches are not joined), where r' = r for a self job and ref_begin + r for an encoded one.  So an encoded job over a
+ * shard of the reference axis yields the components of that shard's edges over all n_rows sketches; the union of the shards'
+ * graphs is the whole graph (shard.merge_component_labels).  *n_edges = number of edges, every unordered pair once.  The labels
+ * do not depend on the order in which the pairs were evaluated.  A job with a separate query set and NULL outputs are
+ * MASHGPU_ERR_INVALID.  Synchronises the stream (the edge count is read on the host). */
+int mashgpu_dist_components(mashgpu_dist_job *job, uint32_t *labels, uint64_t *n_edges);
+int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_labels, uint64_t *n_edges, void *stream);
+
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE
  * instead (a sample sort): a rank sorts only its own rows' hashes, the sorted keys are cut at G-1 splitters, every rank

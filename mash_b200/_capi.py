@@ -123,6 +123,8 @@ def load_library():
                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.mashgpu_dist_set_best_capacity.argtypes = [C.c_void_p, C.c_uint64]
     L.mashgpu_dist_best_stats.argtypes = [C.c_void_p, u64p, u64p, u64p, f64p]
+    L.mashgpu_dist_components.argtypes = [C.c_void_p, u32p, u64p]
+    L.mashgpu_dist_components_dev.argtypes = [C.c_void_p, C.c_void_p, u64p, C.c_void_p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
     L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
@@ -472,6 +474,20 @@ class DistJob:
         blocks = C.c_uint64(0); splits = C.c_uint64(0); cands = C.c_uint64(0); ms = C.c_double(0)
         self.eng._check(self.eng.lib.mashgpu_dist_best_stats(self.h, C.byref(blocks), C.byref(splits), C.byref(cands), C.byref(ms)))
         return {"blocks_run": blocks.value, "blocks_split": splits.value, "candidates": cands.value, "select_ms": ms.value}
+
+    def components(self):
+        """Connected components of the hits (pass and numer > 0) of the lower triangle: (labels, n_edges), labels[i] = smallest
+        query row of row i's component (np.uint32, n_qry entries).  Self and encoded jobs only."""
+        labels = np.zeros(self.n_qry, np.uint32)
+        n = C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_components(self.h, _p(labels, u32p), C.byref(n)))
+        return labels, n.value
+
+    def components_dev(self, d_labels, stream=None):
+        """components() into a device array of n_qry uint32; returns n_edges."""
+        n = C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_components_dev(self.h, d_labels, C.byref(n), stream))
+        return n.value
 
     def set_prefilter(self, mode):
         """-1 = auto (default), 0 = merge every pair, 1 = always probe the reference tiles first."""

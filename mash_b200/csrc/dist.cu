@@ -20,6 +20,8 @@
 // Results are identical with and without the prefilter (tests/test_gpu_dist_prefilter.py).
 // A best run (mashgpu_dist_run_best, DESIGN.md 3.7) runs the same kernels with no dense output: the two places that know a pair's
 // final pass flag, dist_emit and dist_fix_kernel, capture the hits, and dist_best.cuh selects the N nearest of every query.
+// A component run (mashgpu_dist_components, DESIGN.md 3.8) is the same again: at those two places dist_cc.cuh unions the two sketches
+// of every hit of the lower triangle into a forest, whose roots become the components' labels.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -34,6 +36,7 @@
 #include "dict.cuh"
 #include "dist_filter.cuh"
 #include "dist_best.cuh"
+#include "dist_cc.cuh"
 
 namespace mashgpu {
 
@@ -74,6 +77,7 @@ struct DistArgs {
     // deferred p-values (dist_fix_kernel): pairs with shared hashes whose binomial tail is evaluated in a dense second pass
     struct FixEntry *fix_list; unsigned long long *fix_count; uint64_t fix_capacity;
     BestCapture best;           // best runs: hits (pass, common > 0) are captured here; every dense output and the pass list are NULL then
+    CcCapture cc;               // component runs: hits are unioned here (the sketches q and tri_r0 + r); NULL outputs and pass list, as for best
 };
 
 struct FixEntry { uint64_t o; uint32_t common, denom; };
@@ -131,6 +135,7 @@ __device__ __forceinline__ void dist_emit(const DistArgs &a, uint32_t q, uint32_
     if (deferred) return;
     if (a.list_idx && pass) dist_list_append(a, o, common, denom, dist, p);
     if (a.best.cand && pass && common) dist_best_append(a.best, q - a.q_begin, r, common, denom, dist, p);
+    if (a.cc.parent && pass && common) dist_cc_union(a.cc, q, a.tri_r0 + r);
     if (a.pvalue) a.pvalue[o] = p;
     if (a.pass) a.pass[o] = pass ? 1 : 0;
 }
@@ -150,6 +155,7 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
             if (a.list_idx) dist_list_append(a, e.o, e.common, e.denom, dist, p);
             else dist_best_append(a.best, q - a.q_begin, r, e.common, e.denom, dist, p);      // queued pairs share a hash
         }
+        if (a.cc.parent && pass) dist_cc_union(a.cc, q, a.tri_r0 + r);
         if (a.pvalue) a.pvalue[e.o] = p;
         if (a.pass) a.pass[e.o] = pass ? 1 : 0;
     }
@@ -464,8 +470,8 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
         } else if (mine && !((mask >> lane) & 1u)) {
             // empty intersection: the merge would take min(s', |A| + |B|) union steps and count nothing
             const uint32_t denom = min(a.S, nA + nB_all);
-            if (a.best.cand) {
-                // best run: a pair without a shared hash is not a hit, whatever its denominator
+            if (a.best.cand || a.cc.parent) {
+                // best or component run: a pair without a shared hash is not a hit, whatever its denominator
             } else if (denom == a.S && a.list_idx && pass_const == 0) {
                 // filtered run (-d / -v) and distance 1 / p-value 1 does not pass: nothing to write for this pair
             } else if (denom == a.S && !a.list_idx) {
@@ -746,6 +752,7 @@ struct mashgpu_dist_job {
     mashgpu_dist_params params{};
     uint64_t n_ref = 0, n_qry = 0;
     bool self = false;
+    bool encoded = false;               // mashgpu_dist_open_encoded: queries are all rows, references a contiguous range of them
     uint32_t P = 0;
     // rank rows: views used by the kernels (into the buffers below, or the caller's arrays for mashgpu_dist_open_encoded)
     const uint32_t *d_ranks = nullptr, *d_n_eff = nullptr;
@@ -768,6 +775,7 @@ struct mashgpu_dist_job {
     uint64_t best_blocks = 0, best_splits = 0, best_candidates = 0;
     double best_select_ms = 0;
     std::vector<EventPair> best_events;
+    DevBuf<unsigned long long> cc_edges;        // edge counter of mashgpu_dist_components_dev
     // prefilter (dist_probe_kernel): -1 = auto (on; switched off when most combinations turn out to share hashes), 0 = off, 1 = on
     int prefilter_mode = -1;
     bool triangle = false;
@@ -1002,7 +1010,7 @@ extern "C" int mashgpu_dist_open_encoded(mashgpu_ctx *ctx, const uint32_t *d_row
     MG_TRY(check_dist_params(ctx, params));
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     std::unique_ptr<mashgpu_dist_job> job(new mashgpu_dist_job());
-    job->ctx = ctx; job->params = *params; job->self = false;
+    job->ctx = ctx; job->params = *params; job->self = false; job->encoded = true;
     job->n_ref = ref_count; job->n_qry = n_rows;
     job->P = (uint32_t)params->sketch_size + 1;
     job->d_ranks = d_rows; job->d_n_eff = d_n_eff; job->d_lens = d_length;
@@ -1540,6 +1548,64 @@ extern "C" int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, ui
         return mashgpu_dist_run_best_dev(job, q_begin + q, qc, n_best, (uint32_t *)d[0], (uint32_t *)d[1], (uint32_t *)d[2], (uint32_t *)d[3],
                                          (uint32_t *)d[4], (double *)d[5], (double *)d[6], ctx->stream);
     });
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Connected components (DESIGN.md 3.8)
+// ---------------------------------------------------------------------------------------------------------
+constexpr uint64_t CC_BLOCK_PAIRS = 1ull << 31;     // pairs of one run: bounds the work lists, the pair list and the p-value queue
+
+extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_labels, uint64_t *n_edges, void *stream)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "components need a self comparison (qry == NULL) or an encoded job");
+    if (!d_labels || !n_edges) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_edges = 0;
+    const uint64_t n = job->n_qry, n_ref = job->n_ref;
+    if (n == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    if (job->cc_edges.reserve(1) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (edge counter)");
+    MG_CUDA(ctx, cudaMemsetAsync(job->cc_edges.p, 0, 8, st));
+    cc_init_kernel<<<blocks_for(n), 256, 0, st>>>(d_labels, n);
+    MG_CUDA(ctx, cudaGetLastError());
+    // The labels are the forest.  Lower triangle whatever the job's own setting: query q meets the rows below it only, so the
+    // queries up to the first reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
+    const uint64_t q_first = job->self ? 1 : job->ref_row0 + 1;
+    const uint64_t block = std::max<uint64_t>(1, CC_BLOCK_PAIRS / std::max<uint64_t>(n_ref, 1));
+    for (uint64_t q0 = q_first; n_ref && q0 < n; q0 += block) {
+        DistArgs a = dist_args(job, q0, std::min(block, n - q0));
+        a.triangle = 1;
+        a.cc = CcCapture{d_labels, job->cc_edges.p};
+        MG_TRY(dist_enqueue(job, a, st));
+    }
+    cc_flatten_kernel<<<blocks_for(n), 256, 0, st>>>(d_labels, n);
+    MG_CUDA(ctx, cudaGetLastError());
+    ctx->kernel_launches += 2;
+    unsigned long long e = 0;
+    MG_CUDA(ctx, cudaMemcpyAsync(&e, job->cc_edges.p, 8, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    *n_edges = e;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_components(mashgpu_dist_job *job, uint32_t *labels, uint64_t *n_edges)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "components need a self comparison (qry == NULL) or an encoded job");
+    if (!labels || !n_edges) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_edges = 0;
+    const uint64_t n = job->n_qry;
+    if (n == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    DevBuf<uint32_t> d;
+    if (d.alloc(n) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu labels)", (unsigned long long)n);
+    MG_TRY(mashgpu_dist_components_dev(job, d.p, n_edges, ctx->stream));
+    MG_CUDA(ctx, cudaMemcpyAsync(labels, d.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return MASHGPU_OK;
 }
 
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)

@@ -501,6 +501,23 @@ int runWithin(int argc, const char **argv)   // reference CommandContain.cpp:33-
 }
 
 // ---------------------------------------------------------------------------------------------------- triangle
+// `mash triangle -G`: one line per sketch in input order, its name (comment with -C) and its cluster.  The clusters are the connected
+// components of the pairs that pass -d / -v and share a hash, built on the device; they are numbered from 0 in the order of their
+// first member, which is the smallest index of the component, the label the engine returns.
+static void writeClusters(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int threads)
+{
+    const uint64_t n = sketch.getReferenceCount();
+    vector<uint32_t> label(n), cluster(n);
+    uint64_t edges = 0, clusters = 0;
+    if (n && mashgpu_dist_components(job, label.data(), &edges) != MASHGPU_OK) gpuFail();
+    for (uint64_t i = 0; i < n; i++) cluster[i] = label[i] == i ? (uint32_t)clusters++ : cluster[label[i]];
+    mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
+        const Sketch::Reference &ref = sketch.getReference(i);
+        o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.u64(cluster[i]); o.ch('\n');
+    });
+    cerr << "Clusters: " << clusters << " from " << edges << " edges" << endl;
+}
+
 int runTriangle(int argc, const char **argv)
 {
     Command c;
@@ -508,14 +525,20 @@ int runTriangle(int argc, const char **argv)
     c.add("list", Option(Option::Boolean, "l", ""));
     c.add("comment", Option(Option::Boolean, "C", ""));
     c.add("edge", Option(Option::Boolean, "E", ""));
+    c.add("cluster", Option(Option::Boolean, "G", ""));       // not an option of the reference: its users cluster the -E output
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.useSketchOptions();
     if (c.parse(argc, argv)) return 1;
-    if (c.arguments.size() < 1 || c.opt("help").active) { cerr << "usage: mash triangle [options] <seq1> [<seq2>] ..." << endl; return 0; }
-    bool comment = c.opt("comment").active, edge = c.opt("edge").active;
+    if (c.arguments.size() < 1 || c.opt("help").active) {
+        cerr << "usage: mash triangle [options] <seq1> [<seq2>] ..." << endl
+             << "  -G        Clusters: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash (not with -E)." << endl;
+        return 0;
+    }
+    bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active;
+    if (cluster && edge) { cerr << "ERROR: The option -G cannot be used with -E (clusters replace the edge list)." << endl; return 1; }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
-    if (c.opt("pvalue").active || c.opt("distance").active) edge = true;
+    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster) edge = true;
     Sketch::Parameters parameters;
     if (sketchParameterSetup(parameters, c)) return 1;
     if (c.arguments.size() == 1 && !c.opt("list").active) parameters.concatenated = false;
@@ -526,6 +549,18 @@ int runTriangle(int argc, const char **argv)
     KmerWarning w;
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
+    if (cluster) {
+        mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
+        mashgpu_sketch_set set;
+        vector<uint64_t> h, l; vector<uint32_t> nn;
+        sketch.toSketchSet(set, h, nn, l);
+        mashgpu_dist_job *job = 0;
+        if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
+        writeClusters(job, sketch, comment, parameters.parallelism);
+        mashgpu_dist_close(job);
+        if (w.warningCount > 0 && !parameters.reads) warnKmerSize(parameters, w.lengthMax, w.lengthMaxName, w.randomChance, w.kMin, w.warningCount);
+        return 0;
+    }
     if (!edge) {
         cout << '\t' << n << endl;
         cout << (comment ? sketch.getReference(0).comment : sketch.getReference(0).name) << endl;

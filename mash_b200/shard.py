@@ -97,6 +97,48 @@ def merge_best(local, ref_begin, n_best, group=None):
     return merge_best_lists(parts, n_best)
 
 
+def merge_component_labels(parts):
+    """Component labels of a union of graphs on the same n vertices from the labels of each (tensors of n smallest-member labels,
+    as DistJob.components returns them per reference shard) -> the labels of the union, label[i] = smallest vertex of i's component.
+
+    Part r is a star forest i -> L_r[i], which has the components of graph r.  Min-label propagation with pointer jumping over the
+    edges {i, L_r[i]} of all parts: every round hooks each root under the smallest root it is joined to, then flattens the forest
+    until every vertex points at its root; at the fixed point no edge joins two labels.  Labels only ever move to a smaller vertex of
+    the same component, so the fixed point is the smallest member of each.  Torch ops only: runs on the labels' device."""
+    if not parts:
+        raise ValueError("no label arrays to merge")
+    parts = [torch.as_tensor(p).to(torch.int64) for p in parts]
+    n, dev = parts[0].numel(), parts[0].device
+    idx = torch.arange(n, dtype=torch.int64, device=dev)
+    src = torch.cat([idx] * len(parts))
+    dst = torch.cat([p.to(dev).reshape(-1) for p in parts])
+    lab = idx.clone()
+    while True:
+        a, b = lab[src], lab[dst]
+        m = torch.minimum(a, b)
+        new = lab.clone()
+        new.scatter_reduce_(0, a, m, "amin")
+        new.scatter_reduce_(0, b, m, "amin")
+        while True:
+            jumped = new[new]
+            if torch.equal(jumped, new):
+                break
+            new = jumped
+        if torch.equal(new, lab):
+            return lab
+        lab = new
+
+
+def merge_components(labels, group=None):
+    """Global components from per-shard ones.  With the reference axis sharded, DistJob.components of an encoded job on a rank
+    yields the components of that rank's edges over all sketches; the component graph is the union of the ranks' edge sets, so
+    merging the label arrays is exact.  labels: this rank's (n,) labels (numpy or tensor; the same n on every rank).  Returns the
+    global labels (int64) on every rank, on the device of the input."""
+    world = td.get_world_size(group)
+    mine = torch.as_tensor(labels).to(torch.int64).contiguous()
+    return merge_component_labels(list(_all_gather(mine, world, group)))
+
+
 class DictOps:
     """The four device steps of the sharded dictionary build, on torch tensors (C ABI: mashgpu_dict_*).  The CPU tests pass
     a stand-in with the same methods to exercise the exchange protocol under gloo."""
