@@ -318,6 +318,23 @@ int mashgpu_dist_best_stats(mashgpu_dist_job *job, uint64_t *blocks_run, uint64_
 int mashgpu_dist_components(mashgpu_dist_job *job, uint32_t *labels, uint64_t *n_edges);
 int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_labels, uint64_t *n_edges, void *stream);
 
+/* Minimum spanning forest of the component graph above, weighted by distance (DESIGN.md 3.9); no counterpart in the reference.
+ * Self jobs (qry == NULL) and encoded jobs only; the lower triangle whatever mashgpu_dist_set_triangle says.  The graph is the one of
+ * mashgpu_dist_components: an edge {i, j}, j < i, for every pair (q = i, r) with pass == 1 and numer > 0, j = r for a self job and
+ * ref_begin + r for an encoded one.  Edges are ordered by the strict total order (distance as a double, j, i), under which the forest
+ * is unique: it equals Kruskal's algorithm over the dense grid under that order, whatever the evaluation order or the merge path.
+ * For every t <= max_distance the forest edges with distance <= t have the components of mashgpu_dist_components at
+ * max_distance t (the same max_pvalue): the forest is the single-linkage dendrogram of the passing pairs.
+ * Outputs: *n_edges <= n_qry - 1 edges in that order (capacity n_qry - 1 each), row = i, col = j, and numer, denom, distance, pvalue
+ * bit-identical to what mashgpu_dist_run returns for (q = i, r = j - ref_begin) of the same job.  *n_rounds = Boruvka rounds run
+ * (at most ceil(log2 n_qry) + 1).  An encoded job over a shard of the reference axis yields the forest of that shard's edges; the
+ * forest of the union of the shards' forests is the global one (shard.merge_spanning_forests).  0 or 1 sketches give 0 edges and
+ * 0 rounds.  A job with a separate query set and NULL outputs are MASHGPU_ERR_INVALID.  Synchronises the stream. */
+int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row, uint32_t *col, uint32_t *numer, uint32_t *denom, double *distance,
+                                 double *pvalue, uint64_t *n_edges, uint64_t *n_rounds);
+int mashgpu_dist_spanning_forest_dev(mashgpu_dist_job *job, uint32_t *d_row, uint32_t *d_col, uint32_t *d_numer, uint32_t *d_denom,
+                                     double *d_distance, double *d_pvalue, uint64_t *n_edges, uint64_t *n_rounds, void *stream);
+
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE
  * instead (a sample sort): a rank sorts only its own rows' hashes, the sorted keys are cut at G-1 splitters, every rank

@@ -125,6 +125,9 @@ def load_library():
     L.mashgpu_dist_best_stats.argtypes = [C.c_void_p, u64p, u64p, u64p, f64p]
     L.mashgpu_dist_components.argtypes = [C.c_void_p, u32p, u64p]
     L.mashgpu_dist_components_dev.argtypes = [C.c_void_p, C.c_void_p, u64p, C.c_void_p]
+    L.mashgpu_dist_spanning_forest.argtypes = [C.c_void_p, u32p, u32p, u32p, u32p, f64p, f64p, u64p, u64p]
+    L.mashgpu_dist_spanning_forest_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   u64p, u64p, C.c_void_p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
     L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
@@ -488,6 +491,29 @@ class DistJob:
         n = C.c_uint64(0)
         self.eng._check(self.eng.lib.mashgpu_dist_components_dev(self.h, d_labels, C.byref(n), stream))
         return n.value
+
+    def spanning_forest(self):
+        """Minimum spanning forest of the same graph as components(), under the order (distance, col, row): a dict of the edges in
+        that order, row (> col), col, numer, denom, distance, pvalue (values as run() returns them for (q = row, r = col - ref_begin)),
+        plus "rounds", the Boruvka rounds run.  Self and encoded jobs only."""
+        m = max(self.n_qry - 1, 0)
+        out = {"row": np.zeros(m, np.uint32), "col": np.zeros(m, np.uint32), "numer": np.zeros(m, np.uint32), "denom": np.zeros(m, np.uint32),
+               "distance": np.zeros(m, np.float64), "pvalue": np.zeros(m, np.float64)}
+        n, rounds = C.c_uint64(0), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_spanning_forest(self.h, _p(out["row"], u32p), _p(out["col"], u32p), _p(out["numer"], u32p),
+                                                                  _p(out["denom"], u32p), _p(out["distance"], f64p), _p(out["pvalue"], f64p),
+                                                                  C.byref(n), C.byref(rounds)))
+        out = {k: v[:n.value] for k, v in out.items()}
+        out["rounds"] = rounds.value
+        return out
+
+    def spanning_forest_dev(self, d_row, d_col, d_numer, d_denom, d_distance, d_pvalue, stream=None):
+        """spanning_forest() into device arrays of n_qry - 1 entries (uint32 row, col, numer, denom; float64 distance, pvalue);
+        returns (n_edges, n_rounds)."""
+        n, rounds = C.c_uint64(0), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_spanning_forest_dev(self.h, d_row, d_col, d_numer, d_denom, d_distance, d_pvalue,
+                                                                      C.byref(n), C.byref(rounds), stream))
+        return n.value, rounds.value
 
     def set_prefilter(self, mode):
         """-1 = auto (default), 0 = merge every pair, 1 = always probe the reference tiles first."""

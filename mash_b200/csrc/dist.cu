@@ -22,6 +22,8 @@
 // final pass flag, dist_emit and dist_fix_kernel, capture the hits, and dist_best.cuh selects the N nearest of every query.
 // A component run (mashgpu_dist_components, DESIGN.md 3.8) is the same again: at those two places dist_cc.cuh unions the two sketches
 // of every hit of the lower triangle into a forest, whose roots become the components' labels.
+// A spanning-forest run (mashgpu_dist_spanning_forest, DESIGN.md 3.9) repeats such runs in Boruvka rounds: at the same places
+// dist_msf.cuh offers every hit to the cheapest-edge slots of its two components.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -37,6 +39,7 @@
 #include "dist_filter.cuh"
 #include "dist_best.cuh"
 #include "dist_cc.cuh"
+#include "dist_msf.cuh"
 
 namespace mashgpu {
 
@@ -77,7 +80,8 @@ struct DistArgs {
     // deferred p-values (dist_fix_kernel): pairs with shared hashes whose binomial tail is evaluated in a dense second pass
     struct FixEntry *fix_list; unsigned long long *fix_count; uint64_t fix_capacity;
     BestCapture best;           // best runs: hits (pass, common > 0) are captured here; every dense output and the pass list are NULL then
-    CcCapture cc;               // component runs: hits are unioned here (the sketches q and tri_r0 + r); NULL outputs and pass list, as for best
+    GraphCapture graph;         // component runs and spanning-forest rounds: hits are unioned or offered here (the sketches q and tri_r0 + r);
+                                // NULL outputs and pass list, as for best
 };
 
 struct FixEntry { uint64_t o; uint32_t common, denom; };
@@ -135,7 +139,7 @@ __device__ __forceinline__ void dist_emit(const DistArgs &a, uint32_t q, uint32_
     if (deferred) return;
     if (a.list_idx && pass) dist_list_append(a, o, common, denom, dist, p);
     if (a.best.cand && pass && common) dist_best_append(a.best, q - a.q_begin, r, common, denom, dist, p);
-    if (a.cc.parent && pass && common) dist_cc_union(a.cc, q, a.tri_r0 + r);
+    if (a.graph.forest && pass && common) dist_graph_hit(a.graph, q, a.tri_r0 + r, dist);
     if (a.pvalue) a.pvalue[o] = p;
     if (a.pass) a.pass[o] = pass ? 1 : 0;
 }
@@ -150,12 +154,12 @@ __global__ void __launch_bounds__(256) dist_fix_kernel(const DistArgs a)
         const uint32_t q = a.q_begin + (uint32_t)(e.o / a.n_ref), r = (uint32_t)(e.o % a.n_ref);
         const double p = mash_pvalue(e.common, a.ref_len[r], a.qry_len[q], a.kmer_space, e.denom, &a.binom);
         const bool pass = !(a.max_pvalue >= 0 && p > a.max_pvalue);
-        if ((a.list_idx || a.best.cand) && pass) {
+        if ((a.list_idx || a.best.cand || a.graph.forest) && pass) {        // queued pairs share a hash
             const double dist = (e.denom == a.S) ? a.dist_lut[e.common] : mash_distance(e.common, e.denom, a.kmer_size);
             if (a.list_idx) dist_list_append(a, e.o, e.common, e.denom, dist, p);
-            else dist_best_append(a.best, q - a.q_begin, r, e.common, e.denom, dist, p);      // queued pairs share a hash
+            else if (a.best.cand) dist_best_append(a.best, q - a.q_begin, r, e.common, e.denom, dist, p);
+            else dist_graph_hit(a.graph, q, a.tri_r0 + r, dist);
         }
-        if (a.cc.parent && pass) dist_cc_union(a.cc, q, a.tri_r0 + r);
         if (a.pvalue) a.pvalue[e.o] = p;
         if (a.pass) a.pass[e.o] = pass ? 1 : 0;
     }
@@ -470,8 +474,8 @@ __global__ void __launch_bounds__(PROBE_THREADS, 1) dist_probe_kernel(const Dist
         } else if (mine && !((mask >> lane) & 1u)) {
             // empty intersection: the merge would take min(s', |A| + |B|) union steps and count nothing
             const uint32_t denom = min(a.S, nA + nB_all);
-            if (a.best.cand || a.cc.parent) {
-                // best or component run: a pair without a shared hash is not a hit, whatever its denominator
+            if (a.best.cand || a.graph.forest) {
+                // best, component or spanning-forest run: a pair without a shared hash is not a hit, whatever its denominator
             } else if (denom == a.S && a.list_idx && pass_const == 0) {
                 // filtered run (-d / -v) and distance 1 / p-value 1 does not pass: nothing to write for this pair
             } else if (denom == a.S && !a.list_idx) {
@@ -636,15 +640,9 @@ __global__ void __launch_bounds__(PAIR_WARPS_MAX * 32) dist_pair_kernel(const Di
     }
 }
 
-// General fallback for sketch sizes whose tiles do not fit in shared memory (s > ~1035): one thread per pair, rows read
-// straight from global memory (L1/L2).  Same arithmetic, an order of magnitude slower; large -s is the rare case.
-__global__ void __launch_bounds__(256) dist_kernel_general(const DistArgs a)
+// The sequential merge of one pair (query q, reference r) straight from global memory: (common, denom).
+__device__ __forceinline__ uint2 dist_merge_pair(const DistArgs &a, uint32_t q, uint32_t r)
 {
-    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    const uint64_t total = (uint64_t)a.q_count * a.n_ref;
-    if (t >= total) return;
-    const uint32_t q = a.q_begin + (uint32_t)(t / a.n_ref), r = (uint32_t)(t % a.n_ref);
-    if (a.triangle && a.tri_r0 + r >= q) return;
     const uint32_t *A = a.ranks + (a.ref_row0 + r) * (uint64_t)a.P;
     const uint32_t *B = a.ranks + (a.qry_row0 + q) * (uint64_t)a.P;
     uint32_t i = 0, j = 0;
@@ -657,8 +655,35 @@ __global__ void __launch_bounds__(256) dist_kernel_general(const DistArgs a)
     const uint32_t nA = a.ref_n[r];
     const uint32_t bogus = i > nA ? i - nA : 0;
     const uint32_t denom = a.S - bogus;
-    const uint32_t common = (i - bogus) + (j - bogus) - denom;
-    dist_emit(a, q, r, common, denom, a.ref_len[r]);
+    return make_uint2((i - bogus) + (j - bogus) - denom, denom);
+}
+
+// General fallback for sketch sizes whose tiles do not fit in shared memory (s > ~1035): one thread per pair, rows read
+// straight from global memory (L1/L2).  Same arithmetic, an order of magnitude slower; large -s is the rare case.
+__global__ void __launch_bounds__(256) dist_kernel_general(const DistArgs a)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    const uint64_t total = (uint64_t)a.q_count * a.n_ref;
+    if (t >= total) return;
+    const uint32_t q = a.q_begin + (uint32_t)(t / a.n_ref), r = (uint32_t)(t % a.n_ref);
+    if (a.triangle && a.tri_r0 + r >= q) return;
+    const uint2 cd = dist_merge_pair(a, q, r);
+    dist_emit(a, q, r, cd.x, cd.y, a.ref_len[r]);
+}
+
+// Values of the spanning forest's edges, once after its last round: the sequential merge of dist_kernel_general and the arithmetic
+// of dist_emit / dist_fix_kernel, so every value is the one a dense run returns for (q = i, r = j - tri_r0).  Every forest edge
+// shares a hash, so its p-value is the binomial tail.  `lo` holds the edges (j << 32 | i) in forest order.
+__global__ void __launch_bounds__(256) msf_values_kernel(const DistArgs a, const unsigned long long *lo, uint64_t m, uint32_t *row,
+                                                         uint32_t *col, uint32_t *numer, uint32_t *denom, double *distance, double *pvalue)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t >= m) return;
+    const uint32_t q = (uint32_t)lo[t], j = (uint32_t)(lo[t] >> 32), r = j - a.tri_r0;
+    const uint2 cd = dist_merge_pair(a, q, r);
+    row[t] = q; col[t] = j; numer[t] = cd.x; denom[t] = cd.y;
+    distance[t] = (cd.y == a.S) ? a.dist_lut[cd.x] : mash_distance(cd.x, cd.y, a.kmer_size);
+    pvalue[t] = mash_pvalue(cd.x, a.ref_len[r], a.qry_len[q], a.kmer_space, cd.y, &a.binom);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1555,6 +1580,24 @@ extern "C" int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, ui
 // ---------------------------------------------------------------------------------------------------------
 constexpr uint64_t CC_BLOCK_PAIRS = 1ull << 31;     // pairs of one run: bounds the work lists, the pair list and the p-value queue
 
+// Runs every pair of the lower triangle of a self or encoded job once, in blocks of CC_BLOCK_PAIRS / n_ref queries, with the capture
+// that set_target puts into each run's arguments.  Lower triangle whatever the job's own setting: query q meets the rows below it
+// only, so the queries up to the first reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
+template <class SetTarget>
+static int enqueue_lower_triangle(mashgpu_dist_job *job, cudaStream_t st, SetTarget set_target)
+{
+    const uint64_t n = job->n_qry, n_ref = job->n_ref;
+    const uint64_t q_first = job->self ? 1 : job->ref_row0 + 1;
+    const uint64_t block = std::max<uint64_t>(1, CC_BLOCK_PAIRS / std::max<uint64_t>(n_ref, 1));
+    for (uint64_t q0 = q_first; n_ref && q0 < n; q0 += block) {
+        DistArgs a = dist_args(job, q0, std::min(block, n - q0));
+        a.triangle = 1;
+        set_target(a);
+        MG_TRY(dist_enqueue(job, a, st));
+    }
+    return MASHGPU_OK;
+}
+
 extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_labels, uint64_t *n_edges, void *stream)
 {
     if (!job) return MASHGPU_ERR_INVALID;
@@ -1562,7 +1605,7 @@ extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_la
     if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "components need a self comparison (qry == NULL) or an encoded job");
     if (!d_labels || !n_edges) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     *n_edges = 0;
-    const uint64_t n = job->n_qry, n_ref = job->n_ref;
+    const uint64_t n = job->n_qry;
     if (n == 0) return MASHGPU_OK;
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
@@ -1570,16 +1613,8 @@ extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_la
     MG_CUDA(ctx, cudaMemsetAsync(job->cc_edges.p, 0, 8, st));
     cc_init_kernel<<<blocks_for(n), 256, 0, st>>>(d_labels, n);
     MG_CUDA(ctx, cudaGetLastError());
-    // The labels are the forest.  Lower triangle whatever the job's own setting: query q meets the rows below it only, so the
-    // queries up to the first reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
-    const uint64_t q_first = job->self ? 1 : job->ref_row0 + 1;
-    const uint64_t block = std::max<uint64_t>(1, CC_BLOCK_PAIRS / std::max<uint64_t>(n_ref, 1));
-    for (uint64_t q0 = q_first; n_ref && q0 < n; q0 += block) {
-        DistArgs a = dist_args(job, q0, std::min(block, n - q0));
-        a.triangle = 1;
-        a.cc = CcCapture{d_labels, job->cc_edges.p};
-        MG_TRY(dist_enqueue(job, a, st));
-    }
+    // the labels are the forest
+    MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) { a.graph = GraphCapture{d_labels, job->cc_edges.p, nullptr}; }));
     cc_flatten_kernel<<<blocks_for(n), 256, 0, st>>>(d_labels, n);
     MG_CUDA(ctx, cudaGetLastError());
     ctx->kernel_launches += 2;
@@ -1605,6 +1640,100 @@ extern "C" int mashgpu_dist_components(mashgpu_dist_job *job, uint32_t *labels, 
     MG_TRY(mashgpu_dist_components_dev(job, d.p, n_edges, ctx->stream));
     MG_CUDA(ctx, cudaMemcpyAsync(labels, d.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
     MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return MASHGPU_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Minimum spanning forest (DESIGN.md 3.9)
+// ---------------------------------------------------------------------------------------------------------
+extern "C" int mashgpu_dist_spanning_forest_dev(mashgpu_dist_job *job, uint32_t *d_row, uint32_t *d_col, uint32_t *d_numer, uint32_t *d_denom,
+                                                double *d_distance, double *d_pvalue, uint64_t *n_edges, uint64_t *n_rounds, void *stream)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "a spanning forest needs a self comparison (qry == NULL) or an encoded job");
+    if (!d_row || !d_col || !d_numer || !d_denom || !d_distance || !d_pvalue || !n_edges || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_edges = 0; *n_rounds = 0;
+    const uint64_t n = job->n_qry;
+    if (n < 2 || job->n_ref == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    const uint64_t cap = n - 1;
+    // O(n) state: labels, the union-find of the forest, one slot per component, the forest's keys and their sorted copy
+    DevBuf<uint32_t> label, parent; DevBuf<MsfKey> best; DevBuf<unsigned long long> lo, hi, lo2, hi2, count; DevBuf<uint8_t> tmp;
+    if (label.alloc(n) != cudaSuccess || parent.alloc(n) != cudaSuccess || best.alloc(n) != cudaSuccess || lo.alloc(cap) != cudaSuccess ||
+        hi.alloc(cap) != cudaSuccess || lo2.alloc(cap) != cudaSuccess || hi2.alloc(cap) != cudaSuccess || count.alloc(1) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (spanning forest of %llu sketches)", (unsigned long long)n);
+    cc_init_kernel<<<blocks_for(n), 256, 0, st>>>(label.p, n);
+    cc_init_kernel<<<blocks_for(n), 256, 0, st>>>(parent.p, n);
+    MG_CUDA(ctx, cudaMemsetAsync(count.p, 0, 8, st));
+    MG_CUDA(ctx, cudaGetLastError());
+    ctx->kernel_launches += 2;
+    // A productive round joins every component that has an edge to another one, so it at least halves their number: more than
+    // ceil(log2 n) + 1 rounds (the last one finds no edge) cannot happen.
+    uint64_t max_rounds = 1;
+    while ((1ull << (max_rounds - 1)) < n) max_rounds++;
+    unsigned long long edges = 0;
+    uint64_t rounds = 0;
+    while (edges < cap) {
+        if (rounds == max_rounds) return fail(ctx, MASHGPU_ERR_CUDA, "internal error: spanning forest not done after %llu rounds", (unsigned long long)rounds);
+        MG_CUDA(ctx, cudaMemsetAsync(best.p, 0xFF, n * sizeof(MsfKey), st));
+        MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) { a.graph = GraphCapture{label.p, nullptr, best.p}; }));
+        msf_hook_kernel<<<blocks_for(n), 256, 0, st>>>(label.p, best.p, parent.p, count.p, lo.p, hi.p, cap, n);
+        cc_flatten_kernel<<<blocks_for(n), 256, 0, st>>>(parent.p, n);
+        MG_CUDA(ctx, cudaGetLastError());
+        MG_CUDA(ctx, cudaMemcpyAsync(label.p, parent.p, n * 4, cudaMemcpyDeviceToDevice, st));
+        ctx->kernel_launches += 2;
+        unsigned long long now = 0;
+        MG_CUDA(ctx, cudaMemcpyAsync(&now, count.p, 8, cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        rounds++;
+        if (now > cap) return fail(ctx, MASHGPU_ERR_CUDA, "internal error: %llu spanning forest edges over %llu sketches", now, (unsigned long long)n);
+        if (now == edges) break;
+        edges = now;
+    }
+    *n_rounds = rounds;
+    if (edges == 0) return MASHGPU_OK;
+    // forest order: (j, i) first, then a stable pass on the distance bits
+    size_t tb = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb, lo.p, lo2.p, hi.p, hi2.p, (int)edges, 0, 64, st);
+    if (tmp.alloc(tb) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (sort scratch)");
+    MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tb, lo.p, lo2.p, hi.p, hi2.p, (int)edges, 0, 64, st));
+    MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tb, hi2.p, hi.p, lo2.p, lo.p, (int)edges, 0, 64, st));
+    DistArgs a = dist_args(job, 0, n);
+    msf_values_kernel<<<blocks_for(edges), 256, 0, st>>>(a, lo.p, edges, d_row, d_col, d_numer, d_denom, d_distance, d_pvalue);
+    MG_CUDA(ctx, cudaGetLastError());
+    MG_CUDA(ctx, cudaStreamSynchronize(st));        // the scratch goes out of scope
+    ctx->kernel_launches += 9;         // two radix sorts and the values
+    *n_edges = edges;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row, uint32_t *col, uint32_t *numer, uint32_t *denom,
+                                            double *distance, double *pvalue, uint64_t *n_edges, uint64_t *n_rounds)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "a spanning forest needs a self comparison (qry == NULL) or an encoded job");
+    if (!row || !col || !numer || !denom || !distance || !pvalue || !n_edges || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_edges = 0; *n_rounds = 0;
+    const uint64_t n = job->n_qry;
+    if (n < 2) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    const uint64_t cap = n - 1;
+    DevBuf<uint32_t> d32; DevBuf<double> d64;
+    if (d32.alloc(4 * cap) != cudaSuccess || d64.alloc(2 * cap) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu forest edges)", (unsigned long long)cap);
+    MG_TRY(mashgpu_dist_spanning_forest_dev(job, d32.p, d32.p + cap, d32.p + 2 * cap, d32.p + 3 * cap, d64.p, d64.p + cap, n_edges, n_rounds, ctx->stream));
+    const uint64_t m = *n_edges;
+    cudaStream_t st = ctx->stream;
+    MG_CUDA(ctx, cudaMemcpyAsync(row, d32.p, m * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(col, d32.p + cap, m * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(numer, d32.p + 2 * cap, m * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(denom, d32.p + 3 * cap, m * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(distance, d64.p, m * 8, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(pvalue, d64.p + cap, m * 8, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
     return MASHGPU_OK;
 }
 

@@ -12,12 +12,6 @@
 
 namespace mashgpu {
 
-// Capture target inside DistArgs; parent == nullptr outside component runs.
-struct CcCapture {
-    uint32_t *parent;               // the forest: parent[i] <= i, parent[i] == i at a root; indexed by query row
-    unsigned long long *edges;      // edges captured (every unordered pair once: the run enumerates the lower triangle)
-};
-
 // Parent reads and the halving writes go through L2 (relaxed, device scope): a plain load may be served from a stale L1 line
 // inside the retry loop of a hook.
 __device__ __forceinline__ uint32_t cc_load(const uint32_t *p)
@@ -47,20 +41,28 @@ __device__ __forceinline__ uint32_t cc_find(uint32_t *parent, uint32_t x)
     return x;
 }
 
-// Joins the components of q and r (r_global: the reference's row in the query numbering, tri_r0 + r) and counts the edge.  Not
-// inlined, like dist_best_append: the merge kernels' epilogues keep their register allocation.
-__device__ __noinline__ void dist_cc_union(const CcCapture c, uint32_t q, uint32_t r_global)
+// Joins the trees of x and y: the larger root is hooked under the smaller one.  Shared by the component runs and the spanning
+// forest's rounds (dist_msf.cuh).
+__device__ __forceinline__ void cc_join(uint32_t *parent, uint32_t x, uint32_t y)
 {
-    const unsigned peers = __activemask();          // one counter update per warp for the lanes that report an edge together
-    if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(c.edges, (unsigned long long)__popc(peers));
-    uint32_t a = cc_find(c.parent, q), b = cc_find(c.parent, r_global);
+    uint32_t a = cc_find(parent, x), b = cc_find(parent, y);
     while (a != b) {
         if (a < b) { const uint32_t t = a; a = b; b = t; }         // hook the larger root a under the smaller b
-        const uint32_t old = atomicCAS(c.parent + a, a, b);
+        const uint32_t old = atomicCAS(parent + a, a, b);
         if (old == a) break;
-        a = cc_find(c.parent, old);                                 // a was hooked meanwhile: retry from its new root
-        b = cc_find(c.parent, b);
+        a = cc_find(parent, old);                                   // a was hooked meanwhile: retry from its new root
+        b = cc_find(parent, b);
     }
+}
+
+// Joins the components of q and r (r_global: the reference's row in the query numbering, tri_r0 + r) in the forest `parent`
+// (parent[i] <= i, parent[i] == i at a root; indexed by query row) and counts the edge in `edges` (every unordered pair once: the
+// run enumerates the lower triangle).  Called through the not-inlined dist_graph_hit (dist_msf.cuh).
+__device__ __forceinline__ void dist_cc_union(uint32_t *parent, unsigned long long *edges, uint32_t q, uint32_t r_global)
+{
+    const unsigned peers = __activemask();          // one counter update per warp for the lanes that report an edge together
+    if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(edges, (unsigned long long)__popc(peers));
+    cc_join(parent, q, r_global);
 }
 
 __global__ void cc_init_kernel(uint32_t *parent, uint64_t n)

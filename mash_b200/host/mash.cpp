@@ -3,7 +3,8 @@
 // CommandTriangle.cpp:45-214, CommandContain.cpp:33-203, CommandScreen.cpp:54-461, CommandTaxScreen.cpp:57-480,
 // CommandInfo.cpp:222-299): same option identifiers and defaults (Command.cpp:165-200), same stdout formats (iostream default
 // precision), same ordering contracts.  It exists so that the reference's `make test` flow can be replayed against the GPU engine;
-// help text, `bounds` and `find` are out of scope.
+// help text, `bounds` and `find` are out of scope.  `triangle -G` (clusters) and `triangle -T` (the single-linkage tree as a minimum
+// spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -518,6 +519,25 @@ static void writeClusters(mashgpu_dist_job *job, const Sketch &sketch, bool comm
     cerr << "Clusters: " << clusters << " from " << edges << " edges" << endl;
 }
 
+// `mash triangle -T`: the minimum spanning forest of the same graph, weighted by distance (ties broken by the smaller, then the
+// larger sketch index), built on the device.  One `-E` line per forest edge, in forest order: the lines up to distance t are a
+// forest of the clusters `-G -d t` gives, so a cut at any t <= -d is a prefix of the output (single linkage).
+static void writeForest(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int threads)
+{
+    const uint64_t n = sketch.getReferenceCount(), cap = n ? n - 1 : 0;
+    vector<uint32_t> row(cap), col(cap), numer(cap), denom(cap);
+    vector<double> distance(cap), pValue(cap);
+    uint64_t edges = 0, rounds = 0;
+    if (n > 1 && mashgpu_dist_spanning_forest(job, row.data(), col.data(), numer.data(), denom.data(), distance.data(), pValue.data(), &edges,
+                                              &rounds) != MASHGPU_OK) gpuFail();
+    mashhost::writeRows(edges, threads, 1, [&](uint64_t e, mashhost::OutBuf &o) {      // the -E line of the pair (q = row, r = col)
+        const Sketch::Reference &ref = sketch.getReference(row[e]), &qry = sketch.getReference(col[e]);
+        o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.str(comment ? qry.comment : qry.name); o.ch('\t');
+        o.dbl(distance[e]); o.ch('\t'); o.dbl(pValue[e]); o.ch('\t'); o.u64(numer[e]); o.ch('/'); o.u64(denom[e]); o.ch('\n');
+    });
+    cerr << "Forest: " << edges << " edges, " << n - edges << " trees in " << rounds << " rounds" << endl;
+}
+
 int runTriangle(int argc, const char **argv)
 {
     Command c;
@@ -526,19 +546,24 @@ int runTriangle(int argc, const char **argv)
     c.add("comment", Option(Option::Boolean, "C", ""));
     c.add("edge", Option(Option::Boolean, "E", ""));
     c.add("cluster", Option(Option::Boolean, "G", ""));       // not an option of the reference: its users cluster the -E output
+    c.add("tree", Option(Option::Boolean, "T", ""));          // not an option of the reference either
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.useSketchOptions();
     if (c.parse(argc, argv)) return 1;
     if (c.arguments.size() < 1 || c.opt("help").active) {
         cerr << "usage: mash triangle [options] <seq1> [<seq2>] ..." << endl
-             << "  -G        Clusters: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash (not with -E)." << endl;
+             << "  -G        Clusters: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash (not with -E)." << endl
+             << "  -T        Single-linkage tree: the minimum spanning forest of the -G graph by distance, as -E lines in order of distance (not with" << endl
+             << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl;
         return 0;
     }
-    bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active;
+    bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active, tree = c.opt("tree").active;
     if (cluster && edge) { cerr << "ERROR: The option -G cannot be used with -E (clusters replace the edge list)." << endl; return 1; }
+    if (tree && edge) { cerr << "ERROR: The option -T cannot be used with -E (the forest replaces the edge list)." << endl; return 1; }
+    if (tree && cluster) { cerr << "ERROR: The option -T cannot be used with -G (cut the forest at the distance instead)." << endl; return 1; }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
-    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster) edge = true;
+    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree) edge = true;
     Sketch::Parameters parameters;
     if (sketchParameterSetup(parameters, c)) return 1;
     if (c.arguments.size() == 1 && !c.opt("list").active) parameters.concatenated = false;
@@ -549,14 +574,15 @@ int runTriangle(int argc, const char **argv)
     KmerWarning w;
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
-    if (cluster) {
+    if (cluster || tree) {
         mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
         mashgpu_sketch_set set;
         vector<uint64_t> h, l; vector<uint32_t> nn;
         sketch.toSketchSet(set, h, nn, l);
         mashgpu_dist_job *job = 0;
         if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
-        writeClusters(job, sketch, comment, parameters.parallelism);
+        if (tree) writeForest(job, sketch, comment, parameters.parallelism);
+        else writeClusters(job, sketch, comment, parameters.parallelism);
         mashgpu_dist_close(job);
         if (w.warningCount > 0 && !parameters.reads) warnKmerSize(parameters, w.lengthMax, w.lengthMaxName, w.randomChance, w.kMin, w.warningCount);
         return 0;

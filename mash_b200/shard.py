@@ -110,9 +110,12 @@ def merge_component_labels(parts):
     parts = [torch.as_tensor(p).to(torch.int64) for p in parts]
     n, dev = parts[0].numel(), parts[0].device
     idx = torch.arange(n, dtype=torch.int64, device=dev)
-    src = torch.cat([idx] * len(parts))
-    dst = torch.cat([p.to(dev).reshape(-1) for p in parts])
-    lab = idx.clone()
+    return _min_labels(n, torch.cat([idx] * len(parts)), torch.cat([p.to(dev).reshape(-1) for p in parts]), dev)
+
+
+def _min_labels(n, src, dst, dev):
+    """label[i] = smallest vertex of i's component in the graph on n vertices with the edges {src[e], dst[e]} (int64 tensors)"""
+    lab = torch.arange(n, dtype=torch.int64, device=dev)
     while True:
         a, b = lab[src], lab[dst]
         m = torch.minimum(a, b)
@@ -127,6 +130,68 @@ def merge_component_labels(parts):
         if torch.equal(new, lab):
             return lab
         lab = new
+
+
+FOREST_KEYS = ("row", "col", "numer", "denom", "distance", "pvalue")
+
+
+def merge_spanning_forests(parts, n):
+    """Minimum spanning forest of the union of several edge sets on the same n vertices, from the minimum spanning forest of each
+    (dicts as DistJob.spanning_forest returns them, `col` global, e.g. one per reference shard).  Exact: by the cycle property an edge
+    that is not in its own part's forest is the largest of a cycle in the union, so the union of the parts' forests contains the
+    forest of the union.  Edges are ranked once by (distance, col, row), the forest's strict order; Boruvka rounds on the rank then
+    pick every component's cheapest edge with scatter_reduce and join the components with the min-label propagation of
+    merge_component_labels.  Torch ops only: runs on the device of the parts, with no communication.  Returns the forest's edges in
+    forest order as a dict of tensors (integers as int64)."""
+    if not parts:
+        raise ValueError("no forests to merge")
+    cols = {k: torch.cat([torch.as_tensor(p[k]).reshape(-1).to(torch.float64 if k in ("distance", "pvalue") else torch.int64) for p in parts])
+            for k in FOREST_KEYS}
+    dev = cols["row"].device
+    cols = {k: v.to(dev) for k, v in cols.items()}
+    # rank = position in (distance, col, row) order: stable sorts from the last key to the first
+    order = torch.sort(cols["row"], stable=True).indices
+    order = order[torch.sort(cols["col"][order], stable=True).indices]
+    order = order[torch.sort(cols["distance"][order], stable=True).indices]
+    u, v = cols["row"][order], cols["col"][order]
+    m = u.numel()
+    rank = torch.arange(m, dtype=torch.int64, device=dev)
+    chosen = torch.zeros(m, dtype=torch.bool, device=dev)
+    lab = torch.arange(n, dtype=torch.int64, device=dev)
+    while True:
+        a, b = lab[u], lab[v]
+        live = a != b
+        if not bool(live.any()):
+            break
+        best = torch.full((n,), m, dtype=torch.int64, device=dev)
+        best.scatter_reduce_(0, a[live], rank[live], "amin")
+        best.scatter_reduce_(0, b[live], rank[live], "amin")
+        chosen[best[best < m]] = True           # a mutual pick is one edge
+        lab = _min_labels(n, u[chosen], v[chosen], dev)
+    keep = order[chosen]
+    return {k: c[keep] for k, c in cols.items()}
+
+
+def spanning_forest(local, group=None):
+    """Global minimum spanning forest from per-shard ones.  With the reference axis sharded, DistJob.spanning_forest of an encoded job on
+    a rank yields the forest of that rank's edges; all ranks gather the shards' forests (at most n - 1 edges each) and merge them
+    (merge_spanning_forests).  local: this rank's forest (numpy arrays or tensors).  Returns the global forest on every rank, as tensors
+    on the device of the inputs (integers as int64)."""
+    world = td.get_world_size(group)
+    mine = {k: torch.as_tensor(local[k]).reshape(-1) for k in FOREST_KEYS}
+    mine = {k: v.to(torch.float64 if k in ("distance", "pvalue") else torch.int64).contiguous() for k, v in mine.items()}
+    dev = mine["row"].device
+    counts = _all_gather(torch.tensor([mine["row"].numel()], dtype=torch.int64, device=dev), world, group).view(-1).tolist()
+    top = max(counts)
+    parts = [dict() for _ in range(world)]
+    for k, v in mine.items():
+        padded = torch.zeros(top, dtype=v.dtype, device=dev)
+        padded[:v.numel()] = v
+        got = _all_gather(padded, world, group)
+        for r in range(world):
+            parts[r][k] = got[r, :counts[r]]
+    n = max((int(p["row"].max()) + 1 for p in parts if p["row"].numel()), default=0)     # vertices without an edge play no part
+    return merge_spanning_forests(parts, n)
 
 
 def merge_components(labels, group=None):
