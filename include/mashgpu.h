@@ -335,6 +335,30 @@ int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row, uint32_t 
 int mashgpu_dist_spanning_forest_dev(mashgpu_dist_job *job, uint32_t *d_row, uint32_t *d_col, uint32_t *d_numer, uint32_t *d_denom,
                                      double *d_distance, double *d_pvalue, uint64_t *n_edges, uint64_t *n_rounds, void *stream);
 
+/* Neighbor joining (DESIGN.md 3.10); no counterpart in the reference.  Canonical Saitou-Nei / Studier-Keppler NJ over a symmetric
+ * n x n float64 matrix D of which only the lower triangle (j < i) is read, with the operation order fixed so that it is
+ * reproducible bit for bit (tests/nj_model.py):
+ *   r_i = sum of D(i, k) over ascending k, D(i, i) = 0.  While m = |live| > 3, over live positions p < q (a = L[p], b = L[q]) the
+ *   least (Q, q, p) with Q = ((m - 2) * D(a, b) - r_a) - r_b is joined into node u = n + s (join s):
+ *   la = D(a, b) * 0.5 + (r_a - r_b) / (2 * (m - 2)), lb = D(a, b) - la, D(u, k) = ((D(a, k) + D(b, k)) - D(a, b)) * 0.5,
+ *   r_k = ((r_k - D(a, k)) - D(b, k)) + D(u, k), r_u = ((r_a + r_b) - m * D(a, b)) * 0.5; u takes position p, q is removed.
+ *   The last three x, y, z hang from the center 2n - 3 with lx = ((D(x, y) + D(x, z)) - D(y, z)) * 0.5 and so on.
+ * Every step is one IEEE double operation, never fused.  Row sums are updated, not recomputed, so they drift from the exact sums
+ * by rounding; negative branch lengths are returned as computed (no clamping).
+ * Outputs of 2n - 2 entries, nodes 0..n-1 the leaves: parent[v] and length[v] of v's branch; the center has parent UINT32_MAX and
+ * length 0.  Memory: the matrix plus O(n). */
+/* NJ over the caller's n x n float64 device matrix (row i at d_matrix + i * ld, ld >= n; lower triangle read; the matrix is used as
+ * scratch and overwritten).  Host outputs of 2n-2 entries; synchronises `stream` (NULL: the context's stream).  n < 3 or a
+ * non-finite entry in the lower triangle: MASHGPU_ERR_INVALID (the entry is found on the device before the first join). */
+int mashgpu_neighbor_joining_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64_t n, uint64_t ld,
+                                    uint32_t *parent, double *length, void *stream);
+/* NJ over every pair's distance of a self job (qry == NULL): D(i, j), j < i, is the distance mashgpu_dist_run returns for
+ * (q = i, r = j), whatever max_distance, max_pvalue and mashgpu_dist_set_triangle say (none of them is changed).  The job fills an
+ * n x n device matrix with its own runs, then runs mashgpu_neighbor_joining_matrix on it.  n_qry < 3 and a job with a separate query
+ * set: MASHGPU_ERR_INVALID.  Encoded (sharded) jobs: MASHGPU_ERR_UNSUPPORTED.  8 n^2 bytes beyond the device's free memory:
+ * MASHGPU_ERR_NOMEM before anything is allocated. */
+int mashgpu_dist_neighbor_joining(mashgpu_dist_job *job, uint32_t *parent, double *length);
+
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE
  * instead (a sample sort): a rank sorts only its own rows' hashes, the sorted keys are cut at G-1 splitters, every rank

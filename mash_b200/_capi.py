@@ -128,6 +128,8 @@ def load_library():
     L.mashgpu_dist_spanning_forest.argtypes = [C.c_void_p, u32p, u32p, u32p, u32p, f64p, f64p, u64p, u64p]
     L.mashgpu_dist_spanning_forest_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    u64p, u64p, C.c_void_p]
+    L.mashgpu_dist_neighbor_joining.argtypes = [C.c_void_p, u32p, f64p]
+    L.mashgpu_neighbor_joining_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, u32p, f64p, C.c_void_p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
     L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
@@ -346,6 +348,23 @@ class Engine:
         return DistJob.encoded(self, d_rows, d_n_eff, d_length, n_rows, ref_begin, ref_count, sketch_size, k, kmer_space,
                                max_distance, max_pvalue, keepalive)
 
+    def neighbor_joining_matrix(self, d_matrix, n, ld=None, stream=None):
+        """Neighbor-joining tree (DESIGN.md 3.10) of the n x n float64 matrix in the CUDA tensor d_matrix (row i at element i * ld;
+        ld defaults to the row stride of a 2-D tensor, else n).  Only the lower triangle is read, and the whole matrix is overwritten.
+        Returns {"parent": uint32[2n - 2], "length": float64[2n - 2]}: leaves 0..n-1, join s makes node n + s, the center 2n - 3 has
+        parent 0xFFFFFFFF and length 0."""
+        if not getattr(d_matrix, "is_cuda", False) or str(d_matrix.dtype) != "torch.float64":
+            raise ValueError("d_matrix must be a CUDA float64 tensor")
+        if ld is None:
+            ld = d_matrix.stride(0) if d_matrix.dim() == 2 else n
+        if n >= 1 and (n - 1) * ld + n > d_matrix.numel():
+            raise ValueError(f"d_matrix holds {d_matrix.numel()} elements, fewer than an {n} x {n} matrix with ld {ld}")
+        m = max(2 * int(n) - 2, 0)
+        out = {"parent": np.zeros(m, np.uint32), "length": np.zeros(m, np.float64)}
+        self._check(self.lib.mashgpu_neighbor_joining_matrix(self.h, d_matrix.data_ptr(), int(n), int(ld), _p(out["parent"], u32p),
+                                                             _p(out["length"], f64p), stream))
+        return out
+
     # ---- sharded dictionary build (device pointers; see mash_b200/shard.py) ----------------------------------
     def dict_local_sort(self, d_hashes, d_n_hashes, n, stride, sketch_size, d_keys, d_slots, stream=None):
         st = SketchSet(n, stride, d_hashes, d_n_hashes, None, 1)
@@ -514,6 +533,15 @@ class DistJob:
         self.eng._check(self.eng.lib.mashgpu_dist_spanning_forest_dev(self.h, d_row, d_col, d_numer, d_denom, d_distance, d_pvalue,
                                                                       C.byref(n), C.byref(rounds), stream))
         return n.value, rounds.value
+
+    def neighbor_joining(self):
+        """Neighbor-joining tree (DESIGN.md 3.10) of every pair's distance of a self job, D(i, j) = run()'s distance at (q = i, r = j),
+        j < i, whatever max_distance, max_pvalue and set_triangle say: {"parent": uint32[2n - 2], "length": float64[2n - 2]} as
+        Engine.neighbor_joining_matrix returns them.  At least 3 sketches; encoded jobs are refused."""
+        m = max(2 * self.n_qry - 2, 0)
+        out = {"parent": np.zeros(m, np.uint32), "length": np.zeros(m, np.float64)}
+        self.eng._check(self.eng.lib.mashgpu_dist_neighbor_joining(self.h, _p(out["parent"], u32p), _p(out["length"], f64p)))
+        return out
 
     def set_prefilter(self, mode):
         """-1 = auto (default), 0 = merge every pair, 1 = always probe the reference tiles first."""

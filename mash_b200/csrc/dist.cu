@@ -24,6 +24,8 @@
 // of every hit of the lower triangle into a forest, whose roots become the components' labels.
 // A spanning-forest run (mashgpu_dist_spanning_forest, DESIGN.md 3.9) repeats such runs in Boruvka rounds: at the same places
 // dist_msf.cuh offers every hit to the cheapest-edge slots of its two components.
+// Neighbor joining (mashgpu_dist_neighbor_joining, DESIGN.md 3.10) fills an n x n matrix with plain lower-triangle runs (distance
+// output only) and hands it to nj.cu.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -1735,6 +1737,33 @@ extern "C" int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row
     MG_CUDA(ctx, cudaMemcpyAsync(pvalue, d64.p + cap, m * 8, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     return MASHGPU_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Neighbor joining over a self job's distances (DESIGN.md 3.10; the joins are in nj.cu)
+// ---------------------------------------------------------------------------------------------------------
+extern "C" int mashgpu_dist_neighbor_joining(mashgpu_dist_job *job, uint32_t *parent, double *length)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "neighbor joining of an encoded (sharded) job");
+    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining needs a self comparison (qry == NULL)");
+    if (!parent || !length) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    const uint64_t n = job->n_qry;
+    if (n < 3) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining needs at least 3 sketches (got %llu)", (unsigned long long)n);
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    size_t free_b = 0, total_b = 0;
+    MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+    if ((double)n * (double)n * 8.0 > (double)free_b)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "a %llu x %llu distance matrix needs %.3g GB, the device has %.3g GB free", (unsigned long long)n,
+                    (unsigned long long)n, (double)n * (double)n * 8e-9, (double)free_b * 1e-9);
+    DevBuf<double> matrix;
+    if (matrix.alloc(n * n) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu x %llu distance matrix)", (unsigned long long)n, (unsigned long long)n);
+    cudaStream_t st = ctx->stream;
+    // distance output only, row q at matrix + q * n; the lower triangle is all the joins read
+    MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) { a.distance = matrix.p + (uint64_t)a.q_begin * n; }));
+    return mashgpu_neighbor_joining_matrix(ctx, matrix.p, n, n, parent, length, st);
 }
 
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)

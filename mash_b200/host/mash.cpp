@@ -4,7 +4,8 @@
 // CommandInfo.cpp:222-299): same option identifiers and defaults (Command.cpp:165-200), same stdout formats (iostream default
 // precision), same ordering contracts.  It exists so that the reference's `make test` flow can be replayed against the GPU engine;
 // help text, `bounds` and `find` are out of scope.  `triangle -G` (clusters) and `triangle -T` (the single-linkage tree as a minimum
-// spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.
+// spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.  Nor has `triangle -N` (the
+// neighbor-joining tree as a Newick line), which its users compute from the matrix with an NJ program.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -21,6 +22,7 @@
 #include <unistd.h>
 
 #include "fastout.hpp"
+#include "newick.hpp"
 #include "fastx.hpp"
 #include "taxdb.hpp"
 
@@ -538,6 +540,33 @@ static void writeForest(mashgpu_dist_job *job, const Sketch &sketch, bool commen
     cerr << "Forest: " << edges << " edges, " << n - edges << " trees in " << rounds << " rounds" << endl;
 }
 
+// `mash triangle -N`: the neighbor-joining tree of every pair's distance (DESIGN.md 3.10) as one Newick line.  One sketch is its
+// name, two are a cherry with half the distance on each branch; from three on the tree is built on the device.
+static void writeNeighborJoining(mashgpu_dist_job *job, const Sketch &sketch, bool comment)
+{
+    const uint64_t n = sketch.getReferenceCount();
+    vector<string> names(n);
+    for (uint64_t i = 0; i < n; i++) names[i] = comment ? sketch.getReference(i).comment : sketch.getReference(i).name;
+    mashhost::OutBuf o;
+    if (n == 1) {
+        mashhost::newickName(o, names[0]); o.ch(';'); o.ch('\n');
+    } else if (n == 2) {
+        double d[2] = {0, 0};                                                          // row q = 1: (1, 0) and (1, 1)
+        if (mashgpu_dist_run(job, 1, 1, 0, 0, d, 0, 0) != MASHGPU_OK) gpuFail();
+        o.ch('('); mashhost::newickName(o, names[0]); o.ch(':'); o.dbl(d[0] * 0.5); o.ch(',');
+        mashhost::newickName(o, names[1]); o.ch(':'); o.dbl(d[0] * 0.5); o.ch(')'); o.ch(';'); o.ch('\n');
+    } else if (n > 2) {
+        vector<uint32_t> parent(2 * n - 2);
+        vector<double> length(2 * n - 2);
+        if (mashgpu_dist_neighbor_joining(job, parent.data(), length.data()) != MASHGPU_OK) gpuFail();
+        mashhost::writeNewick(o, parent, length, names);
+    }
+    cout.flush();
+    fwrite(o.b.data(), 1, o.b.size(), stdout);
+    fflush(stdout);
+    cerr << "Tree: " << n << " leaves, " << (n > 3 ? n - 3 : 0) << " joins" << endl;
+}
+
 int runTriangle(int argc, const char **argv)
 {
     Command c;
@@ -547,6 +576,7 @@ int runTriangle(int argc, const char **argv)
     c.add("edge", Option(Option::Boolean, "E", ""));
     c.add("cluster", Option(Option::Boolean, "G", ""));       // not an option of the reference: its users cluster the -E output
     c.add("tree", Option(Option::Boolean, "T", ""));          // not an option of the reference either
+    c.add("nj", Option(Option::Boolean, "N", ""));            // nor is this one
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.useSketchOptions();
@@ -555,13 +585,22 @@ int runTriangle(int argc, const char **argv)
         cerr << "usage: mash triangle [options] <seq1> [<seq2>] ..." << endl
              << "  -G        Clusters: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash (not with -E)." << endl
              << "  -T        Single-linkage tree: the minimum spanning forest of the -G graph by distance, as -E lines in order of distance (not with" << endl
-             << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl;
+             << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl
+             << "  -N        Neighbor-joining tree of every pair's distance, as one Newick line (not with -E, -G, -T, -d or -v)." << endl;
         return 0;
     }
     bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active, tree = c.opt("tree").active;
     if (cluster && edge) { cerr << "ERROR: The option -G cannot be used with -E (clusters replace the edge list)." << endl; return 1; }
     if (tree && edge) { cerr << "ERROR: The option -T cannot be used with -E (the forest replaces the edge list)." << endl; return 1; }
     if (tree && cluster) { cerr << "ERROR: The option -T cannot be used with -G (cut the forest at the distance instead)." << endl; return 1; }
+    const bool nj = c.opt("nj").active;
+    if (nj) {
+        for (const char *o : {"edge", "cluster", "tree", "distance", "pvalue"})
+            if (c.opt(o).active) {
+                cerr << "ERROR: The option -N cannot be used with -" << c.opt(o).identifier << " (the tree is built from every pair's distance)." << endl;
+                return 1;
+            }
+    }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
     if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree) edge = true;
     Sketch::Parameters parameters;
@@ -574,14 +613,15 @@ int runTriangle(int argc, const char **argv)
     KmerWarning w;
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
-    if (cluster || tree) {
+    if (cluster || tree || nj) {
         mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
         mashgpu_sketch_set set;
         vector<uint64_t> h, l; vector<uint32_t> nn;
         sketch.toSketchSet(set, h, nn, l);
         mashgpu_dist_job *job = 0;
         if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
-        if (tree) writeForest(job, sketch, comment, parameters.parallelism);
+        if (nj) writeNeighborJoining(job, sketch, comment);
+        else if (tree) writeForest(job, sketch, comment, parameters.parallelism);
         else writeClusters(job, sketch, comment, parameters.parallelism);
         mashgpu_dist_close(job);
         if (w.warningCount > 0 && !parameters.reads) warnKmerSize(parameters, w.lengthMax, w.lengthMaxName, w.randomChance, w.kMin, w.warningCount);
