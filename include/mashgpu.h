@@ -359,6 +359,37 @@ int mashgpu_neighbor_joining_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64_t
  * MASHGPU_ERR_NOMEM before anything is allocated. */
 int mashgpu_dist_neighbor_joining(mashgpu_dist_job *job, uint32_t *parent, double *length);
 
+/* Average (UPGMA) and complete linkage (DESIGN.md 3.11); no counterpart in the reference.  Hierarchical clustering of a symmetric
+ * n x n float64 matrix D of which only the lower triangle (j < i) is read, with the merge order and the operation order fixed so
+ * that it is reproducible bit for bit (tests/linkage_model.py):
+ *   Clusters occupy slots; leaf i starts in slot i.  While more than one slot is live, the least (D(a, b), b, a) over live slots
+ *   a < b is merged (ties go to the first pair of the lower triangle in row-major order).  Merge s makes node u = n + s with
+ *   height D(a, b) and size n_a + n_b; u takes slot a, slot b dies, and for every other live k
+ *     average:  D(u, k) = ((double)n_a * D(a, k) + (double)n_b * D(b, k)) / (double)(n_a + n_b)
+ *     complete: D(u, k) = max(D(a, k), D(b, k)) (D(a, k) when they are equal).
+ * Every step is one IEEE double operation, never fused.  Heights are returned as computed: rounding in the average can make a
+ * later height smaller than an earlier one by an ulp.  The average is the size-weighted mean of scipy's `average` method, but scipy
+ * merges in another order, so its values may differ in the last bits.
+ * Outputs of n - 1 entries in merge order, scipy's Z layout (scipy.cluster.hierarchy.fcluster, cophenet and dendrogram take it
+ * unchanged): id_lo[s] < id_hi[s] the merged node ids (0..n-1 the leaves), height[s], size[s] the leaves under n + s.
+ * rows_rescanned (may be NULL): the rows whose nearest-neighbour cache was rebuilt, which is what the device work scales with
+ * beyond its O(n) per merge.  Memory: the matrix plus O(n). */
+#define MASHGPU_LINKAGE_AVERAGE 0
+#define MASHGPU_LINKAGE_COMPLETE 1
+/* Linkage over the caller's n x n float64 device matrix (row i at d_matrix + i * ld, ld >= n; lower triangle read; the matrix is
+ * used as scratch and overwritten, columns past n are neither read nor written).  Host outputs of n - 1 entries; synchronises
+ * `stream` (NULL: the context's stream).  n < 2, ld < n, NULL outputs, a method other than the two above, or a non-finite entry in
+ * the lower triangle: MASHGPU_ERR_INVALID (the entry is found on the device before the first merge). */
+int mashgpu_linkage_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64_t n, uint64_t ld, int method, uint32_t *id_lo, uint32_t *id_hi,
+                           double *height, uint32_t *size, uint64_t *rows_rescanned, void *stream);
+/* Linkage over every pair's distance of a self job (qry == NULL): D(i, j), j < i, is the distance mashgpu_dist_run returns for
+ * (q = i, r = j), whatever max_distance, max_pvalue and mashgpu_dist_set_triangle say (none of them is changed); pairs without a
+ * shared hash have distance 1.  The job fills an n x n device matrix with its own runs, then runs mashgpu_linkage_matrix on it.
+ * n_qry < 2, a job with a separate query set, NULL outputs or an unknown method: MASHGPU_ERR_INVALID.  Encoded (sharded) jobs:
+ * MASHGPU_ERR_UNSUPPORTED.  8 n^2 bytes beyond the device's free memory: MASHGPU_ERR_NOMEM before anything is allocated. */
+int mashgpu_dist_linkage(mashgpu_dist_job *job, int method, uint32_t *id_lo, uint32_t *id_hi, double *height, uint32_t *size,
+                         uint64_t *rows_rescanned);
+
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE
  * instead (a sample sort): a rank sorts only its own rows' hashes, the sorted keys are cut at G-1 splitters, every rank

@@ -130,6 +130,8 @@ def load_library():
                                                    u64p, u64p, C.c_void_p]
     L.mashgpu_dist_neighbor_joining.argtypes = [C.c_void_p, u32p, f64p]
     L.mashgpu_neighbor_joining_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, u32p, f64p, C.c_void_p]
+    L.mashgpu_dist_linkage.argtypes = [C.c_void_p, C.c_int, u32p, u32p, f64p, u32p, u64p]
+    L.mashgpu_linkage_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, u32p, u32p, f64p, u32p, u64p, C.c_void_p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
     L.mashgpu_within_run.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, u32p, u32p, f64p, f64p, u8p]
@@ -164,6 +166,34 @@ def load_library():
 
 def _p(a, t):
     return a.ctypes.data_as(t) if a is not None else None
+
+
+LINKAGE_METHODS = {"average": 0, "complete": 1}
+
+
+def _linkage_method(method):
+    """a method name, or a raw integer passed through as is (the C ABI refuses unknown values)"""
+    if isinstance(method, str):
+        if method not in LINKAGE_METHODS:
+            raise ValueError(f"linkage method must be one of {sorted(LINKAGE_METHODS)}, not {method!r}")
+        return LINKAGE_METHODS[method]
+    return int(method)
+
+
+def _linkage_outputs(n):
+    m = max(int(n) - 1, 0)
+    return {"id_lo": np.zeros(m, np.uint32), "id_hi": np.zeros(m, np.uint32), "height": np.zeros(m, np.float64),
+            "size": np.zeros(m, np.uint32)}
+
+
+def _linkage_pointers(out):
+    return _p(out["id_lo"], u32p), _p(out["id_hi"], u32p), _p(out["height"], f64p), _p(out["size"], u32p)
+
+
+def linkage_z(merges):
+    """the (n - 1, 4) float64 Z of scipy.cluster.hierarchy from the merges of linkage() / linkage_matrix()"""
+    return np.column_stack([merges["id_lo"].astype(np.float64), merges["id_hi"].astype(np.float64), merges["height"],
+                            merges["size"].astype(np.float64)])
 
 
 def _as_u8(s):
@@ -365,6 +395,23 @@ class Engine:
                                                              _p(out["length"], f64p), stream))
         return out
 
+    def linkage_matrix(self, d_matrix, n, ld=None, method="average", stream=None):
+        """Average or complete linkage (DESIGN.md 3.11) of the n x n float64 matrix in the CUDA tensor d_matrix (row i at element
+        i * ld; ld defaults to the row stride of a 2-D tensor, else n).  Only the lower triangle is read, and the first n columns of
+        every row are overwritten.  Returns the n - 1 merges in merge order, scipy's Z layout: {"id_lo": uint32, "id_hi": uint32,
+        "height": float64, "size": uint32, "rows_rescanned": int}; linkage_z() makes the (n - 1, 4) Z of it."""
+        if not getattr(d_matrix, "is_cuda", False) or str(d_matrix.dtype) != "torch.float64":
+            raise ValueError("d_matrix must be a CUDA float64 tensor")
+        if ld is None:
+            ld = d_matrix.stride(0) if d_matrix.dim() == 2 else n
+        if n >= 1 and (n - 1) * ld + n > d_matrix.numel():
+            raise ValueError(f"d_matrix holds {d_matrix.numel()} elements, fewer than an {n} x {n} matrix with ld {ld}")
+        out, rows = _linkage_outputs(n), C.c_uint64(0)
+        self._check(self.lib.mashgpu_linkage_matrix(self.h, d_matrix.data_ptr(), int(n), int(ld), _linkage_method(method),
+                                                    *_linkage_pointers(out), C.byref(rows), stream))
+        out["rows_rescanned"] = rows.value
+        return out
+
     # ---- sharded dictionary build (device pointers; see mash_b200/shard.py) ----------------------------------
     def dict_local_sort(self, d_hashes, d_n_hashes, n, stride, sketch_size, d_keys, d_slots, stream=None):
         st = SketchSet(n, stride, d_hashes, d_n_hashes, None, 1)
@@ -541,6 +588,15 @@ class DistJob:
         m = max(2 * self.n_qry - 2, 0)
         out = {"parent": np.zeros(m, np.uint32), "length": np.zeros(m, np.float64)}
         self.eng._check(self.eng.lib.mashgpu_dist_neighbor_joining(self.h, _p(out["parent"], u32p), _p(out["length"], f64p)))
+        return out
+
+    def linkage(self, method="average"):
+        """Average or complete linkage (DESIGN.md 3.11) of every pair's distance of a self job, D(i, j) = run()'s distance at
+        (q = i, r = j), j < i, whatever max_distance, max_pvalue and set_triangle say: the merges as Engine.linkage_matrix returns
+        them.  At least 2 sketches; encoded jobs are refused."""
+        out, rows = _linkage_outputs(self.n_qry), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_linkage(self.h, _linkage_method(method), *_linkage_pointers(out), C.byref(rows)))
+        out["rows_rescanned"] = rows.value
         return out
 
     def set_prefilter(self, mode):

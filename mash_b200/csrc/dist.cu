@@ -24,8 +24,8 @@
 // of every hit of the lower triangle into a forest, whose roots become the components' labels.
 // A spanning-forest run (mashgpu_dist_spanning_forest, DESIGN.md 3.9) repeats such runs in Boruvka rounds: at the same places
 // dist_msf.cuh offers every hit to the cheapest-edge slots of its two components.
-// Neighbor joining (mashgpu_dist_neighbor_joining, DESIGN.md 3.10) fills an n x n matrix with plain lower-triangle runs (distance
-// output only) and hands it to nj.cu.
+// Neighbor joining (mashgpu_dist_neighbor_joining, DESIGN.md 3.10) and average / complete linkage (mashgpu_dist_linkage, 3.11)
+// fill an n x n matrix with plain lower-triangle runs (distance output only) and hand it to nj.cu or linkage.cu.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -1740,30 +1740,51 @@ extern "C" int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// Neighbor joining over a self job's distances (DESIGN.md 3.10; the joins are in nj.cu)
+// Trees over every pair's distance of a self job: neighbor joining (DESIGN.md 3.10; the joins are in nj.cu) and average /
+// complete linkage (DESIGN.md 3.11; the merges are in linkage.cu)
 // ---------------------------------------------------------------------------------------------------------
-extern "C" int mashgpu_dist_neighbor_joining(mashgpu_dist_job *job, uint32_t *parent, double *length)
+// The n x n matrix of a self job's distances, lower triangle filled (row q at matrix + q * n), for `what` of at least min_n
+// sketches.  outputs = the caller's outputs are all non-NULL.  8 n^2 bytes beyond the free device memory are refused before
+// anything is allocated.
+static int fill_distance_matrix(mashgpu_dist_job *job, const char *what, uint64_t min_n, bool outputs, DevBuf<double> &matrix)
 {
-    if (!job) return MASHGPU_ERR_INVALID;
     mashgpu_ctx *ctx = job->ctx;
-    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "neighbor joining of an encoded (sharded) job");
-    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining needs a self comparison (qry == NULL)");
-    if (!parent || !length) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "%s of an encoded (sharded) job", what);
+    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "%s needs a self comparison (qry == NULL)", what);
+    if (!outputs) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     const uint64_t n = job->n_qry;
-    if (n < 3) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining needs at least 3 sketches (got %llu)", (unsigned long long)n);
+    if (n < min_n) return fail(ctx, MASHGPU_ERR_INVALID, "%s needs at least %llu sketches (got %llu)", what, (unsigned long long)min_n, (unsigned long long)n);
     MG_CUDA(ctx, cudaSetDevice(ctx->device));
     size_t free_b = 0, total_b = 0;
     MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
     if ((double)n * (double)n * 8.0 > (double)free_b)
         return fail(ctx, MASHGPU_ERR_NOMEM, "a %llu x %llu distance matrix needs %.3g GB, the device has %.3g GB free", (unsigned long long)n,
                     (unsigned long long)n, (double)n * (double)n * 8e-9, (double)free_b * 1e-9);
-    DevBuf<double> matrix;
     if (matrix.alloc(n * n) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu x %llu distance matrix)", (unsigned long long)n, (unsigned long long)n);
-    cudaStream_t st = ctx->stream;
-    // distance output only, row q at matrix + q * n; the lower triangle is all the joins read
-    MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) { a.distance = matrix.p + (uint64_t)a.q_begin * n; }));
-    return mashgpu_neighbor_joining_matrix(ctx, matrix.p, n, n, parent, length, st);
+    // distance output only; the lower triangle is all the trees read
+    return enqueue_lower_triangle(job, ctx->stream, [&](DistArgs &a) { a.distance = matrix.p + (uint64_t)a.q_begin * n; });
+}
+
+extern "C" int mashgpu_dist_neighbor_joining(mashgpu_dist_job *job, uint32_t *parent, double *length)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    DevBuf<double> matrix;
+    MG_TRY(fill_distance_matrix(job, "neighbor joining", 3, parent && length, matrix));
+    const uint64_t n = job->n_qry;
+    return mashgpu_neighbor_joining_matrix(job->ctx, matrix.p, n, n, parent, length, job->ctx->stream);
+}
+
+extern "C" int mashgpu_dist_linkage(mashgpu_dist_job *job, int method, uint32_t *id_lo, uint32_t *id_hi, double *height, uint32_t *size,
+                                    uint64_t *rows_rescanned)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    if (method != MASHGPU_LINKAGE_AVERAGE && method != MASHGPU_LINKAGE_COMPLETE)
+        return fail(job->ctx, MASHGPU_ERR_INVALID, "unknown linkage method %d", method);
+    DevBuf<double> matrix;
+    MG_TRY(fill_distance_matrix(job, "linkage", 2, id_lo && id_hi && height && size, matrix));
+    const uint64_t n = job->n_qry;
+    return mashgpu_linkage_matrix(job->ctx, matrix.p, n, n, method, id_lo, id_hi, height, size, rows_rescanned, job->ctx->stream);
 }
 
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)

@@ -6,8 +6,8 @@
 // nvcc never contracts into an FMA; the one division per join (of the branch lengths) is done on the host from the join records.
 // Per step the host only enqueues two kernels; nothing is read back until the end.
 //
-// Matrix: the caller's n x ld array.  nj_mirror_kernel copies the lower triangle to the upper one and zeroes the diagonal, so
-// that every live row holds all live columns and the join writes a row and a column.  Rows never move: row slot a stays the row
+// Matrix: the caller's n x ld array.  nj_mirror_kernel (dense.cuh) copies the lower triangle to the upper one and zeroes the
+// diagonal, so that every live row holds all live columns and the join writes a row and a column.  Rows never move: row slot a stays the row
 // of the node at that position (a join puts u into the slot of a, the smaller position).  The live positions are kept as lists of
 // row slot, column index, node id and row sum, in position order (double-buffered, rewritten by each join).  Columns are
 // compacted in place, row by row, whenever the live count falls to 3/4 of the column span, so a scan reads at most 4/3 of the
@@ -17,80 +17,17 @@
 #include <vector>
 
 #include "common.cuh"
+#include "dense.cuh"
 
 namespace mashgpu {
 namespace {
 
-constexpr unsigned NJ_THREADS = 256;
 constexpr uint32_t NJ_NONE = 0xFFFFFFFFu;
-constexpr unsigned long long NJ_NO_KEY = ~0ull;
 
-struct NjBest { double q; unsigned long long key; };    // key = q << 32 | p (positions, p < q)
 struct NjJoin { uint32_t a, b; double dab, diff; };     // join s: node ids of a and b, D(a, b) and r_a - r_b
 struct NjLast { uint32_t id[3]; double len[3]; };       // the last three nodes and their branches
 
 unsigned nj_blocks(uint64_t n, unsigned tb = NJ_THREADS) { return (unsigned)std::max<uint64_t>(1, (n + tb - 1) / tb); }
-
-// strict total order on (Q, q, p); a NaN Q is never before anything
-__device__ __forceinline__ bool nj_before(double q1, unsigned long long k1, double q2, unsigned long long k2)
-{
-    return q1 < q2 || (q1 == q2 && k1 < k2);
-}
-
-__device__ __forceinline__ void nj_warp_min(double &q, unsigned long long &k)
-{
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const double q2 = __shfl_xor_sync(0xFFFFFFFFu, q, o);
-        const unsigned long long k2 = __shfl_xor_sync(0xFFFFFFFFu, k, o);
-        if (nj_before(q2, k2, q, k)) { q = q2; k = k2; }
-    }
-}
-
-// the minimum over the block, returned to every thread
-__device__ NjBest nj_block_min(double q, unsigned long long k)
-{
-    __shared__ double sq[NJ_THREADS / 32];
-    __shared__ unsigned long long sk[NJ_THREADS / 32];
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    nj_warp_min(q, k);
-    if (lane == 0) { sq[warp] = q; sk[warp] = k; }
-    __syncthreads();
-    if (warp == 0) {
-        q = lane < NJ_THREADS / 32 ? sq[lane] : __longlong_as_double(0x7FF0000000000000ll);
-        k = lane < NJ_THREADS / 32 ? sk[lane] : NJ_NO_KEY;
-        nj_warp_min(q, k);
-        if (lane == 0) { sq[0] = q; sk[0] = k; }
-    }
-    __syncthreads();
-    return NjBest{sq[0], sk[0]};
-}
-
-// Lower triangle -> upper triangle through 32 x 32 tiles in shared memory, diagonal := 0, and the finiteness test of every
-// lower-triangle entry.  Grid (tiles, tiles); tiles above the diagonal exit.  Upper entries are only written and lower ones only
-// read, so tiles need no ordering.
-__global__ void __launch_bounds__(256) nj_mirror_kernel(double *D, uint64_t ld, uint32_t n, int *nonfinite)
-{
-    __shared__ double t[32][33];
-    const uint32_t bi = blockIdx.y, bj = blockIdx.x;
-    if (bj > bi) return;
-    const uint32_t i0 = bi * 32, j0 = bj * 32, x = threadIdx.x;
-    bool bad = false;
-    for (uint32_t y = threadIdx.y; y < 32; y += 8) {
-        const uint32_t i = i0 + y, j = j0 + x;
-        if (i < n && j < i) {
-            const double v = D[(uint64_t)i * ld + j];
-            t[y][x] = v;
-            bad |= !isfinite(v);
-        }
-    }
-    if (__syncthreads_or(bad) && x == 0 && threadIdx.y == 0) *nonfinite = 1;
-    for (uint32_t y = threadIdx.y; y < 32; y += 8) {         // upper entry (r, c), r < c, is D(c, r) = t[x][y]
-        const uint32_t r = j0 + y, c = i0 + x;
-        if (c < n && r < c) D[(uint64_t)r * ld + c] = t[x][y];
-        else if (c < n && r == c) D[(uint64_t)r * ld + c] = 0.0;
-    }
-}
 
 // r_i = sum over ascending k of D(i, k), the diagonal's 0 included; thread i walks column i, so a warp reads 32 adjacent doubles
 __global__ void __launch_bounds__(64) nj_rowsum_kernel(const double *__restrict__ D, uint64_t ld, uint32_t n, double *r)

@@ -5,7 +5,8 @@
 // precision), same ordering contracts.  It exists so that the reference's `make test` flow can be replayed against the GPU engine;
 // help text, `bounds` and `find` are out of scope.  `triangle -G` (clusters) and `triangle -T` (the single-linkage tree as a minimum
 // spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.  Nor has `triangle -N` (the
-// neighbor-joining tree as a Newick line), which its users compute from the matrix with an NJ program.
+// neighbor-joining tree as a Newick line), which its users compute from the matrix with an NJ program, nor `triangle -L` (average
+// or complete linkage as a Newick line, or its flat clusters at `-d`), which its users compute from the matrix with scipy.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -567,6 +568,57 @@ static void writeNeighborJoining(mashgpu_dist_job *job, const Sketch &sketch, bo
     cerr << "Tree: " << n << " leaves, " << (n > 3 ? n - 3 : 0) << " joins" << endl;
 }
 
+// `mash triangle -L average|complete`: average (UPGMA) or complete linkage of every pair's distance (DESIGN.md 3.11), merged on the
+// device.  Without -d, the rooted tree as one Newick line: a merge's node sits at half its height, leaves at 0, and a branch is the
+// parent's height minus the child's.  With -d t, per sketch its flat cluster at t in -G's format: scipy's fcluster(Z, t, "distance"),
+// a maximal subtree whose every merge has height <= t (the largest height in it, since rounding in the average can make a later
+// merge lower by an ulp), numbered from 0 in the order of their first member.  One sketch has no merge: its name, or cluster 0.
+static void writeLinkage(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int method, bool cutting, double t, int threads)
+{
+    const uint64_t n = sketch.getReferenceCount(), m = n ? n - 1 : 0, nodes = n + m;
+    vector<uint32_t> lo(m), hi(m), size(m);
+    vector<double> height(m);
+    uint64_t rows = 0;
+    if (n > 1 && mashgpu_dist_linkage(job, method, lo.data(), hi.data(), height.data(), size.data(), &rows) != MASHGPU_OK) gpuFail();
+    if (cutting) {
+        vector<double> worst(nodes, 0.0);                  // the largest merge height in each node's subtree
+        for (uint64_t s = 0; s < m; s++) worst[n + s] = std::max(height[s], std::max(worst[lo[s]], worst[hi[s]]));
+        vector<uint64_t> top(nodes);                       // the root of each node's flat cluster, assigned from the root down
+        if (nodes) top[nodes - 1] = nodes - 1;
+        for (uint64_t s = m; s-- > 0;) {
+            const uint64_t u = n + s;
+            top[lo[s]] = worst[u] <= t ? top[u] : lo[s];
+            top[hi[s]] = worst[u] <= t ? top[u] : hi[s];
+        }
+        vector<uint32_t> number(nodes, UINT32_MAX), cluster(n);
+        uint32_t clusters = 0;
+        for (uint64_t i = 0; i < n; i++) cluster[i] = number[top[i]] == UINT32_MAX ? (number[top[i]] = clusters++) : number[top[i]];
+        mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
+            const Sketch::Reference &ref = sketch.getReference(i);
+            o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.u64(cluster[i]); o.ch('\n');
+        });
+        cerr << "Clusters: " << clusters << " at height <= " << t << endl;
+        return;
+    }
+    vector<string> names(n);
+    for (uint64_t i = 0; i < n; i++) names[i] = comment ? sketch.getReference(i).comment : sketch.getReference(i).name;
+    mashhost::OutBuf o;
+    if (n == 1) {
+        mashhost::newickName(o, names[0]); o.ch(';'); o.ch('\n');
+    } else if (n > 1) {
+        vector<uint32_t> parent(nodes, UINT32_MAX);
+        vector<double> length(nodes, 0.0);
+        auto nodeHeight = [&](uint64_t v) { return v < n ? 0.0 : height[v - n] * 0.5; };
+        for (uint64_t s = 0; s < m; s++) parent[lo[s]] = parent[hi[s]] = (uint32_t)(n + s);
+        for (uint64_t v = 0; v + 1 < nodes; v++) length[v] = nodeHeight(parent[v]) - nodeHeight(v);
+        mashhost::writeNewick(o, parent, length, names);    // its center, the last node, is the root 2n - 2
+    }
+    cout.flush();
+    fwrite(o.b.data(), 1, o.b.size(), stdout);
+    fflush(stdout);
+    cerr << "Tree: " << n << " leaves, " << m << " merges, " << rows << " rows rescanned" << endl;
+}
+
 int runTriangle(int argc, const char **argv)
 {
     Command c;
@@ -577,6 +629,7 @@ int runTriangle(int argc, const char **argv)
     c.add("cluster", Option(Option::Boolean, "G", ""));       // not an option of the reference: its users cluster the -E output
     c.add("tree", Option(Option::Boolean, "T", ""));          // not an option of the reference either
     c.add("nj", Option(Option::Boolean, "N", ""));            // nor is this one
+    c.add("linkage", Option(Option::String, "L", ""));        // nor this one
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.useSketchOptions();
@@ -586,14 +639,26 @@ int runTriangle(int argc, const char **argv)
              << "  -G        Clusters: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash (not with -E)." << endl
              << "  -T        Single-linkage tree: the minimum spanning forest of the -G graph by distance, as -E lines in order of distance (not with" << endl
              << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl
-             << "  -N        Neighbor-joining tree of every pair's distance, as one Newick line (not with -E, -G, -T, -d or -v)." << endl;
+             << "  -N        Neighbor-joining tree of every pair's distance, as one Newick line (not with -E, -G, -T, -d or -v)." << endl
+             << "  -L <m>    Average or complete linkage (m = average or complete) of every pair's distance as one Newick line; with -d t, per sketch its cluster at height <= t (not with -E, -G, -T, -N or -v)." << endl;
         return 0;
     }
     bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active, tree = c.opt("tree").active;
     if (cluster && edge) { cerr << "ERROR: The option -G cannot be used with -E (clusters replace the edge list)." << endl; return 1; }
     if (tree && edge) { cerr << "ERROR: The option -T cannot be used with -E (the forest replaces the edge list)." << endl; return 1; }
     if (tree && cluster) { cerr << "ERROR: The option -T cannot be used with -G (cut the forest at the distance instead)." << endl; return 1; }
-    const bool nj = c.opt("nj").active;
+    const bool nj = c.opt("nj").active, link = c.opt("linkage").active;
+    int linkMethod = -1;
+    if (link) {
+        const string &m = c.opt("linkage").argument;
+        linkMethod = m == "average" ? MASHGPU_LINKAGE_AVERAGE : m == "complete" ? MASHGPU_LINKAGE_COMPLETE : -1;
+        if (linkMethod < 0) { cerr << "ERROR: The argument to -L must be average or complete (" << m << " given)." << endl; return 1; }
+        for (const char *o : {"edge", "cluster", "tree", "nj", "pvalue"})
+            if (c.opt(o).active) {
+                cerr << "ERROR: The option -L cannot be used with -" << c.opt(o).identifier << " (the tree is built from every pair's distance; -d cuts it)." << endl;
+                return 1;
+            }
+    }
     if (nj) {
         for (const char *o : {"edge", "cluster", "tree", "distance", "pvalue"})
             if (c.opt(o).active) {
@@ -602,7 +667,7 @@ int runTriangle(int argc, const char **argv)
             }
     }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
-    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree) edge = true;
+    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree && !link) edge = true;
     Sketch::Parameters parameters;
     if (sketchParameterSetup(parameters, c)) return 1;
     if (c.arguments.size() == 1 && !c.opt("list").active) parameters.concatenated = false;
@@ -613,14 +678,17 @@ int runTriangle(int argc, const char **argv)
     KmerWarning w;
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
-    if (cluster || tree || nj) {
+    if (cluster || tree || nj || link) {
         mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
         mashgpu_sketch_set set;
         vector<uint64_t> h, l; vector<uint32_t> nn;
         sketch.toSketchSet(set, h, nn, l);
         mashgpu_dist_job *job = 0;
         if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
-        if (nj) writeNeighborJoining(job, sketch, comment);
+        // the cut is the -d argument read as a double, so that -d 0.1 cuts where fcluster(Z, 0.1, "distance") does (-d itself is a float)
+        if (link) writeLinkage(job, sketch, comment, linkMethod, c.opt("distance").active, strtod(c.opt("distance").argument.c_str(), nullptr),
+                               parameters.parallelism);
+        else if (nj) writeNeighborJoining(job, sketch, comment);
         else if (tree) writeForest(job, sketch, comment, parameters.parallelism);
         else writeClusters(job, sketch, comment, parameters.parallelism);
         mashgpu_dist_close(job);
