@@ -22,11 +22,13 @@ def assert_bits(got, want):
 
 
 def on_device(D, ld=None):
-    """D into a CUDA tensor of n rows of ld doubles (the columns past n hold junk that must not be read)"""
+    """D into a CUDA tensor of n rows of ld doubles (the columns past n hold junk that must not be read).  The engine runs on
+    its own stream, so torch's fill and copy are waited for."""
     n = len(D)
     ld = ld or n
     M = torch.full((n, ld), float("nan"), dtype=torch.float64, device="cuda")
     M[:, :n] = torch.from_numpy(np.ascontiguousarray(D, np.float64)).cuda()
+    torch.cuda.synchronize()
     return M
 
 
@@ -89,6 +91,7 @@ def test_additive_trees_are_recovered(gpu, kind, n):
     for i0 in range(0, n, 1024):
         rows = np.stack([tm.row(a) for a in range(i0, min(n, i0 + 1024))])
         M[i0:i0 + len(rows)] = torch.from_numpy(rows).cuda()
+    torch.cuda.synchronize()
     got = gpu.neighbor_joining_matrix(M, n)
     assert splits(got["parent"], got["length"], n) == splits(parent, length, n)
 
