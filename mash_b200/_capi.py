@@ -180,6 +180,16 @@ def _linkage_method(method):
     return int(method)
 
 
+def _matrix_ld(d_matrix, n, ld):
+    if not getattr(d_matrix, "is_cuda", False) or str(d_matrix.dtype) != "torch.float64":
+        raise ValueError("d_matrix must be a CUDA float64 tensor")
+    if ld is None:
+        ld = d_matrix.stride(0) if d_matrix.dim() == 2 else n
+    if n >= 1 and (n - 1) * ld + n > d_matrix.numel():
+        raise ValueError(f"d_matrix holds {d_matrix.numel()} elements, fewer than an {n} x {n} matrix with ld {ld}")
+    return int(ld)
+
+
 def _linkage_outputs(n):
     m = max(int(n) - 1, 0)
     return {"id_lo": np.zeros(m, np.uint32), "id_hi": np.zeros(m, np.uint32), "height": np.zeros(m, np.float64),
@@ -383,15 +393,10 @@ class Engine:
         ld defaults to the row stride of a 2-D tensor, else n).  Only the lower triangle is read, and the whole matrix is overwritten.
         Returns {"parent": uint32[2n - 2], "length": float64[2n - 2]}: leaves 0..n-1, join s makes node n + s, the center 2n - 3 has
         parent 0xFFFFFFFF and length 0."""
-        if not getattr(d_matrix, "is_cuda", False) or str(d_matrix.dtype) != "torch.float64":
-            raise ValueError("d_matrix must be a CUDA float64 tensor")
-        if ld is None:
-            ld = d_matrix.stride(0) if d_matrix.dim() == 2 else n
-        if n >= 1 and (n - 1) * ld + n > d_matrix.numel():
-            raise ValueError(f"d_matrix holds {d_matrix.numel()} elements, fewer than an {n} x {n} matrix with ld {ld}")
+        ld = _matrix_ld(d_matrix, n, ld)
         m = max(2 * int(n) - 2, 0)
         out = {"parent": np.zeros(m, np.uint32), "length": np.zeros(m, np.float64)}
-        self._check(self.lib.mashgpu_neighbor_joining_matrix(self.h, d_matrix.data_ptr(), int(n), int(ld), _p(out["parent"], u32p),
+        self._check(self.lib.mashgpu_neighbor_joining_matrix(self.h, d_matrix.data_ptr(), int(n), ld, _p(out["parent"], u32p),
                                                              _p(out["length"], f64p), stream))
         return out
 
@@ -400,14 +405,8 @@ class Engine:
         i * ld; ld defaults to the row stride of a 2-D tensor, else n).  Only the lower triangle is read, and the first n columns of
         every row are overwritten.  Returns the n - 1 merges in merge order, scipy's Z layout: {"id_lo": uint32, "id_hi": uint32,
         "height": float64, "size": uint32, "rows_rescanned": int}; linkage_z() makes the (n - 1, 4) Z of it."""
-        if not getattr(d_matrix, "is_cuda", False) or str(d_matrix.dtype) != "torch.float64":
-            raise ValueError("d_matrix must be a CUDA float64 tensor")
-        if ld is None:
-            ld = d_matrix.stride(0) if d_matrix.dim() == 2 else n
-        if n >= 1 and (n - 1) * ld + n > d_matrix.numel():
-            raise ValueError(f"d_matrix holds {d_matrix.numel()} elements, fewer than an {n} x {n} matrix with ld {ld}")
-        out, rows = _linkage_outputs(n), C.c_uint64(0)
-        self._check(self.lib.mashgpu_linkage_matrix(self.h, d_matrix.data_ptr(), int(n), int(ld), _linkage_method(method),
+        ld, out, rows = _matrix_ld(d_matrix, n, ld), _linkage_outputs(n), C.c_uint64(0)
+        self._check(self.lib.mashgpu_linkage_matrix(self.h, d_matrix.data_ptr(), int(n), ld, _linkage_method(method),
                                                     *_linkage_pointers(out), C.byref(rows), stream))
         out["rows_rescanned"] = rows.value
         return out

@@ -1580,9 +1580,15 @@ extern "C" int mashgpu_dist_run_best(mashgpu_dist_job *job, uint64_t q_begin, ui
 // ---------------------------------------------------------------------------------------------------------
 // Connected components (DESIGN.md 3.8)
 // ---------------------------------------------------------------------------------------------------------
-constexpr uint64_t CC_BLOCK_PAIRS = 1ull << 31;     // pairs of one run: bounds the work lists, the pair list and the p-value queue
+constexpr uint64_t TRIANGLE_RUN_PAIRS = 1ull << 31;     // pairs of one lower-triangle run: bounds its work lists, pair list and p-value queue
 
-// Runs every pair of the lower triangle of a self or encoded job once, in blocks of CC_BLOCK_PAIRS / n_ref queries, with the capture
+// components and spanning forests read the lower triangle of a self or encoded job; `what` starts the refusal
+static int need_self_or_encoded(mashgpu_dist_job *job, const char *what)
+{
+    return job->self || job->encoded ? MASHGPU_OK : fail(job->ctx, MASHGPU_ERR_INVALID, "%s a self comparison (qry == NULL) or an encoded job", what);
+}
+
+// Runs every pair of the lower triangle of a self or encoded job once, in blocks of TRIANGLE_RUN_PAIRS / n_ref queries, with the capture
 // that set_target puts into each run's arguments.  Lower triangle whatever the job's own setting: query q meets the rows below it
 // only, so the queries up to the first reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
 template <class SetTarget>
@@ -1590,7 +1596,7 @@ static int enqueue_lower_triangle(mashgpu_dist_job *job, cudaStream_t st, SetTar
 {
     const uint64_t n = job->n_qry, n_ref = job->n_ref;
     const uint64_t q_first = job->self ? 1 : job->ref_row0 + 1;
-    const uint64_t block = std::max<uint64_t>(1, CC_BLOCK_PAIRS / std::max<uint64_t>(n_ref, 1));
+    const uint64_t block = std::max<uint64_t>(1, TRIANGLE_RUN_PAIRS / std::max<uint64_t>(n_ref, 1));
     for (uint64_t q0 = q_first; n_ref && q0 < n; q0 += block) {
         DistArgs a = dist_args(job, q0, std::min(block, n - q0));
         a.triangle = 1;
@@ -1604,7 +1610,7 @@ extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_la
 {
     if (!job) return MASHGPU_ERR_INVALID;
     mashgpu_ctx *ctx = job->ctx;
-    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "components need a self comparison (qry == NULL) or an encoded job");
+    MG_TRY(need_self_or_encoded(job, "components need"));
     if (!d_labels || !n_edges) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     *n_edges = 0;
     const uint64_t n = job->n_qry;
@@ -1631,7 +1637,7 @@ extern "C" int mashgpu_dist_components(mashgpu_dist_job *job, uint32_t *labels, 
 {
     if (!job) return MASHGPU_ERR_INVALID;
     mashgpu_ctx *ctx = job->ctx;
-    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "components need a self comparison (qry == NULL) or an encoded job");
+    MG_TRY(need_self_or_encoded(job, "components need"));
     if (!labels || !n_edges) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     *n_edges = 0;
     const uint64_t n = job->n_qry;
@@ -1653,7 +1659,7 @@ extern "C" int mashgpu_dist_spanning_forest_dev(mashgpu_dist_job *job, uint32_t 
 {
     if (!job) return MASHGPU_ERR_INVALID;
     mashgpu_ctx *ctx = job->ctx;
-    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "a spanning forest needs a self comparison (qry == NULL) or an encoded job");
+    MG_TRY(need_self_or_encoded(job, "a spanning forest needs"));
     if (!d_row || !d_col || !d_numer || !d_denom || !d_distance || !d_pvalue || !n_edges || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     *n_edges = 0; *n_rounds = 0;
     const uint64_t n = job->n_qry;
@@ -1716,7 +1722,7 @@ extern "C" int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row
 {
     if (!job) return MASHGPU_ERR_INVALID;
     mashgpu_ctx *ctx = job->ctx;
-    if (!job->self && !job->encoded) return fail(ctx, MASHGPU_ERR_INVALID, "a spanning forest needs a self comparison (qry == NULL) or an encoded job");
+    MG_TRY(need_self_or_encoded(job, "a spanning forest needs"));
     if (!row || !col || !numer || !denom || !distance || !pvalue || !n_edges || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
     *n_edges = 0; *n_rounds = 0;
     const uint64_t n = job->n_qry;

@@ -8,29 +8,23 @@
 // row's cache is lowered to (D(i, a), a) or kept (lk_update_kernel).  The same rule is restated in tests/linkage_model.py, which
 // checks it against the naive global minimum.
 //
-// Matrix: the caller's n x ld array, mirrored by nj_mirror_kernel (dense.cuh) so that rows a and b hold every column.  A merge
+// Matrix: the caller's n x ld array, mirrored by dense_mirror_kernel (dense.cuh) so that rows a and b hold every column.  A merge
 // writes row a and column a; rows after b get NaN in column b, so a rescan of row i reads its i entries and skips dead ones (a
 // NaN is never before anything, and a live entry may be +inf: an average that overflowed is still a distance).  Row b is never
 // written.  Per merge the host enqueues three kernels and never synchronises; the merge records are copied back at the end.
 // Every device arithmetic step is one IEEE double operation (__dmul_rn, __dadd_rn, __ddiv_rn); __ddiv_rn is the correctly rounded
 // quotient, so the DFMAs of its Newton steps are the only ones in linkage.o.
-#include <algorithm>
-#include <cstdint>
 #include <vector>
 
-#include "common.cuh"
 #include "dense.cuh"
 
 namespace mashgpu {
 namespace {
 
-constexpr uint32_t LK_NONE = 0xFFFFFFFFu;
 constexpr unsigned LK_RESCAN_THREADS = 1024;    // one CTA per rescanned row: a row of n doubles in a few round trips
 
 struct LkMerge { double height; uint32_t lo, hi, size; };   // merge s, Z layout: node ids (smaller first), height, leaves
 struct LkStep { uint32_t a, b; };                           // the slots of the merge in flight
-
-unsigned lk_blocks(uint64_t n, unsigned tb = NJ_THREADS) { return (unsigned)std::max<uint64_t>(1, (n + tb - 1) / tb); }
 
 // slot i: a leaf of size 1, no cached neighbour, and on the rescan list (which therefore holds every row)
 __global__ void lk_init_kernel(double *cv, uint32_t *cj, uint8_t *alive, uint32_t *size, uint32_t *id, uint32_t *list, uint32_t *count,
@@ -40,7 +34,7 @@ __global__ void lk_init_kernel(double *cv, uint32_t *cj, uint8_t *alive, uint32_
     if (i == 0) *count = n;
     if (i >= n) return;
     cv[i] = __longlong_as_double(0x7FF0000000000000ll);
-    cj[i] = LK_NONE;
+    cj[i] = DENSE_NONE;
     alive[i] = 1;
     size[i] = 1;
     id[i] = list[i] = i;
@@ -48,18 +42,18 @@ __global__ void lk_init_kernel(double *cv, uint32_t *cj, uint8_t *alive, uint32_
 
 // The least (cache value, row) over the rows with a cached neighbour, one partial per CTA; key = row << 32 | neighbour.  Block 0
 // also empties the rescan list for this step's lk_update_kernel.
-__global__ void __launch_bounds__(NJ_THREADS) lk_argmin_kernel(const double *__restrict__ cv, const uint32_t *__restrict__ cj, uint32_t n,
-                                                               NjBest *partial, uint32_t *count)
+__global__ void __launch_bounds__(DENSE_THREADS) lk_argmin_kernel(const double *__restrict__ cv, const uint32_t *__restrict__ cj, uint32_t n,
+                                                                  DenseMin *partial, uint32_t *count)
 {
     if (blockIdx.x == 0 && threadIdx.x == 0) *count = 0;
     double bq = __longlong_as_double(0x7FF0000000000000ll);
-    unsigned long long bk = NJ_NO_KEY;
-    for (uint32_t i = blockIdx.x * NJ_THREADS + threadIdx.x; i < n; i += gridDim.x * NJ_THREADS) {
+    unsigned long long bk = DENSE_NO_KEY;
+    for (uint32_t i = blockIdx.x * DENSE_THREADS + threadIdx.x; i < n; i += gridDim.x * DENSE_THREADS) {
         const uint32_t j = cj[i];
         const unsigned long long key = (unsigned long long)i << 32 | j;
-        if (j != LK_NONE && nj_before(cv[i], key, bq, bk)) { bq = cv[i]; bk = key; }
+        if (j != DENSE_NONE && dense_before(cv[i], key, bq, bk)) { bq = cv[i]; bk = key; }
     }
-    const NjBest b = nj_block_min(bq, bk);
+    const DenseMin b = dense_block_min(bq, bk);
     if (threadIdx.x == 0) partial[blockIdx.x] = b;
 }
 
@@ -73,28 +67,22 @@ __global__ void __launch_bounds__(NJ_THREADS) lk_argmin_kernel(const double *__r
 // Thread a writes the merge record and puts row a on the list; thread b retires slot b.  Sizes and ids are only read here (the
 // rescan kernel updates slot a's), and no entry is touched by two threads.
 template <bool AVERAGE>
-__global__ void __launch_bounds__(NJ_THREADS) lk_update_kernel(double *D, uint64_t ld, const NjBest *__restrict__ partial, uint32_t n_partial,
-                                                               uint32_t n, double *cv, uint32_t *cj, uint8_t *alive,
-                                                               const uint32_t *__restrict__ size, const uint32_t *__restrict__ id,
-                                                               uint32_t *list, uint32_t *count, LkMerge *rec, LkStep *step, int *no_pair)
+__global__ void __launch_bounds__(DENSE_THREADS) lk_update_kernel(double *D, uint64_t ld, const DenseMin *__restrict__ partial, uint32_t n_partial,
+                                                                  uint32_t n, double *cv, uint32_t *cj, uint8_t *alive,
+                                                                  const uint32_t *__restrict__ size, const uint32_t *__restrict__ id,
+                                                                  uint32_t *list, uint32_t *count, LkMerge *rec, LkStep *step, int *no_pair)
 {
-    double bq = __longlong_as_double(0x7FF0000000000000ll);
-    unsigned long long bk = NJ_NO_KEY;
-    for (uint32_t t = threadIdx.x; t < n_partial; t += NJ_THREADS) {
-        const NjBest c = partial[t];
-        if (nj_before(c.q, c.key, bq, bk)) { bq = c.q; bk = c.key; }
-    }
-    const NjBest best = nj_block_min(bq, bk);
-    if (best.key == NJ_NO_KEY) {            // no row has a live neighbour with a comparable distance: the result is refused
+    const DenseMin best = dense_partials_min(partial, n_partial);
+    if (best.key == DENSE_NO_KEY) {         // no row has a live neighbour with a comparable distance: the result is refused
         if (blockIdx.x == 0 && threadIdx.x == 0) *no_pair = 1;
         return;
     }
     const uint32_t b = (uint32_t)(best.key >> 32), a = (uint32_t)best.key;
-    const uint32_t k = blockIdx.x * NJ_THREADS + threadIdx.x;
+    const uint32_t k = blockIdx.x * DENSE_THREADS + threadIdx.x;
     if (k >= n) return;
     if (k == b) {
         cv[b] = __longlong_as_double(0x7FF0000000000000ll);
-        cj[b] = LK_NONE;
+        cj[b] = DENSE_NONE;
         alive[b] = 0;
         return;
     }
@@ -121,7 +109,7 @@ __global__ void __launch_bounds__(NJ_THREADS) lk_update_kernel(double *D, uint64
     if (j == a || j == b) {
         if (v <= c) { cv[k] = v; cj[k] = a; }
         else list[atomicAdd(count, 1u)] = k;
-    } else if (nj_before(v, a, c, j)) {
+    } else if (dense_before(v, a, c, j)) {
         cv[k] = v; cj[k] = a;
     }
 }
@@ -145,7 +133,7 @@ __global__ void __launch_bounds__(LK_RESCAN_THREADS) lk_rescan_kernel(const doub
         const uint32_t i = list[r];
         const double *row = D + (uint64_t)i * ld;
         double bq = __longlong_as_double(0x7FF0000000000000ll);
-        unsigned long long bk = NJ_NO_KEY;
+        unsigned long long bk = DENSE_NO_KEY;
         uint32_t j = threadIdx.x;
         for (; j + 3 * T < i; j += 4 * T) {         // four independent loads in flight per thread
             double d[4];
@@ -153,14 +141,14 @@ __global__ void __launch_bounds__(LK_RESCAN_THREADS) lk_rescan_kernel(const doub
             for (int x = 0; x < 4; x++) d[x] = row[j + x * T];
 #pragma unroll
             for (int x = 0; x < 4; x++)
-                if (nj_before(d[x], j + x * T, bq, bk)) { bq = d[x]; bk = j + x * T; }
+                if (dense_before(d[x], j + x * T, bq, bk)) { bq = d[x]; bk = j + x * T; }
         }
         for (; j < i; j += T)
-            if (nj_before(row[j], j, bq, bk)) { bq = row[j]; bk = j; }
-        const NjBest b = nj_block_min<T>(bq, bk);
+            if (dense_before(row[j], j, bq, bk)) { bq = row[j]; bk = j; }
+        const DenseMin b = dense_block_min<T>(bq, bk);
         if (threadIdx.x == 0) {
-            cv[i] = b.key == NJ_NO_KEY ? __longlong_as_double(0x7FF0000000000000ll) : b.q;
-            cj[i] = b.key == NJ_NO_KEY ? LK_NONE : (uint32_t)b.key;
+            cv[i] = b.key == DENSE_NO_KEY ? __longlong_as_double(0x7FF0000000000000ll) : b.q;
+            cj[i] = b.key == DENSE_NO_KEY ? DENSE_NONE : (uint32_t)b.key;
         }
         __syncthreads();                            // the block minimum's shared slots are reused by the next row
     }
@@ -178,45 +166,34 @@ extern "C" int mashgpu_linkage_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64
     if (!d_matrix || !id_lo || !id_hi || !height || !size) return fail(ctx, MASHGPU_ERR_INVALID, "NULL argument");
     if (method != MASHGPU_LINKAGE_AVERAGE && method != MASHGPU_LINKAGE_COMPLETE)
         return fail(ctx, MASHGPU_ERR_INVALID, "unknown linkage method %d", method);
-    if (n < 2) return fail(ctx, MASHGPU_ERR_INVALID, "linkage needs at least 2 leaves (got %llu)", (unsigned long long)n);
-    if (ld < n) return fail(ctx, MASHGPU_ERR_INVALID, "leading dimension %llu below n = %llu", (unsigned long long)ld, (unsigned long long)n);
-    if (n >= 0x7FFFFFFFull) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "more than 2^31 - 1 leaves");
-    MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    cudaStream_t st;
+    MG_TRY(dense_begin(ctx, d_matrix, n, ld, 2, "linkage", stream, st));
     const uint32_t N = (uint32_t)n;
-    const uint32_t g = std::min<uint32_t>((uint32_t)ctx->sm_count * 8, lk_blocks(n));
+    const uint32_t g = std::min<uint32_t>((uint32_t)ctx->sm_count * 8, dense_blocks(n));
     const uint32_t rescan_grid = (uint32_t)ctx->sm_count * 2;
     // O(n) state: the caches (value, neighbour), liveness, sizes, ids, the rescan list, the argmin's partials, the merge records
-    DevBuf<double> cv; DevBuf<uint32_t> words; DevBuf<uint8_t> alive; DevBuf<NjBest> partial; DevBuf<LkMerge> d_rec; DevBuf<LkStep> d_step;
-    DevBuf<unsigned long long> d_rescanned; DevBuf<int> flags;
+    DevBuf<double> cv; DevBuf<uint32_t> words; DevBuf<uint8_t> alive; DevBuf<DenseMin> partial; DevBuf<LkMerge> d_rec; DevBuf<LkStep> d_step;
+    DevBuf<unsigned long long> d_rescanned; DevBuf<int> d_no_pair;
     if (cv.alloc(n) != cudaSuccess || words.alloc(4 * n + 1) != cudaSuccess || alive.alloc(n) != cudaSuccess || partial.alloc(g) != cudaSuccess ||
-        d_rec.alloc(n - 1) != cudaSuccess || d_step.alloc(1) != cudaSuccess || d_rescanned.alloc(1) != cudaSuccess || flags.alloc(2) != cudaSuccess)
+        d_rec.alloc(n - 1) != cudaSuccess || d_step.alloc(1) != cudaSuccess || d_rescanned.alloc(1) != cudaSuccess || d_no_pair.alloc(1) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (linkage state of %llu leaves)", (unsigned long long)n);
     uint32_t *cj = words.p, *sz = words.p + n, *id = words.p + 2 * n, *list = words.p + 3 * n, *count = words.p + 4 * n;
-    MG_CUDA(ctx, cudaMemsetAsync(flags.p, 0, 2 * sizeof(int), st));
+    MG_CUDA(ctx, cudaMemsetAsync(d_no_pair.p, 0, sizeof(int), st));
     MG_CUDA(ctx, cudaMemsetAsync(d_rescanned.p, 0, sizeof(unsigned long long), st));
-    const uint32_t tiles = (N + 31) / 32;
-    nj_mirror_kernel<<<dim3(tiles, tiles), dim3(32, 8), 0, st>>>(d_matrix, ld, N, flags.p);
-    MG_CUDA(ctx, cudaGetLastError());
-    int nonfinite = 0;
-    MG_CUDA(ctx, cudaMemcpyAsync(&nonfinite, flags.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    MG_CUDA(ctx, cudaStreamSynchronize(st));
-    ctx->kernel_launches++;
-    if (nonfinite) return fail(ctx, MASHGPU_ERR_INVALID, "the distance matrix has a NaN or infinite entry in its lower triangle");
-    lk_init_kernel<<<lk_blocks(n), NJ_THREADS, 0, st>>>(cv.p, cj, alive.p, sz, id, list, count, N);
+    lk_init_kernel<<<dense_blocks(n), DENSE_THREADS, 0, st>>>(cv.p, cj, alive.p, sz, id, list, count, N);
     lk_rescan_kernel<<<std::min<uint32_t>(N, ctx->sm_count * 16u), LK_RESCAN_THREADS, 0, st>>>(d_matrix, ld, list, count, cv.p, cj, nullptr, 0, sz,
                                                                                                id, d_rescanned.p);
     MG_CUDA(ctx, cudaGetLastError());
     ctx->kernel_launches += 2;
     const bool average = method == MASHGPU_LINKAGE_AVERAGE;
     for (uint32_t s = 0; s + 1 < N; s++) {
-        lk_argmin_kernel<<<g, NJ_THREADS, 0, st>>>(cv.p, cj, N, partial.p, count);
+        lk_argmin_kernel<<<g, DENSE_THREADS, 0, st>>>(cv.p, cj, N, partial.p, count);
         if (average)
-            lk_update_kernel<true><<<lk_blocks(n), NJ_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, N, cv.p, cj, alive.p, sz, id, list, count,
-                                                                       d_rec.p + s, d_step.p, flags.p + 1);
+            lk_update_kernel<true><<<dense_blocks(n), DENSE_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, N, cv.p, cj, alive.p, sz, id, list, count,
+                                                                          d_rec.p + s, d_step.p, d_no_pair.p);
         else
-            lk_update_kernel<false><<<lk_blocks(n), NJ_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, N, cv.p, cj, alive.p, sz, id, list, count,
-                                                                        d_rec.p + s, d_step.p, flags.p + 1);
+            lk_update_kernel<false><<<dense_blocks(n), DENSE_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, N, cv.p, cj, alive.p, sz, id, list, count,
+                                                                           d_rec.p + s, d_step.p, d_no_pair.p);
         lk_rescan_kernel<<<rescan_grid, LK_RESCAN_THREADS, 0, st>>>(d_matrix, ld, list, count, cv.p, cj, d_step.p, N + s, sz, id, d_rescanned.p);
         MG_CUDA(ctx, cudaGetLastError());
         ctx->kernel_launches += 3;
@@ -226,7 +203,7 @@ extern "C" int mashgpu_linkage_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64
     int no_pair = 0;
     MG_CUDA(ctx, cudaMemcpyAsync(rec.data(), d_rec.p, (n - 1) * sizeof(LkMerge), cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaMemcpyAsync(&rescanned, d_rescanned.p, sizeof(rescanned), cudaMemcpyDeviceToHost, st));
-    MG_CUDA(ctx, cudaMemcpyAsync(&no_pair, flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(&no_pair, d_no_pair.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     if (no_pair) return fail(ctx, MASHGPU_ERR_INVALID, "linkage found no pair with a comparable distance (an update overflowed)");
     for (uint64_t s = 0; s + 1 < n; s++) {

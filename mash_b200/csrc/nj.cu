@@ -6,28 +6,21 @@
 // nvcc never contracts into an FMA; the one division per join (of the branch lengths) is done on the host from the join records.
 // Per step the host only enqueues two kernels; nothing is read back until the end.
 //
-// Matrix: the caller's n x ld array.  nj_mirror_kernel (dense.cuh) copies the lower triangle to the upper one and zeroes the
+// Matrix: the caller's n x ld array.  dense_mirror_kernel (dense.cuh) copies the lower triangle to the upper one and zeroes the
 // diagonal, so that every live row holds all live columns and the join writes a row and a column.  Rows never move: row slot a stays the row
 // of the node at that position (a join puts u into the slot of a, the smaller position).  The live positions are kept as lists of
 // row slot, column index, node id and row sum, in position order (double-buffered, rewritten by each join).  Columns are
 // compacted in place, row by row, whenever the live count falls to 3/4 of the column span, so a scan reads at most 4/3 of the
 // live lower triangle's bytes (plus sector rounding) and never the full n x n.  Dead rows are skipped outright.
-#include <algorithm>
-#include <cstdint>
 #include <vector>
 
-#include "common.cuh"
 #include "dense.cuh"
 
 namespace mashgpu {
 namespace {
 
-constexpr uint32_t NJ_NONE = 0xFFFFFFFFu;
-
 struct NjJoin { uint32_t a, b; double dab, diff; };     // join s: node ids of a and b, D(a, b) and r_a - r_b
 struct NjLast { uint32_t id[3]; double len[3]; };       // the last three nodes and their branches
-
-unsigned nj_blocks(uint64_t n, unsigned tb = NJ_THREADS) { return (unsigned)std::max<uint64_t>(1, (n + tb - 1) / tb); }
 
 // r_i = sum over ascending k of D(i, k), the diagonal's 0 included; thread i walks column i, so a warp reads 32 adjacent doubles
 __global__ void __launch_bounds__(64) nj_rowsum_kernel(const double *__restrict__ D, uint64_t ld, uint32_t n, double *r)
@@ -51,12 +44,12 @@ __global__ void nj_init_kernel(uint32_t *rs, uint32_t *cs, uint32_t *id, uint32_
 // Moves the live columns of every live row to their positions: row rs[k], column cs[p] -> column p.  cs is ascending, so
 // cs[p] >= p: a chunk of positions reads only columns at or after its own start, and later chunks only columns after its end.
 // One barrier between a chunk's reads and its writes is all the ordering needed.  Rows are independent.
-__global__ void __launch_bounds__(NJ_THREADS) nj_compact_kernel(double *D, uint64_t ld, const uint32_t *__restrict__ rs,
-                                                                const uint32_t *__restrict__ cs, uint32_t m)
+__global__ void __launch_bounds__(DENSE_THREADS) nj_compact_kernel(double *D, uint64_t ld, const uint32_t *__restrict__ rs,
+                                                                   const uint32_t *__restrict__ cs, uint32_t m)
 {
     for (uint32_t k = blockIdx.x; k < m; k += gridDim.x) {
         double *row = D + (uint64_t)rs[k] * ld;
-        for (uint32_t c0 = 0; c0 < m; c0 += NJ_THREADS) {
+        for (uint32_t c0 = 0; c0 < m; c0 += DENSE_THREADS) {
             const uint32_t p = c0 + threadIdx.x;
             const double v = p < m ? row[cs[p]] : 0.0;
             __syncthreads();
@@ -74,16 +67,16 @@ __global__ void nj_iota_kernel(uint32_t *v, uint32_t m)
 // One warp per item of two rows (q = 1 + it and q = m - 1 - it: m positions per item), grid-stride.  Q is never stored: each lane
 // keeps its least (Q, q, p) and the block writes one partial.
 //   Q(p, q) = ((m - 2) * D(a, b) - r_a) - r_b,  a = L[p], b = L[q], p < q
-__global__ void __launch_bounds__(NJ_THREADS) nj_scan_kernel(const double *__restrict__ D, uint64_t ld, const uint32_t *__restrict__ rs,
-                                                             const uint32_t *__restrict__ cs, const double *__restrict__ r, uint32_t m,
-                                                             NjBest *partial)
+__global__ void __launch_bounds__(DENSE_THREADS) nj_scan_kernel(const double *__restrict__ D, uint64_t ld, const uint32_t *__restrict__ rs,
+                                                                const uint32_t *__restrict__ cs, const double *__restrict__ r, uint32_t m,
+                                                                DenseMin *partial)
 {
     const double mm2 = (double)(m - 2);
     double bq = __longlong_as_double(0x7FF0000000000000ll);
-    unsigned long long bk = NJ_NO_KEY;
+    unsigned long long bk = DENSE_NO_KEY;
     const uint32_t lane = threadIdx.x & 31, items = m / 2;
-    const uint32_t warps = (gridDim.x * NJ_THREADS) >> 5;
-    for (uint32_t it = (blockIdx.x * NJ_THREADS + threadIdx.x) >> 5; it < items; it += warps) {
+    const uint32_t warps = (gridDim.x * DENSE_THREADS) >> 5;
+    for (uint32_t it = (blockIdx.x * DENSE_THREADS + threadIdx.x) >> 5; it < items; it += warps) {
         for (int h = 0; h < 2; h++) {
             const uint32_t q = h ? m - 1 - it : it + 1;
             if (h && q == it + 1) break;
@@ -98,16 +91,16 @@ __global__ void __launch_bounds__(NJ_THREADS) nj_scan_kernel(const double *__res
 #pragma unroll
                 for (int u = 0; u < 4; u++) {
                     const double Q = __dsub_rn(__dsub_rn(__dmul_rn(mm2, d[u]), rp[u]), rq);
-                    if (nj_before(Q, kq | (p + 32 * u), bq, bk)) { bq = Q; bk = kq | (p + 32 * u); }
+                    if (dense_before(Q, kq | (p + 32 * u), bq, bk)) { bq = Q; bk = kq | (p + 32 * u); }
                 }
             }
             for (; p < q; p += 32) {
                 const double Q = __dsub_rn(__dsub_rn(__dmul_rn(mm2, row[cs[p]]), r[p]), rq);
-                if (nj_before(Q, kq | p, bq, bk)) { bq = Q; bk = kq | p; }
+                if (dense_before(Q, kq | p, bq, bk)) { bq = Q; bk = kq | p; }
             }
         }
     }
-    const NjBest b = nj_block_min(bq, bk);
+    const DenseMin b = dense_block_min(bq, bk);
     if (threadIdx.x == 0) partial[blockIdx.x] = b;
 }
 
@@ -119,24 +112,18 @@ __global__ void __launch_bounds__(NJ_THREADS) nj_scan_kernel(const double *__res
 // does when it reads the records back (nj_tree), so no device arithmetic of the joins is a DFMA.  Thread k reads row a and row b
 // at column cs[k] and writes row a at cs[k] and row rs[k] at cs[p]; no other thread touches those entries, and D(a, b) (row b) is
 // not written.
-__global__ void __launch_bounds__(NJ_THREADS) nj_join_kernel(double *D, uint64_t ld, const NjBest *__restrict__ partial, uint32_t n_partial,
-                                                             uint32_t m, uint32_t u, const uint32_t *__restrict__ rs, const uint32_t *__restrict__ cs,
-                                                             const uint32_t *__restrict__ id, const double *__restrict__ r, uint32_t *rs2,
-                                                             uint32_t *cs2, uint32_t *id2, double *r2, NjJoin *rec, int *no_pair)
+__global__ void __launch_bounds__(DENSE_THREADS) nj_join_kernel(double *D, uint64_t ld, const DenseMin *__restrict__ partial, uint32_t n_partial,
+                                                                uint32_t m, uint32_t u, const uint32_t *__restrict__ rs, const uint32_t *__restrict__ cs,
+                                                                const uint32_t *__restrict__ id, const double *__restrict__ r, uint32_t *rs2,
+                                                                uint32_t *cs2, uint32_t *id2, double *r2, NjJoin *rec, int *no_pair)
 {
-    double bq = __longlong_as_double(0x7FF0000000000000ll);
-    unsigned long long bk = NJ_NO_KEY;
-    for (uint32_t t = threadIdx.x; t < n_partial; t += NJ_THREADS) {
-        const NjBest c = partial[t];
-        if (nj_before(c.q, c.key, bq, bk)) { bq = c.q; bk = c.key; }
-    }
-    const NjBest best = nj_block_min(bq, bk);
-    if (best.key == NJ_NO_KEY) {            // every Q was NaN (sums that overflowed): the result is refused
+    const DenseMin best = dense_partials_min(partial, n_partial);
+    if (best.key == DENSE_NO_KEY) {         // every Q was NaN (sums that overflowed): the result is refused
         if (blockIdx.x == 0 && threadIdx.x == 0) *no_pair = 1;
         return;
     }
     const uint32_t p = (uint32_t)best.key, q = (uint32_t)(best.key >> 32);
-    const uint32_t k = blockIdx.x * NJ_THREADS + threadIdx.x;
+    const uint32_t k = blockIdx.x * DENSE_THREADS + threadIdx.x;
     if (k >= m || k == q) return;
     const uint32_t a = rs[p], ca = cs[p];
     double *row_a = D + (uint64_t)a * ld;
@@ -177,46 +164,35 @@ extern "C" int mashgpu_neighbor_joining_matrix(mashgpu_ctx *ctx, double *d_matri
 {
     if (!ctx) return MASHGPU_ERR_INVALID;
     if (!d_matrix || !parent || !length) return fail(ctx, MASHGPU_ERR_INVALID, "NULL argument");
-    if (n < 3) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining needs at least 3 leaves (got %llu)", (unsigned long long)n);
-    if (ld < n) return fail(ctx, MASHGPU_ERR_INVALID, "leading dimension %llu below n = %llu", (unsigned long long)ld, (unsigned long long)n);
-    if (n >= 0x7FFFFFFFull) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "more than 2^31 - 1 leaves");
-    MG_CUDA(ctx, cudaSetDevice(ctx->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    cudaStream_t st;
+    MG_TRY(dense_begin(ctx, d_matrix, n, ld, 3, "neighbor joining", stream, st));
     const uint32_t N = (uint32_t)n, nodes = 2 * N - 2;
     const uint32_t max_partials = (uint32_t)ctx->sm_count * 8;
-    // O(n) state: two buffers of the position lists (slot, column, node id; row sums), the join records, the scan's partials, two flags
-    DevBuf<uint32_t> lists; DevBuf<double> sums; DevBuf<NjJoin> d_rec; DevBuf<NjLast> d_last; DevBuf<NjBest> partial; DevBuf<int> flags;
+    // O(n) state: two buffers of the position lists (slot, column, node id; row sums), the join records, the scan's partials, a flag
+    DevBuf<uint32_t> lists; DevBuf<double> sums; DevBuf<NjJoin> d_rec; DevBuf<NjLast> d_last; DevBuf<DenseMin> partial; DevBuf<int> d_no_pair;
     if (lists.alloc(6ull * n) != cudaSuccess || sums.alloc(2ull * n) != cudaSuccess || d_rec.alloc(n - 3) != cudaSuccess ||
-        d_last.alloc(1) != cudaSuccess || partial.alloc(max_partials) != cudaSuccess || flags.alloc(2) != cudaSuccess)
+        d_last.alloc(1) != cudaSuccess || partial.alloc(max_partials) != cudaSuccess || d_no_pair.alloc(1) != cudaSuccess)
         return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (neighbor joining state of %llu leaves)", (unsigned long long)n);
     uint32_t *rs[2] = {lists.p, lists.p + n}, *cs[2] = {lists.p + 2 * n, lists.p + 3 * n}, *id[2] = {lists.p + 4 * n, lists.p + 5 * n};
     double *r[2] = {sums.p, sums.p + n};
-    MG_CUDA(ctx, cudaMemsetAsync(flags.p, 0, 2 * sizeof(int), st));
-    const uint32_t tiles = (N + 31) / 32;
-    nj_mirror_kernel<<<dim3(tiles, tiles), dim3(32, 8), 0, st>>>(d_matrix, ld, N, flags.p);
-    MG_CUDA(ctx, cudaGetLastError());
-    int nonfinite = 0;
-    MG_CUDA(ctx, cudaMemcpyAsync(&nonfinite, flags.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    MG_CUDA(ctx, cudaStreamSynchronize(st));
-    ctx->kernel_launches++;
-    if (nonfinite) return fail(ctx, MASHGPU_ERR_INVALID, "the distance matrix has a NaN or infinite entry in its lower triangle");
-    nj_rowsum_kernel<<<nj_blocks(n, 64), 64, 0, st>>>(d_matrix, ld, N, r[0]);
-    nj_init_kernel<<<nj_blocks(n), NJ_THREADS, 0, st>>>(rs[0], cs[0], id[0], N);
+    MG_CUDA(ctx, cudaMemsetAsync(d_no_pair.p, 0, sizeof(int), st));
+    nj_rowsum_kernel<<<dense_blocks(n, 64), 64, 0, st>>>(d_matrix, ld, N, r[0]);
+    nj_init_kernel<<<dense_blocks(n), DENSE_THREADS, 0, st>>>(rs[0], cs[0], id[0], N);
     MG_CUDA(ctx, cudaGetLastError());
     ctx->kernel_launches += 2;
     uint32_t span = N;          // columns in use: [0, span)
     for (uint32_t s = 0; s + 3 < N; s++) {
         const uint32_t m = N - s, c = s & 1;
         if (4ull * m <= 3ull * span) {
-            nj_compact_kernel<<<std::min<uint32_t>(m, ctx->sm_count * 16u), NJ_THREADS, 0, st>>>(d_matrix, ld, rs[c], cs[c], m);
-            nj_iota_kernel<<<nj_blocks(m), NJ_THREADS, 0, st>>>(cs[c], m);
+            nj_compact_kernel<<<std::min<uint32_t>(m, ctx->sm_count * 16u), DENSE_THREADS, 0, st>>>(d_matrix, ld, rs[c], cs[c], m);
+            nj_iota_kernel<<<dense_blocks(m), DENSE_THREADS, 0, st>>>(cs[c], m);
             ctx->kernel_launches += 2;
             span = m;
         }
-        const uint32_t g = std::min<uint32_t>(max_partials, nj_blocks(m / 2, NJ_THREADS / 32));
-        nj_scan_kernel<<<g, NJ_THREADS, 0, st>>>(d_matrix, ld, rs[c], cs[c], r[c], m, partial.p);
-        nj_join_kernel<<<nj_blocks(m), NJ_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, m, N + s, rs[c], cs[c], id[c], r[c], rs[c ^ 1], cs[c ^ 1],
-                                                            id[c ^ 1], r[c ^ 1], d_rec.p + s, flags.p + 1);
+        const uint32_t g = std::min<uint32_t>(max_partials, dense_blocks(m / 2, DENSE_THREADS / 32));
+        nj_scan_kernel<<<g, DENSE_THREADS, 0, st>>>(d_matrix, ld, rs[c], cs[c], r[c], m, partial.p);
+        nj_join_kernel<<<dense_blocks(m), DENSE_THREADS, 0, st>>>(d_matrix, ld, partial.p, g, m, N + s, rs[c], cs[c], id[c], r[c], rs[c ^ 1], cs[c ^ 1],
+                                                               id[c ^ 1], r[c ^ 1], d_rec.p + s, d_no_pair.p);
         MG_CUDA(ctx, cudaGetLastError());
         ctx->kernel_launches += 2;
     }
@@ -229,7 +205,7 @@ extern "C" int mashgpu_neighbor_joining_matrix(mashgpu_ctx *ctx, double *d_matri
     int no_pair = 0;
     if (n > 3) MG_CUDA(ctx, cudaMemcpyAsync(rec.data(), d_rec.p, (n - 3) * sizeof(NjJoin), cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaMemcpyAsync(&last, d_last.p, sizeof(NjLast), cudaMemcpyDeviceToHost, st));
-    MG_CUDA(ctx, cudaMemcpyAsync(&no_pair, flags.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(&no_pair, d_no_pair.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     if (no_pair) return fail(ctx, MASHGPU_ERR_INVALID, "neighbor joining found no pair with a comparable Q (row sums overflowed)");
     // la = D(a, b) * 0.5 + (r_a - r_b) / (2 * (m - 2)), lb = D(a, b) - la: IEEE double operations in this order (x86-64 without FMA
@@ -242,7 +218,7 @@ extern "C" int mashgpu_neighbor_joining_matrix(mashgpu_ctx *ctx, double *d_matri
         length[j.b] = j.dab - la;
     }
     for (int i = 0; i < 3; i++) { parent[last.id[i]] = nodes - 1; length[last.id[i]] = last.len[i]; }
-    parent[nodes - 1] = NJ_NONE;
+    parent[nodes - 1] = DENSE_NONE;
     length[nodes - 1] = 0.0;
     return MASHGPU_OK;
 }

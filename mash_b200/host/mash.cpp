@@ -272,6 +272,17 @@ int runSketch(int argc, const char **argv)
 }
 
 // ---------------------------------------------------------------------------------------------------- dist
+// one line of dist's output (reference CommandDistance.cpp:247-304): reference, query (name:comment with -C) and the pair's values
+static void writePair(mashhost::OutBuf &o, const Sketch &sketchRef, uint64_t r, const Sketch &sketchQuery, uint64_t q, bool comment,
+                      double distance, double pValue, uint64_t numer, uint64_t denom)
+{
+    o.str(sketchRef.getReference(r).name);
+    if (comment) { o.ch(':'); o.str(sketchRef.getReference(r).comment); }
+    o.ch('\t'); o.str(sketchQuery.getReference(q).name);
+    if (comment) { o.ch(':'); o.str(sketchQuery.getReference(q).comment); }
+    o.ch('\t'); o.dbl(distance); o.ch('\t'); o.dbl(pValue); o.ch('\t'); o.u64(numer); o.ch('/'); o.u64(denom); o.ch('\n');
+}
+
 struct PairBlock {
     vector<uint32_t> numer, denom; vector<double> distance, pValue; vector<uint8_t> pass;
     void resize(size_t n) { numer.resize(n); denom.resize(n); distance.resize(n); pValue.resize(n); pass.resize(n); }
@@ -289,13 +300,8 @@ static void writeBestHits(mashgpu_dist_job *job, uint32_t nBest, const Sketch &s
         const uint64_t r = std::min(rows, nQry - q);
         if (mashgpu_dist_run_best(job, q, r, nBest, hits.data(), 0, ref.data(), numer.data(), denom.data(), distance.data(), pValue.data()) != MASHGPU_OK) gpuFail();
         mashhost::writeRows(r, threads, nBest, [&](uint64_t i, mashhost::OutBuf &o) {
-            for (uint64_t e = i * nBest; e < i * nBest + hits[i]; e++) {
-                o.str(sketchRef.getReference(ref[e]).name);
-                if (comment) { o.ch(':'); o.str(sketchRef.getReference(ref[e]).comment); }
-                o.ch('\t'); o.str(sketchQuery.getReference(q + i).name);
-                if (comment) { o.ch(':'); o.str(sketchQuery.getReference(q + i).comment); }
-                o.ch('\t'); o.dbl(distance[e]); o.ch('\t'); o.dbl(pValue[e]); o.ch('\t'); o.u64(numer[e]); o.ch('/'); o.u64(denom[e]); o.ch('\n');
-            }
+            for (uint64_t e = i * nBest; e < i * nBest + hits[i]; e++)
+                writePair(o, sketchRef, ref[e], sketchQuery, q + i, comment, distance[e], pValue[e], numer[e], denom[e]);
         });
     }
 }
@@ -393,12 +399,7 @@ int runDist(int argc, const char **argv)
                 if (mashgpu_dist_run_list(job, q, r, listCapacity, lIdx.data(), lNumer.data(), lDenom.data(), lDist.data(), lP.data(), &nPass) != MASHGPU_OK) gpuFail();
                 if (nPass <= listCapacity) {
                     mashhost::writeRows(nPass, parameters.parallelism, 1, [&](uint64_t e, mashhost::OutBuf &o) {
-                        uint64_t i = lIdx[e] / nRef, j = lIdx[e] % nRef;
-                        o.str(sketchRef.getReference(j).name);
-                        if (comment) { o.ch(':'); o.str(sketchRef.getReference(j).comment); }
-                        o.ch('\t'); o.str(sketchQuery.getReference(q + i).name);
-                        if (comment) { o.ch(':'); o.str(sketchQuery.getReference(q + i).comment); }
-                        o.ch('\t'); o.dbl(lDist[e]); o.ch('\t'); o.dbl(lP[e]); o.ch('\t'); o.u64(lNumer[e]); o.ch('/'); o.u64(lDenom[e]); o.ch('\n');
+                        writePair(o, sketchRef, lIdx[e] % nRef, sketchQuery, q + lIdx[e] / nRef, comment, lDist[e], lP[e], lNumer[e], lDenom[e]);
                     });
                     continue;
                 }
@@ -413,11 +414,7 @@ int runDist(int argc, const char **argv)
                         o.ch('\t');
                         if (out.pass[k]) o.dbl(out.distance[k]);
                     } else if (out.pass[k]) {
-                        o.str(sketchRef.getReference(j).name);
-                        if (comment) { o.ch(':'); o.str(sketchRef.getReference(j).comment); }
-                        o.ch('\t'); o.str(sketchQuery.getReference(q + i).name);
-                        if (comment) { o.ch(':'); o.str(sketchQuery.getReference(q + i).comment); }
-                        o.ch('\t'); o.dbl(out.distance[k]); o.ch('\t'); o.dbl(out.pValue[k]); o.ch('\t'); o.u64(out.numer[k]); o.ch('/'); o.u64(out.denom[k]); o.ch('\n');
+                        writePair(o, sketchRef, j, sketchQuery, q + i, comment, out.distance[k], out.pValue[k], out.numer[k], out.denom[k]);
                     }
                 }
                 if (table) o.ch('\n');
@@ -505,20 +502,66 @@ int runWithin(int argc, const char **argv)   // reference CommandContain.cpp:33-
 }
 
 // ---------------------------------------------------------------------------------------------------- triangle
-// `mash triangle -G`: one line per sketch in input order, its name (comment with -C) and its cluster.  The clusters are the connected
-// components of the pairs that pass -d / -v and share a hash, built on the device; they are numbered from 0 in the order of their
-// first member, which is the smallest index of the component, the label the engine returns.
+// a sketch as triangle prints it: its comment with -C, else its name
+static const string &sketchLabel(const Sketch &s, uint64_t i, bool comment) { return comment ? s.getReference(i).comment : s.getReference(i).name; }
+
+// the -E line of the pair (row, col): both sketches, distance, p-value and shared hashes
+static void writeEdge(mashhost::OutBuf &o, const Sketch &sketch, uint64_t row, uint64_t col, bool comment, double distance, double pValue,
+                      uint64_t numer, uint64_t denom)
+{
+    o.str(sketchLabel(sketch, row, comment)); o.ch('\t'); o.str(sketchLabel(sketch, col, comment)); o.ch('\t');
+    o.dbl(distance); o.ch('\t'); o.dbl(pValue); o.ch('\t'); o.u64(numer); o.ch('/'); o.u64(denom); o.ch('\n');
+}
+
+// `-G`, and `-L` with -d: one line per sketch in input order, its name (comment with -C) and its cluster.  Sketches of one cluster
+// share a key (key[i] < keys); the clusters are numbered from 0 in the order of their first member.  Returns the cluster count.
+static uint32_t writeClusterLines(const Sketch &sketch, bool comment, int threads, const vector<uint32_t> &key, uint64_t keys)
+{
+    const uint64_t n = sketch.getReferenceCount();
+    vector<uint32_t> number(keys, UINT32_MAX), cluster(n);
+    uint32_t clusters = 0;
+    for (uint64_t i = 0; i < n; i++) cluster[i] = number[key[i]] == UINT32_MAX ? (number[key[i]] = clusters++) : number[key[i]];
+    mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
+        o.str(sketchLabel(sketch, i, comment)); o.ch('\t'); o.u64(cluster[i]); o.ch('\n');
+    });
+    return clusters;
+}
+
+// `-N`, and `-L` without -d: the tree (writeNewick's parent / length form) as one Newick line; one sketch is its name alone
+static void writeNewickLine(const Sketch &sketch, bool comment, const vector<uint32_t> &parent, const vector<double> &length)
+{
+    const uint64_t n = sketch.getReferenceCount();
+    vector<string> names(n);
+    for (uint64_t i = 0; i < n; i++) names[i] = sketchLabel(sketch, i, comment);
+    mashhost::OutBuf o;
+    if (n == 1) { mashhost::newickName(o, names[0]); o.ch(';'); o.ch('\n'); }
+    else if (n > 1) mashhost::writeNewick(o, parent, length, names);
+    cout.flush();
+    fwrite(o.b.data(), 1, o.b.size(), stdout);
+    fflush(stdout);
+}
+
+// the self job over every sketch, with the -d / -v thresholds
+static mashgpu_dist_job *openSelfJob(const Sketch &sketch, double distanceMax, double pValueMax)
+{
+    mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
+    mashgpu_sketch_set set;
+    vector<uint64_t> h, l; vector<uint32_t> nn;
+    sketch.toSketchSet(set, h, nn, l);
+    mashgpu_dist_job *job = 0;
+    if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
+    return job;
+}
+
+// `mash triangle -G`: per sketch its cluster, the connected component of the pairs that pass -d / -v and share a hash, built on the
+// device.  The label the engine returns is the smallest index of the component, its first member.
 static void writeClusters(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int threads)
 {
     const uint64_t n = sketch.getReferenceCount();
-    vector<uint32_t> label(n), cluster(n);
-    uint64_t edges = 0, clusters = 0;
+    vector<uint32_t> label(n);
+    uint64_t edges = 0;
     if (n && mashgpu_dist_components(job, label.data(), &edges) != MASHGPU_OK) gpuFail();
-    for (uint64_t i = 0; i < n; i++) cluster[i] = label[i] == i ? (uint32_t)clusters++ : cluster[label[i]];
-    mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
-        const Sketch::Reference &ref = sketch.getReference(i);
-        o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.u64(cluster[i]); o.ch('\n');
-    });
+    const uint32_t clusters = writeClusterLines(sketch, comment, threads, label, n);
     cerr << "Clusters: " << clusters << " from " << edges << " edges" << endl;
 }
 
@@ -534,37 +577,26 @@ static void writeForest(mashgpu_dist_job *job, const Sketch &sketch, bool commen
     if (n > 1 && mashgpu_dist_spanning_forest(job, row.data(), col.data(), numer.data(), denom.data(), distance.data(), pValue.data(), &edges,
                                               &rounds) != MASHGPU_OK) gpuFail();
     mashhost::writeRows(edges, threads, 1, [&](uint64_t e, mashhost::OutBuf &o) {      // the -E line of the pair (q = row, r = col)
-        const Sketch::Reference &ref = sketch.getReference(row[e]), &qry = sketch.getReference(col[e]);
-        o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.str(comment ? qry.comment : qry.name); o.ch('\t');
-        o.dbl(distance[e]); o.ch('\t'); o.dbl(pValue[e]); o.ch('\t'); o.u64(numer[e]); o.ch('/'); o.u64(denom[e]); o.ch('\n');
+        writeEdge(o, sketch, row[e], col[e], comment, distance[e], pValue[e], numer[e], denom[e]);
     });
     cerr << "Forest: " << edges << " edges, " << n - edges << " trees in " << rounds << " rounds" << endl;
 }
 
-// `mash triangle -N`: the neighbor-joining tree of every pair's distance (DESIGN.md 3.10) as one Newick line.  One sketch is its
-// name, two are a cherry with half the distance on each branch; from three on the tree is built on the device.
+// `mash triangle -N`: the neighbor-joining tree of every pair's distance (DESIGN.md 3.10) as one Newick line.  Two sketches are a
+// cherry with half the distance on each branch; from three on the tree is built on the device.
 static void writeNeighborJoining(mashgpu_dist_job *job, const Sketch &sketch, bool comment)
 {
     const uint64_t n = sketch.getReferenceCount();
-    vector<string> names(n);
-    for (uint64_t i = 0; i < n; i++) names[i] = comment ? sketch.getReference(i).comment : sketch.getReference(i).name;
-    mashhost::OutBuf o;
-    if (n == 1) {
-        mashhost::newickName(o, names[0]); o.ch(';'); o.ch('\n');
-    } else if (n == 2) {
+    vector<uint32_t> parent(n > 2 ? 2 * n - 2 : 0);
+    vector<double> length(parent.size());
+    if (n > 2 && mashgpu_dist_neighbor_joining(job, parent.data(), length.data()) != MASHGPU_OK) gpuFail();
+    if (n == 2) {
         double d[2] = {0, 0};                                                          // row q = 1: (1, 0) and (1, 1)
         if (mashgpu_dist_run(job, 1, 1, 0, 0, d, 0, 0) != MASHGPU_OK) gpuFail();
-        o.ch('('); mashhost::newickName(o, names[0]); o.ch(':'); o.dbl(d[0] * 0.5); o.ch(',');
-        mashhost::newickName(o, names[1]); o.ch(':'); o.dbl(d[0] * 0.5); o.ch(')'); o.ch(';'); o.ch('\n');
-    } else if (n > 2) {
-        vector<uint32_t> parent(2 * n - 2);
-        vector<double> length(2 * n - 2);
-        if (mashgpu_dist_neighbor_joining(job, parent.data(), length.data()) != MASHGPU_OK) gpuFail();
-        mashhost::writeNewick(o, parent, length, names);
+        parent = {2, 2, UINT32_MAX};                                                   // the cherry's center is node 2
+        length = {d[0] * 0.5, d[0] * 0.5, 0.0};
     }
-    cout.flush();
-    fwrite(o.b.data(), 1, o.b.size(), stdout);
-    fflush(stdout);
+    writeNewickLine(sketch, comment, parent, length);
     cerr << "Tree: " << n << " leaves, " << (n > 3 ? n - 3 : 0) << " joins" << endl;
 }
 
@@ -572,7 +604,7 @@ static void writeNeighborJoining(mashgpu_dist_job *job, const Sketch &sketch, bo
 // device.  Without -d, the rooted tree as one Newick line: a merge's node sits at half its height, leaves at 0, and a branch is the
 // parent's height minus the child's.  With -d t, per sketch its flat cluster at t in -G's format: scipy's fcluster(Z, t, "distance"),
 // a maximal subtree whose every merge has height <= t (the largest height in it, since rounding in the average can make a later
-// merge lower by an ulp), numbered from 0 in the order of their first member.  One sketch has no merge: its name, or cluster 0.
+// merge lower by an ulp).  One sketch has no merge: its name, or cluster 0.
 static void writeLinkage(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int method, bool cutting, double t, int threads)
 {
     const uint64_t n = sketch.getReferenceCount(), m = n ? n - 1 : 0, nodes = n + m;
@@ -583,39 +615,23 @@ static void writeLinkage(mashgpu_dist_job *job, const Sketch &sketch, bool comme
     if (cutting) {
         vector<double> worst(nodes, 0.0);                  // the largest merge height in each node's subtree
         for (uint64_t s = 0; s < m; s++) worst[n + s] = std::max(height[s], std::max(worst[lo[s]], worst[hi[s]]));
-        vector<uint64_t> top(nodes);                       // the root of each node's flat cluster, assigned from the root down
-        if (nodes) top[nodes - 1] = nodes - 1;
+        vector<uint32_t> top(nodes);                       // the root of each node's flat cluster, assigned from the root down
+        if (nodes) top[nodes - 1] = (uint32_t)(nodes - 1);
         for (uint64_t s = m; s-- > 0;) {
-            const uint64_t u = n + s;
+            const uint32_t u = (uint32_t)(n + s);
             top[lo[s]] = worst[u] <= t ? top[u] : lo[s];
             top[hi[s]] = worst[u] <= t ? top[u] : hi[s];
         }
-        vector<uint32_t> number(nodes, UINT32_MAX), cluster(n);
-        uint32_t clusters = 0;
-        for (uint64_t i = 0; i < n; i++) cluster[i] = number[top[i]] == UINT32_MAX ? (number[top[i]] = clusters++) : number[top[i]];
-        mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
-            const Sketch::Reference &ref = sketch.getReference(i);
-            o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.u64(cluster[i]); o.ch('\n');
-        });
+        const uint32_t clusters = writeClusterLines(sketch, comment, threads, top, nodes);
         cerr << "Clusters: " << clusters << " at height <= " << t << endl;
         return;
     }
-    vector<string> names(n);
-    for (uint64_t i = 0; i < n; i++) names[i] = comment ? sketch.getReference(i).comment : sketch.getReference(i).name;
-    mashhost::OutBuf o;
-    if (n == 1) {
-        mashhost::newickName(o, names[0]); o.ch(';'); o.ch('\n');
-    } else if (n > 1) {
-        vector<uint32_t> parent(nodes, UINT32_MAX);
-        vector<double> length(nodes, 0.0);
-        auto nodeHeight = [&](uint64_t v) { return v < n ? 0.0 : height[v - n] * 0.5; };
-        for (uint64_t s = 0; s < m; s++) parent[lo[s]] = parent[hi[s]] = (uint32_t)(n + s);
-        for (uint64_t v = 0; v + 1 < nodes; v++) length[v] = nodeHeight(parent[v]) - nodeHeight(v);
-        mashhost::writeNewick(o, parent, length, names);    // its center, the last node, is the root 2n - 2
-    }
-    cout.flush();
-    fwrite(o.b.data(), 1, o.b.size(), stdout);
-    fflush(stdout);
+    vector<uint32_t> parent(nodes, UINT32_MAX);
+    vector<double> length(nodes, 0.0);
+    auto nodeHeight = [&](uint64_t v) { return v < n ? 0.0 : height[v - n] * 0.5; };
+    for (uint64_t s = 0; s < m; s++) parent[lo[s]] = parent[hi[s]] = (uint32_t)(n + s);
+    for (uint64_t v = 0; v + 1 < nodes; v++) length[v] = nodeHeight(parent[v]) - nodeHeight(v);
+    writeNewickLine(sketch, comment, parent, length);      // its center, the last node, is the root 2n - 2
     cerr << "Tree: " << n << " leaves, " << m << " merges, " << rows << " rows rescanned" << endl;
 }
 
@@ -644,28 +660,27 @@ int runTriangle(int argc, const char **argv)
         return 0;
     }
     bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active, tree = c.opt("tree").active;
-    if (cluster && edge) { cerr << "ERROR: The option -G cannot be used with -E (clusters replace the edge list)." << endl; return 1; }
-    if (tree && edge) { cerr << "ERROR: The option -T cannot be used with -E (the forest replaces the edge list)." << endl; return 1; }
-    if (tree && cluster) { cerr << "ERROR: The option -T cannot be used with -G (cut the forest at the distance instead)." << endl; return 1; }
     const bool nj = c.opt("nj").active, link = c.opt("linkage").active;
     int linkMethod = -1;
     if (link) {
         const string &m = c.opt("linkage").argument;
         linkMethod = m == "average" ? MASHGPU_LINKAGE_AVERAGE : m == "complete" ? MASHGPU_LINKAGE_COMPLETE : -1;
         if (linkMethod < 0) { cerr << "ERROR: The argument to -L must be average or complete (" << m << " given)." << endl; return 1; }
-        for (const char *o : {"edge", "cluster", "tree", "nj", "pvalue"})
-            if (c.opt(o).active) {
-                cerr << "ERROR: The option -L cannot be used with -" << c.opt(o).identifier << " (the tree is built from every pair's distance; -d cuts it)." << endl;
+    }
+    // the output modes that replace the matrix, and the options each refuses, in the order they are checked
+    const struct { const char *mode, *refused[5], *why; } conflicts[] = {
+        {"cluster", {"edge"}, "clusters replace the edge list"},
+        {"tree", {"edge"}, "the forest replaces the edge list"},
+        {"tree", {"cluster"}, "cut the forest at the distance instead"},
+        {"linkage", {"edge", "cluster", "tree", "nj", "pvalue"}, "the tree is built from every pair's distance; -d cuts it"},
+        {"nj", {"edge", "cluster", "tree", "distance", "pvalue"}, "the tree is built from every pair's distance"},
+    };
+    for (const auto &t : conflicts)
+        for (const char *o : t.refused)
+            if (o && c.opt(t.mode).active && c.opt(o).active) {
+                cerr << "ERROR: The option -" << c.opt(t.mode).identifier << " cannot be used with -" << c.opt(o).identifier << " (" << t.why << ")." << endl;
                 return 1;
             }
-    }
-    if (nj) {
-        for (const char *o : {"edge", "cluster", "tree", "distance", "pvalue"})
-            if (c.opt(o).active) {
-                cerr << "ERROR: The option -N cannot be used with -" << c.opt(o).identifier << " (the tree is built from every pair's distance)." << endl;
-                return 1;
-            }
-    }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
     if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree && !link) edge = true;
     Sketch::Parameters parameters;
@@ -679,12 +694,7 @@ int runTriangle(int argc, const char **argv)
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
     if (cluster || tree || nj || link) {
-        mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
-        mashgpu_sketch_set set;
-        vector<uint64_t> h, l; vector<uint32_t> nn;
-        sketch.toSketchSet(set, h, nn, l);
-        mashgpu_dist_job *job = 0;
-        if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
+        mashgpu_dist_job *job = openSelfJob(sketch, distanceMax, pValueMax);
         // the cut is the -d argument read as a double, so that -d 0.1 cuts where fcluster(Z, 0.1, "distance") does (-d itself is a float)
         if (link) writeLinkage(job, sketch, comment, linkMethod, c.opt("distance").active, strtod(c.opt("distance").argument.c_str(), nullptr),
                                parameters.parallelism);
@@ -697,18 +707,13 @@ int runTriangle(int argc, const char **argv)
     }
     if (!edge) {
         cout << '\t' << n << endl;
-        cout << (comment ? sketch.getReference(0).comment : sketch.getReference(0).name) << endl;
+        cout << sketchLabel(sketch, 0, comment) << endl;
     }
     if (n > 1) {
         // row i vs 0..i-1 (reference CommandTriangle.cpp:200-214): reference = sketch i, "query" = sketch j < i.
         // compareSketches(ref = row sketch, qry = column sketch); shared counts and distance are symmetric, the
         // p-value is symmetric in the two lengths, so the all-vs-all job's (q = i, r = j) entry is the same value.
-        mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
-        mashgpu_sketch_set set;
-        vector<uint64_t> h, l; vector<uint32_t> nn;
-        sketch.toSketchSet(set, h, nn, l);
-        mashgpu_dist_job *job = 0;
-        if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
+        mashgpu_dist_job *job = openSelfJob(sketch, distanceMax, pValueMax);
         if (mashgpu_dist_set_triangle(job, 1) != MASHGPU_OK) gpuFail();     // only j < i is read below
         uint64_t rows = std::max<uint64_t>(1, (1ull << 24) / n);
         PairBlock out;
@@ -717,19 +722,11 @@ int runTriangle(int argc, const char **argv)
             uint64_t r = std::min(rows, n - q);
             if (mashgpu_dist_run(job, q, r, out.numer.data(), out.denom.data(), out.distance.data(), out.pValue.data(), out.pass.data()) != MASHGPU_OK) gpuFail();
             mashhost::writeRows(r, parameters.parallelism, n, [&](uint64_t i, mashhost::OutBuf &o) {   // == writeOutput, reference CommandTriangle.cpp:159-198
-                const Sketch::Reference &ref = sketch.getReference(q + i);
-                if (!edge) o.str(comment ? ref.comment : ref.name);
+                if (!edge) o.str(sketchLabel(sketch, q + i, comment));
                 for (uint64_t j = 0; j < q + i; j++) {
                     size_t k = i * n + j;
-                    if (edge) {
-                        if (out.pass[k]) {
-                            const Sketch::Reference &qry = sketch.getReference(j);
-                            o.str(comment ? ref.comment : ref.name); o.ch('\t'); o.str(comment ? qry.comment : qry.name); o.ch('\t');
-                            o.dbl(out.distance[k]); o.ch('\t'); o.dbl(out.pValue[k]); o.ch('\t'); o.u64(out.numer[k]); o.ch('/'); o.u64(out.denom[k]); o.ch('\n');
-                        }
-                    } else {
-                        o.ch('\t'); o.dbl(out.distance[k]);
-                    }
+                    if (!edge) { o.ch('\t'); o.dbl(out.distance[k]); }
+                    else if (out.pass[k]) writeEdge(o, sketch, q + i, j, comment, out.distance[k], out.pValue[k], out.numer[k], out.denom[k]);
                 }
                 if (!edge) o.ch('\n');
             });

@@ -205,3 +205,22 @@ def dense_rank_rows(H, N, sketch_size):
     codes = np.searchsorted(u, H[:, :w]).astype(np.uint32)
     rows[:, :w] = np.where(valid[:, :w], codes, np.uint32(0xFFFFFFFF))
     return rows, ne.astype(np.uint32)
+
+
+def random_matrix(n, seed, scale=1.0):
+    """an n x n distance matrix of uniform [0, scale) values below the diagonal, NaN on and above it (never read)"""
+    D = np.random.Generator(np.random.PCG64(seed)).random((n, n)) * scale
+    D[np.triu_indices(n)] = np.nan
+    return D
+
+
+def on_device(D, ld=None):
+    """D into a CUDA tensor of n rows of ld doubles (default n), NaN in the columns past n, which must be neither read nor
+    written.  The engine runs on its own stream, so torch's fill and copy are waited for."""
+    import torch
+    n = len(D)
+    ld = ld or n
+    M = torch.full((n, ld), float("nan"), dtype=torch.float64, device="cuda")
+    M[:, :n] = torch.from_numpy(np.ascontiguousarray(D, np.float64)).cuda()
+    torch.cuda.synchronize()
+    return M

@@ -10,7 +10,9 @@ import subprocess
 import numpy as np
 import pytest
 
+import mash_b200
 from fixtures import GOLDEN, mutate, synth_genome, synth_sketches
+from msh_reader import read_msh
 from test_shard_components_gloo import min_labels
 
 pytestmark = pytest.mark.gpu
@@ -55,6 +57,45 @@ def triangle(work, *args, rc=0):
     p = subprocess.run([MASH, "triangle", *args], cwd=work, capture_output=True, text=True)
     assert p.returncode == rc, p.stderr
     return p.stdout.splitlines(), p.stderr
+
+
+def sketch_msh(work, out, *args):
+    subprocess.run([MASH, "sketch", "-o", out, *args], cwd=work, check=True, capture_output=True)
+    return work / (out + ".msh")
+
+
+def grid(msh, comment=False):
+    """names and the distance grid of run() over the sketches of msh"""
+    m = read_msh(str(msh))
+    refs = m["references"]
+    s, k = m["sketchSize"], m["kmer"]
+    hs = [np.array(r["hashes64"] or r["hashes32"] or [], np.uint64) for r in refs]      # empty sketches have neither list
+    n = len(refs)
+    H = np.full((n, s), np.uint64(0xFFFFFFFFFFFFFFFF), np.uint64)
+    N = np.array([len(h) for h in hs], np.uint32)
+    for i, h in enumerate(hs):
+        H[i, :len(h)] = h
+    L = np.array([r["length"] for r in refs], np.uint64)
+    names = [r["comment"] if comment else r["name"] for r in refs]
+    if n == 1:
+        return names, np.zeros((1, 1))
+    eng = mash_b200.Engine(0)
+    try:
+        job = eng.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
+        try:
+            D = job.run(0, n, outputs=("distance",))["distance"]
+        finally:
+            job.close()
+    finally:
+        eng.close()
+    return names, D
+
+
+def assert_refused(work, mode, others):
+    """the output mode (its arguments) with each of the others is refused: nothing on stdout, an error naming both options"""
+    for other in others:
+        out, err = triangle(work, *mode, *other, "synth.msh", rc=1)
+        assert out == [] and "ERROR" in err and mode[0] in err and other[0] in err
 
 
 def clusters_from_edges(work, cut, inputs, comment=False):

@@ -2,48 +2,21 @@
 tests/nj_model.py: stdout must be newick(nj(D)) with D the distance grid of an in-process DistJob over the same sketches (read
 from a .msh with tests/msh_reader.py), names from the sketches (comments with -C)."""
 import shutil
-import subprocess
 
-import numpy as np
 import pytest
 
-import mash_b200
 from msh_reader import read_msh
 from nj_model import newick, nj
-from test_gpu_cli_triangle_components import MASH, triangle, work  # noqa: F401  (the module fixture)
+from test_gpu_cli_triangle_components import assert_refused, grid, sketch_msh, triangle, work  # noqa: F401  (the module fixture)
 
 pytestmark = pytest.mark.gpu
 
 
-def sketch_msh(work, out, *args):
-    subprocess.run([MASH, "sketch", "-o", out, *args], cwd=work, check=True, capture_output=True)
-    return work / (out + ".msh")
-
-
 def want_line(msh, comment=False):
-    m = read_msh(str(msh))
-    refs = m["references"]
-    s, k = m["sketchSize"], m["kmer"]
-    hs = [np.array(r["hashes64"] or r["hashes32"] or [], np.uint64) for r in refs]      # empty sketches have neither list
-    n = len(refs)
-    H = np.full((n, s), np.uint64(0xFFFFFFFFFFFFFFFF), np.uint64)
-    N = np.array([len(h) for h in hs], np.uint32)
-    for i, h in enumerate(hs):
-        H[i, :len(h)] = h
-    L = np.array([r["length"] for r in refs], np.uint64)
-    names = [r["comment"] if comment else r["name"] for r in refs]
-    if n == 1:
+    names, D = grid(msh, comment)
+    if len(names) == 1:
         return newick(None, None, names)
-    eng = mash_b200.Engine(0)
-    try:
-        job = eng.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
-        try:
-            D = job.run(0, n, outputs=("distance",))["distance"]
-        finally:
-            job.close()
-    finally:
-        eng.close()
-    if n == 2:
+    if len(names) == 2:
         return newick(None, D[1, 0] * 0.5, names)
     return newick(*nj(D), names)
 
@@ -111,9 +84,7 @@ def test_one_and_two_sketches_and_quoted_names(work):
 
 
 def test_refusals_usage_and_the_other_outputs(work):
-    for other in (["-E"], ["-G"], ["-T"], ["-d", "0.1"], ["-v", "0.5"]):
-        out, err = triangle(work, "-N", *other, "synth.msh", rc=1)
-        assert out == [] and "ERROR" in err and "-N" in err and other[0] in err
+    assert_refused(work, ["-N"], (["-E"], ["-G"], ["-T"], ["-d", "0.1"], ["-v", "0.5"]))
     _, usage = triangle(work, "-h")
     assert "-N " in usage
     m1, _ = triangle(work, "synth.msh")

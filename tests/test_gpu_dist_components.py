@@ -1,7 +1,9 @@
 """GPU tests of the connected components of dist (mashgpu_dist_components): the edges are the pairs of the lower triangle with
 pass == 1 and numer > 0, and every sketch is labelled with the smallest index of its component.  The want is built from the dense
 grid of DistJob.run on the same job (itself checked against the oracle) and scipy's connected components; labels and edge counts
-must be equal."""
+must be equal.  The two largest input sets are shared with test_gpu_dist_forest.py: each is sketched and run once per session
+(one_family_run, shuffled_path_run), and each module checks its own results of that run."""
+import functools
 import os
 
 import numpy as np
@@ -104,8 +106,11 @@ def test_small_sets_against_the_oracle(gpu, oracle):
         assert np.array_equal(labels, min_labels(25, np.stack([q, r], 1))) and n_edges == q.size
 
 
-def test_one_family_every_pair_an_edge(gpu):
-    # every member keeps the family's smallest s/2 hashes: every pair shares a hash, n (n - 1) / 2 edges, one component
+@functools.cache
+def one_family_run(gpu):
+    """20 000 sketches in which every member keeps the family's smallest s/2 hashes, so every pair shares a hash: components()
+    and spanning_forest() twice each, the grid's distances at the forest's edges and at 50 of them run() one row at a time, and
+    the sorted weights of Prim's algorithm over the dense distances on the device (every minimum spanning tree has the same)"""
     n, s, k = 20_000, 64, 21
     rng = np.random.Generator(np.random.PCG64(5))
     base = np.unique(rng.integers(0, 2 ** 60, 4 * s, dtype=np.uint64))
@@ -116,10 +121,36 @@ def test_one_family_every_pair_an_edge(gpu):
     L = np.full(n, 5_000_000, np.uint64)
     job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
     try:
-        first = job.components()
-        second = job.components()
+        out = {"n": n, "components": [job.components(), job.components()], "forests": [job.spanning_forest(), job.spanning_forest()]}
+        f = out["forests"][0]
+        d = torch.empty((n, n), dtype=torch.float64, device="cuda")
+        job.run_dev(0, n, d_distance=d.data_ptr())
+        torch.cuda.synchronize()
+        sample = np.random.Generator(np.random.PCG64(6)).choice(n - 1, 50, replace=False)
+        out["sample"] = [(e, job.run(int(f["row"][e]), 1), int(f["col"][e])) for e in sample]
     finally:
         job.close()
+    out["grid_at_edges"] = d.cpu().numpy()[f["row"], f["col"]]
+    inf = torch.tensor(float("inf"), dtype=torch.float64, device="cuda")
+    key_d = d[0].clone()
+    in_tree = torch.zeros(n, dtype=torch.bool, device="cuda")
+    in_tree[0] = True
+    weights = torch.empty(n - 1, dtype=torch.float64, device="cuda")
+    for t in range(n - 1):
+        masked = torch.where(in_tree, inf, key_d)
+        v = torch.argmin(masked)
+        weights[t] = masked[v]
+        in_tree[v] = True
+        key_d = torch.minimum(key_d, d[v])
+    del d
+    out["prim_weights"] = np.sort(weights.cpu().numpy())
+    return out
+
+
+def test_one_family_every_pair_an_edge(gpu):
+    # every pair shares a hash: n (n - 1) / 2 edges, one component
+    r = one_family_run(gpu)
+    n, (first, second) = r["n"], r["components"]
     assert first[1] == second[1] == n * (n - 1) // 2
     assert not first[0].any() and np.array_equal(first[0], second[0])
 
@@ -143,11 +174,13 @@ def test_mutation_chain_is_a_path(gpu):
     assert n // 2 <= n_edges < 2 * n and len(np.unique(labels)) < n // 4
 
 
-def test_shuffled_path_over_several_query_blocks(gpu):
-    # 50 000 sketches: the host runs the queries in blocks of 2^31 / 50 000 = 42 949, so the forest carries over from one block's
-    # runs to the next and unions join rows of both.  Sketch j of a chain holds the links {L_j, R_j} (small hashes, R_j == L_{j+1}
-    # except at a break) and two fresh large hashes: adjacent sketches share exactly one hash among the first s = 4 of their union,
-    # every other pair shares none.  In shuffled order the trees grow deep, which is what the read-only flatten has to walk.
+@functools.cache
+def shuffled_path_run(gpu):
+    """50 000 sketches: the host runs the queries in blocks of 2^31 / 50 000 = 42 949, so the union-find carries over from one block's
+    runs to the next and unions join rows of both.  Sketch j of a chain holds the links {L_j, R_j} (small hashes, R_j == L_{j+1}
+    except at a break) and two fresh large hashes: adjacent sketches share exactly one hash among the first s = 4 of their union,
+    every other pair shares none.  In shuffled order the trees grow deep, which is what the read-only flatten has to walk.
+    components() and spanning_forest() twice each, with the chains: chain position j is sketch perm[j], no link after a break."""
     n, s, k = 50_000, 4, 21
     rng = np.random.Generator(np.random.PCG64(77))
     breaks = np.zeros(n, bool)
@@ -168,16 +201,22 @@ def test_shuffled_path_over_several_query_blocks(gpu):
     H[perm] = np.sort(np.stack([left, right, fill[:n], fill[n:]], 1), axis=1)
     N = np.full(n, s, np.uint32)
     L = np.full(n, 5_000_000, np.uint64)
-    j = np.flatnonzero(~breaks[:-1])
-    want = min_labels(n, np.stack([perm[j], perm[j + 1]], 1))
     job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
     try:
         assert (2 ** 31) // job.n_ref < n - 1                   # more than one block of queries
-        for _ in range(2):
-            labels, n_edges = job.components()
-            assert n_edges == j.size and np.array_equal(labels, want)
+        return {"n": n, "perm": perm, "breaks": breaks, "components": [job.components(), job.components()],
+                "forests": [job.spanning_forest(), job.spanning_forest()]}
     finally:
         job.close()
+
+
+def test_shuffled_path_over_several_query_blocks(gpu):
+    r = shuffled_path_run(gpu)
+    n, perm, breaks = r["n"], r["perm"], r["breaks"]
+    j = np.flatnonzero(~breaks[:-1])
+    want = min_labels(n, np.stack([perm[j], perm[j + 1]], 1))
+    for labels, n_edges in r["components"]:
+        assert n_edges == j.size and np.array_equal(labels, want)
     assert len(np.unique(want)) == 26
 
 

@@ -1,7 +1,7 @@
 """GPU tests of the minimum spanning forest of dist (mashgpu_dist_spanning_forest): the graph of mashgpu_dist_components (pairs of
 the lower triangle with pass == 1 and numer > 0), edges ordered by (distance, col, row).  The want is Kruskal's algorithm
 (tests/forest_model.py) over the dense grid of DistJob.run on the same job, itself checked against the oracle: edges, order and
-values must be equal bit for bit."""
+values must be equal bit for bit.  The two largest input sets are run once per session, with test_gpu_dist_components.py."""
 import math
 import os
 
@@ -11,6 +11,7 @@ import torch
 
 from fixtures import dense_rank_rows, mutate, synth_genome, synth_sketches
 from forest_model import forest_labels, kruskal
+from test_gpu_dist_components import one_family_run, shuffled_path_run
 from test_gpu_dist_prefilter import mixed_sketches
 
 pytestmark = pytest.mark.gpu
@@ -146,53 +147,21 @@ def test_duplicate_sketches_give_zero_weight_edges(gpu):
 
 
 def test_one_family_every_pair_an_edge(gpu):
-    # every member keeps the family's smallest s/2 hashes: every pair shares a hash, one tree; the grid (4e8 pairs) stays on the
-    # device, where Prim's algorithm over the dense distances gives the forest's weights (every minimum spanning tree has the same)
-    n, s, k = 20_000, 64, 21
-    rng = np.random.Generator(np.random.PCG64(5))
-    base = np.unique(rng.integers(0, 2 ** 60, 4 * s, dtype=np.uint64))
-    H = np.empty((n, s), np.uint64)
-    for i in range(n):
-        H[i] = np.sort(np.concatenate([base[:s // 2], rng.choice(base[s // 2:], s // 2, replace=False)]))
-    N = np.full(n, s, np.uint32)
-    L = np.full(n, 5_000_000, np.uint64)
-    job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
-    try:
-        first = job.spanning_forest()
-        second = job.spanning_forest()
-        d = torch.empty((n, n), dtype=torch.float64, device="cuda")
-        job.run_dev(0, n, d_distance=d.data_ptr())
-        torch.cuda.synchronize()
-        sample = np.random.Generator(np.random.PCG64(6)).choice(n - 1, 50, replace=False)
-        for e in sample:
-            one = job.run(int(first["row"][e]), 1)
-            c = int(first["col"][e])
-            assert one["numer"][0, c] == first["numer"][e] and one["denom"][0, c] == first["denom"][e]
-            assert one["distance"][0, c].tobytes() == first["distance"][e].tobytes()
-            assert one["pvalue"][0, c].tobytes() == first["pvalue"][e].tobytes()
-    finally:
-        job.close()
+    # every pair shares a hash: one tree, whose values are the grid's, and whose weights are those of every minimum spanning tree
+    r = one_family_run(gpu)
+    n, (first, second) = r["n"], r["forests"]
+    for e, one, c in r["sample"]:
+        assert one["numer"][0, c] == first["numer"][e] and one["denom"][0, c] == first["denom"][e]
+        assert one["distance"][0, c].tobytes() == first["distance"][e].tobytes()
+        assert one["pvalue"][0, c].tobytes() == first["pvalue"][e].tobytes()
     assert_same(first, second)
     assert len(first["row"]) == n - 1 and first["rounds"] <= max_rounds(n)
     assert (first["row"] > first["col"]).all()
     assert np.array_equal(forest_labels(n, first["row"], first["col"]), np.zeros(n))
     key = np.lexsort((first["row"], first["col"], first["distance"]))
     assert np.array_equal(key, np.arange(n - 1))
-    assert np.allclose(d.cpu().numpy()[first["row"], first["col"]], first["distance"], rtol=0, atol=0)
-    # Prim over the dense grid: the sorted weights of every minimum spanning tree are the same
-    inf = torch.tensor(float("inf"), dtype=torch.float64, device="cuda")
-    key_d = d[0].clone()
-    in_tree = torch.zeros(n, dtype=torch.bool, device="cuda")
-    in_tree[0] = True
-    weights = torch.empty(n - 1, dtype=torch.float64, device="cuda")
-    for t in range(n - 1):
-        masked = torch.where(in_tree, inf, key_d)
-        v = torch.argmin(masked)
-        weights[t] = masked[v]
-        in_tree[v] = True
-        key_d = torch.minimum(key_d, d[v])
-    del d
-    assert np.array_equal(np.sort(weights.cpu().numpy()), first["distance"])
+    assert np.allclose(r["grid_at_edges"], first["distance"], rtol=0, atol=0)
+    assert np.array_equal(r["prim_weights"], first["distance"])
 
 
 def test_mutation_chain(gpu):
@@ -215,40 +184,16 @@ def test_mutation_chain(gpu):
 
 
 def test_shuffled_path_over_several_query_blocks(gpu):
-    # 50 000 sketches, queries in blocks of 2^31 / 50 000: adjacent sketches of a chain share exactly one hash among the first s = 4 of
-    # their union, every other pair none (see test_gpu_dist_components); the forest is the chains' links, all at one distance, in
-    # (col, row) order.  In shuffled order the trees of the union-find grow deep over the rounds.
-    n, s, k = 50_000, 4, 21
-    rng = np.random.Generator(np.random.PCG64(77))
-    breaks = np.zeros(n, bool)
-    breaks[rng.choice(n - 1, 25, replace=False)] = True
-    links = np.arange(1, 2 * n + 2, dtype=np.uint64)
-    left = np.empty(n, np.uint64); right = np.empty(n, np.uint64)
-    nxt = 0
-    for j in range(n):
-        if j == 0 or breaks[j - 1]:
-            left[j] = links[nxt]; nxt += 1
-        else:
-            left[j] = right[j - 1]
-        right[j] = links[nxt]; nxt += 1
-    fill = np.unique(rng.integers(2 ** 40, 2 ** 62, 3 * n, dtype=np.uint64))[:2 * n]
-    rng.shuffle(fill)
-    perm = rng.permutation(n)
-    H = np.empty((n, s), np.uint64)
-    H[perm] = np.sort(np.stack([left, right, fill[:n], fill[n:]], 1), axis=1)
-    N = np.full(n, s, np.uint32)
-    L = np.full(n, 5_000_000, np.uint64)
+    # the forest is the chains' links, all at one distance, in (col, row) order; in shuffled order the trees of the union-find grow
+    # deep over the rounds
+    r = shuffled_path_run(gpu)
+    n, perm, breaks = r["n"], r["perm"], r["breaks"]
     j = np.flatnonzero(~breaks[:-1])
     a, b = perm[j], perm[j + 1]
     row, col = np.maximum(a, b), np.minimum(a, b)
     o = np.lexsort((row, col))
-    job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k)
-    try:
-        assert (2 ** 31) // job.n_ref < n - 1
-        f = job.spanning_forest()
-        assert_same(job.spanning_forest(), f)
-    finally:
-        job.close()
+    f = r["forests"][0]
+    assert_same(r["forests"][1], f)
     assert np.array_equal(f["row"], row[o]) and np.array_equal(f["col"], col[o])
     assert (f["numer"] == 1).all() and (f["denom"] == 4).all() and len(np.unique(f["distance"])) == 1
     assert f["rounds"] <= max_rounds(n)

@@ -6,9 +6,9 @@ import pytest
 import torch
 
 import mash_b200
-from fixtures import dense_rank_rows, mutate, synth_genome, synth_sketches
+from fixtures import dense_rank_rows, on_device, random_matrix, synth_sketches
 from linkage_model import METHODS, clades, linkage, linkage_cached, symmetric, ultrametric
-from test_gpu_dist_prefilter import mixed_sketches
+from test_gpu_dist_nj import assert_unchanged, job_trees, threshold_trees
 
 pytestmark = pytest.mark.gpu
 
@@ -28,23 +28,6 @@ def assert_model(got, D, method):
     want, rows, _ = linkage_cached(D, method)
     assert_bits(got, want)
     assert got["rows_rescanned"] == rows
-
-
-def on_device(D, ld=None):
-    """D into a CUDA tensor of n rows of ld doubles (the columns past n hold NaN, which must be neither read nor written).  The
-    engine runs on its own stream, so torch's fill and copy are waited for."""
-    n = len(D)
-    ld = ld or n
-    M = torch.full((n, ld), float("nan"), dtype=torch.float64, device="cuda")
-    M[:, :n] = torch.from_numpy(np.ascontiguousarray(D, np.float64)).cuda()
-    torch.cuda.synchronize()
-    return M
-
-
-def random_matrix(n, seed):
-    D = np.random.Generator(np.random.PCG64(seed)).random((n, n))
-    D[np.triu_indices(n)] = np.nan            # the upper triangle and the diagonal are never read
-    return D
 
 
 @pytest.mark.parametrize("method", METHODS)
@@ -136,88 +119,47 @@ def test_refusals(gpu):
         gpu.linkage_matrix(torch.zeros((4, 4), dtype=torch.float32, device="cuda"), 4)
 
 
-# ---- the job entry -------------------------------------------------------------------------------------------------------------
-def job_linkage(gpu, H, N, L, s, k=21, prefilter=None, **kw):
-    job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k, **kw)
-    try:
-        if prefilter is not None:
-            job.set_prefilter(prefilter)
-        grid = job.run(0, job.n_qry)
-        got = {}
-        for method in METHODS:
-            got[method] = job.linkage(method)
-            assert_model(got[method], grid["distance"], method)
-        after = job.run(0, job.n_qry)
-        for key in grid:
-            assert np.array_equal(grid[key], after[key]), key
-    finally:
-        job.close()
-    return got, grid
+# ---- the job entry: the linkages of the job runs of test_gpu_dist_nj.py, one per input set
+def job_linkage(gpu, golden, name, *params):
+    grid, trees, after = job_trees(gpu, golden, name, *params)
+    for method in METHODS:
+        assert_model(trees[method], grid["distance"], method)
+    assert_unchanged(grid, after)
+    return trees, grid
 
 
 def test_golden_genomes(gpu, golden):
-    sk = [golden.golden_sketch(i) for i in range(3)]
-    H = np.stack([h for h, _, _, _ in sk])
-    N = np.array([len(h) for h, _, _, _ in sk], np.uint32)
-    L = np.array([l for _, l, _, _ in sk], np.uint64)
-    got, _ = job_linkage(gpu, H, N, L, 1000)
+    got, _ = job_linkage(gpu, golden, "golden")
     assert got["average"]["size"].tolist() == [2, 3]
 
 
 @pytest.mark.parametrize("prefilter", [0, 1])
 def test_families_of_mutated_genomes(gpu, prefilter):
-    p = gpu.params(k=21, s=1000)
-    seqs = []
-    for f in range(4):
-        g = synth_genome(70 + f, 40_000)
-        for m in range(6):
-            seqs.append(bytes(g))
-            g = mutate(g, 0.003 * (m + 1), 10 * f + m)
-    H, N, L = gpu.sketch(seqs, p)
-    job_linkage(gpu, H, N, L, 1000, prefilter=prefilter)
+    job_linkage(gpu, None, "families", prefilter)
 
 
 @pytest.mark.parametrize("s,prefilter", [(1000, 0), (1000, 1), (300, -1), (10000, -1)])
 def test_synthetic_sketches(gpu, s, prefilter):
-    H, N, L = synth_sketches(150, s, seed=21 + s, n_families=6, ragged=True)
-    N[[3, 8]] = 0                               # empty sketches
-    H[20], N[20] = H[19], N[19]                  # a duplicate
-    job_linkage(gpu, H, N, L, s, prefilter=prefilter)
+    job_linkage(gpu, None, "synthetic", s, prefilter)
 
 
 def test_mostly_unrelated_sketches(gpu):
-    H, N, L = mixed_sketches(400, 1000, seed=4)
-    job_linkage(gpu, H, N, L, 1000, prefilter=1)
+    job_linkage(gpu, None, "mostly_unrelated")
 
 
 def test_all_unrelated_sketches(gpu):
-    rng = np.random.Generator(np.random.PCG64(3))
-    H = np.sort(rng.integers(0, 2**62, (60, 200), dtype=np.uint64), axis=1)
-    N = np.full(60, 200, np.uint32)
-    L = np.full(60, 5_000_000, np.uint64)
-    got, grid = job_linkage(gpu, H, N, L, 200)
+    got, grid = job_linkage(gpu, None, "all_unrelated")
     assert (grid["distance"][np.tril_indices(60, -1)] == 1.0).all()
     assert got["average"]["rows_rescanned"] == 59 and (got["complete"]["height"] == 1.0).all()
 
 
 def test_thresholds_and_triangle_do_not_change_the_merges(gpu):
-    H, N, L = synth_sketches(120, 1000, seed=31, n_families=5, ragged=True)
-    base = job_linkage(gpu, H, N, L, 1000)[0]
-    for kw in ({"max_distance": 0.05}, {"max_pvalue": 1e-30}, {"max_distance": 0.0, "max_pvalue": 0.0}):
-        job = gpu.dist_open(H, N, L, sketch_size=1000, k=21, kmer_space=4.0 ** 21, **kw)
-        try:
-            before = job.run(0, job.n_qry)
-            job.set_triangle(True)
-            for method in METHODS:
-                got = job.linkage(method)
-                assert_bits(got, base[method])
-                assert got["rows_rescanned"] == base[method]["rows_rescanned"]
-            job.set_triangle(False)
-            after = job.run(0, job.n_qry)
-            for key in before:
-                assert np.array_equal(before[key], after[key]), key
-        finally:
-            job.close()
+    base = job_linkage(gpu, None, "thresholds")[0]
+    for before, trees, after in threshold_trees(gpu):
+        for method in METHODS:
+            assert_bits(trees[method], base[method])
+            assert trees[method]["rows_rescanned"] == base[method]["rows_rescanned"]
+        assert_unchanged(before, after)
 
 
 def test_job_refusals(gpu):

@@ -1,12 +1,15 @@
 """GPU tests of neighbor joining (DESIGN.md 3.10): mashgpu_neighbor_joining_matrix (Engine.neighbor_joining_matrix) and
 mashgpu_dist_neighbor_joining (DistJob.neighbor_joining).  The want is tests/nj_model.py's numpy restatement, bit for bit: parent
 equal, length equal as uint64.  Larger additive trees, beyond the model's reach, must be recovered exactly."""
+import functools
+
 import numpy as np
 import pytest
 import torch
 
 import mash_b200
-from fixtures import dense_rank_rows, mutate, synth_genome, synth_sketches
+from fixtures import dense_rank_rows, mutate, on_device, random_matrix, synth_genome, synth_sketches
+from linkage_model import METHODS
 from nj_model import NONE, TreeMatrix, nj, random_tree, splits
 from test_gpu_dist_prefilter import mixed_sketches
 
@@ -19,24 +22,6 @@ def assert_bits(got, want):
     assert got["parent"].dtype == np.uint32 and got["length"].dtype == np.float64
     assert np.array_equal(got["parent"], want[0])
     assert np.array_equal(got["length"].view(np.uint64), want[1].view(np.uint64))
-
-
-def on_device(D, ld=None):
-    """D into a CUDA tensor of n rows of ld doubles (the columns past n hold junk that must not be read).  The engine runs on
-    its own stream, so torch's fill and copy are waited for."""
-    n = len(D)
-    ld = ld or n
-    M = torch.full((n, ld), float("nan"), dtype=torch.float64, device="cuda")
-    M[:, :n] = torch.from_numpy(np.ascontiguousarray(D, np.float64)).cuda()
-    torch.cuda.synchronize()
-    return M
-
-
-def random_matrix(n, seed, scale=1.0):
-    rng = np.random.Generator(np.random.PCG64(seed))
-    D = rng.random((n, n)) * scale
-    D[np.triu_indices(n)] = np.nan            # the upper triangle and the diagonal are never read
-    return D
 
 
 @pytest.mark.parametrize("n", [3, 4, 5, 17, 64, 257, 1000, 1500])
@@ -117,84 +102,117 @@ def test_refusals(gpu):
         gpu.neighbor_joining_matrix(torch.zeros((4, 4), dtype=torch.float32, device="cuda"), 4)
 
 
-# ---- the job entry -------------------------------------------------------------------------------------------------------------
-def job_tree(gpu, H, N, L, s, k=21, prefilter=None, **kw):
-    job = gpu.dist_open(H, N, L, sketch_size=s, k=k, kmer_space=4.0 ** k, **kw)
+# ---- the job entry: one self job per input set gives its grid, the NJ tree and both linkages, which test_gpu_dist_linkage.py checks
+def job_set(gpu, golden, name, *params):
+    """(H, N, L, s, prefilter) of the job-entry input set `name`"""
+    if name == "golden":
+        sk = [golden.golden_sketch(i) for i in range(3)]
+        H = np.stack([h for h, _, _, _ in sk])
+        N = np.array([len(h) for h, _, _, _ in sk], np.uint32)
+        L = np.array([l for _, l, _, _ in sk], np.uint64)
+        return H, N, L, 1000, None
+    if name == "families":
+        seqs = []
+        for f in range(4):
+            g = synth_genome(70 + f, 40_000)
+            for m in range(6):
+                seqs.append(bytes(g))
+                g = mutate(g, 0.003 * (m + 1), 10 * f + m)
+        return (*gpu.sketch(seqs, gpu.params(k=21, s=1000)), 1000, params[0])
+    if name == "synthetic":
+        s, prefilter = params
+        H, N, L = synth_sketches(150, s, seed=21 + s, n_families=6, ragged=True)
+        N[[3, 8]] = 0                           # empty sketches
+        H[20], N[20] = H[19], N[19]              # a duplicate
+        return H, N, L, s, prefilter
+    if name == "mostly_unrelated":
+        return (*mixed_sketches(400, 1000, seed=4), 1000, 1)
+    if name == "all_unrelated":
+        rng = np.random.Generator(np.random.PCG64(3))
+        H = np.sort(rng.integers(0, 2**62, (60, 200), dtype=np.uint64), axis=1)
+        return H, np.full(60, 200, np.uint32), np.full(60, 5_000_000, np.uint64), 200, None
+    assert name == "thresholds"
+    return (*synth_sketches(120, 1000, seed=31, n_families=5, ragged=True), 1000, None)
+
+
+def job_trees_of(job):
+    return {"nj": job.neighbor_joining(), **{method: job.linkage(method) for method in METHODS}}
+
+
+@functools.cache
+def job_trees(gpu, golden, name, *params):
+    """(grid, trees, grid after): the job's grid, then its NJ tree and both linkages, then its grid again"""
+    H, N, L, s, prefilter = job_set(gpu, golden, name, *params)
+    job = gpu.dist_open(H, N, L, sketch_size=s, k=21, kmer_space=4.0 ** 21)
     try:
         if prefilter is not None:
             job.set_prefilter(prefilter)
         grid = job.run(0, job.n_qry)
-        got = job.neighbor_joining()
-        assert_bits(got, nj(grid["distance"]))
-        after = job.run(0, job.n_qry)
-        for key in grid:
-            assert np.array_equal(grid[key], after[key]), key
+        trees = job_trees_of(job)
+        return grid, trees, job.run(0, job.n_qry)
     finally:
         job.close()
-    return got, grid
+
+
+@functools.cache
+def threshold_trees(gpu):
+    """(grid before, trees, grid after) of the "thresholds" set under three thresholds, the trees taken with the triangle set"""
+    H, N, L, s, _ = job_set(gpu, None, "thresholds")
+    out = []
+    for kw in ({"max_distance": 0.05}, {"max_pvalue": 1e-30}, {"max_distance": 0.0, "max_pvalue": 0.0}):
+        job = gpu.dist_open(H, N, L, sketch_size=s, k=21, kmer_space=4.0 ** 21, **kw)
+        try:
+            before = job.run(0, job.n_qry)
+            job.set_triangle(True)
+            trees = job_trees_of(job)
+            job.set_triangle(False)
+            out.append((before, trees, job.run(0, job.n_qry)))
+        finally:
+            job.close()
+    return out
+
+
+def assert_unchanged(before, after):
+    for key in before:
+        assert np.array_equal(before[key], after[key]), key
+
+
+def job_tree(gpu, golden, name, *params):
+    grid, trees, after = job_trees(gpu, golden, name, *params)
+    assert_bits(trees["nj"], nj(grid["distance"]))
+    assert_unchanged(grid, after)
+    return trees["nj"], grid
 
 
 def test_golden_genomes(gpu, golden):
-    sk = [golden.golden_sketch(i) for i in range(3)]
-    H = np.stack([h for h, _, _, _ in sk])
-    N = np.array([len(h) for h, _, _, _ in sk], np.uint32)
-    L = np.array([l for _, l, _, _ in sk], np.uint64)
-    got, _ = job_tree(gpu, H, N, L, 1000)
+    got, _ = job_tree(gpu, golden, "golden")
     assert sorted(got["parent"][:3]) == [3, 3, 3]
 
 
 @pytest.mark.parametrize("prefilter", [0, 1])
 def test_families_of_mutated_genomes(gpu, prefilter):
-    eng = gpu
-    p = eng.params(k=21, s=1000)
-    seqs = []
-    for f in range(4):
-        g = synth_genome(70 + f, 40_000)
-        for m in range(6):
-            seqs.append(bytes(g))
-            g = mutate(g, 0.003 * (m + 1), 10 * f + m)
-    H, N, L = eng.sketch(seqs, p)
-    job_tree(gpu, H, N, L, 1000, prefilter=prefilter)
+    job_tree(gpu, None, "families", prefilter)
 
 
 @pytest.mark.parametrize("s,prefilter", [(1000, 0), (1000, 1), (300, -1), (10000, -1)])
 def test_synthetic_sketches(gpu, s, prefilter):
-    H, N, L = synth_sketches(150, s, seed=21 + s, n_families=6, ragged=True)
-    N[[3, 8]] = 0                               # empty sketches
-    H[20], N[20] = H[19], N[19]                  # a duplicate
-    job_tree(gpu, H, N, L, s, prefilter=prefilter)
+    job_tree(gpu, None, "synthetic", s, prefilter)
 
 
 def test_mostly_unrelated_sketches(gpu):
-    H, N, L = mixed_sketches(400, 1000, seed=4)
-    job_tree(gpu, H, N, L, 1000, prefilter=1)
+    job_tree(gpu, None, "mostly_unrelated")
 
 
 def test_all_unrelated_sketches(gpu):
-    rng = np.random.Generator(np.random.PCG64(3))
-    H = np.sort(rng.integers(0, 2**62, (60, 200), dtype=np.uint64), axis=1)
-    N = np.full(60, 200, np.uint32)
-    L = np.full(60, 5_000_000, np.uint64)
-    got, grid = job_tree(gpu, H, N, L, 200)
+    _, grid = job_tree(gpu, None, "all_unrelated")
     assert (grid["distance"][np.tril_indices(60, -1)] == 1.0).all()
 
 
 def test_thresholds_and_triangle_do_not_change_the_tree(gpu):
-    H, N, L = synth_sketches(120, 1000, seed=31, n_families=5, ragged=True)
-    base = job_tree(gpu, H, N, L, 1000)[0]
-    for kw in ({"max_distance": 0.05}, {"max_pvalue": 1e-30}, {"max_distance": 0.0, "max_pvalue": 0.0}):
-        job = gpu.dist_open(H, N, L, sketch_size=1000, k=21, kmer_space=4.0 ** 21, **kw)
-        try:
-            before = job.run(0, job.n_qry)
-            job.set_triangle(True)
-            got = job.neighbor_joining()
-            assert_bits(got, (base["parent"], base["length"]))
-            job.set_triangle(False)
-            after = job.run(0, job.n_qry)
-            for key in before:
-                assert np.array_equal(before[key], after[key]), key
-        finally:
-            job.close()
+    base = job_tree(gpu, None, "thresholds")[0]
+    for before, trees, after in threshold_trees(gpu):
+        assert_bits(trees["nj"], (base["parent"], base["length"]))
+        assert_unchanged(before, after)
 
 
 def test_job_refusals(gpu):

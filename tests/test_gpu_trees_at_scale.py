@@ -15,7 +15,7 @@ import pytest
 import torch
 
 import tree_ref
-from fixtures import synth_sketches
+from fixtures import on_device, synth_sketches
 from linkage_model import METHODS
 from nj_model import TreeMatrix, random_tree, splits
 
@@ -25,15 +25,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def exe(tmp_path_factory):
     return tree_ref.build(tmp_path_factory.mktemp("tree_ref"))
-
-
-def on_device(D, ld):
-    """D into a CUDA tensor of n rows of ld doubles, NaN in the columns past n"""
-    n = len(D)
-    M = torch.full((n, ld), float("nan"), dtype=torch.float64, device="cuda")
-    M[:, :n] = torch.from_numpy(D).cuda()
-    torch.cuda.synchronize()
-    return M
 
 
 def collection(kind, n, s):
