@@ -104,52 +104,76 @@ __host__ __device__ __forceinline__ uint64_t murmur3_tail_k1(uint64_t t)
     return t * 0x4cf5ad432745937fULL;
 }
 
-// The body of MurmurHash3_x64_128 up to the finalisation: h1, h2 after the length xor and the two cross adds.
-// K1_GIVEN (tails of 1..8 bytes only): the tail's k1 is `k1_tail` (murmur3_tail_k1, e.g. from a table) and the tail words of
-// `a` are not read.
-template <int K, int NA, bool K1_GIVEN = false>
-__device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t seed, u64x2 &h1_out, u64x2 &h2_out,
-                                             u64x2 k1_tail = u64x2{0u, 0u})
+// The body of MurmurHash3_x64_128 up to the finalisation, from the first multiply of every block lane: p1[b] = k1 * c1 and
+// p2[b] = k2 * c2 of block b (b = K / 16: the tail, its k1 and k2 zero-extended; an entry the tail does not have is not
+// read).  h1, h2 after the length xor and the two cross adds.  K1_GIVEN (tails of 1..8 bytes only): the tail's k1 is
+// `k1_tail` (murmur3_tail_k1, e.g. from a table) and p1 of the tail is not read.
+template <int K>
+struct MurmurShape {
+    static constexpr int NB = K / 16, TAIL = K & 15;
+    static constexpr int NP = (K + 15) / 16;         // blocks with products, the tail included
+};
+
+template <int K, bool K1_GIVEN = false>
+__device__ __forceinline__ void murmur3_mix(const u64x2 (&p1)[MurmurShape<K>::NP], const u64x2 (&p2)[MurmurShape<K>::NP], uint32_t seed,
+                                            u64x2 &h1_out, u64x2 &h2_out, u64x2 k1_tail = u64x2{0u, 0u})
 {
     constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
-    constexpr int NB = K / 16, TAIL = K & 15;
+    constexpr int NB = MurmurShape<K>::NB, TAIL = MurmurShape<K>::TAIL;
     u64x2 h1{seed, 0u}, h2{seed, 0u};
     // block 0 adds h2 while it is still the seed: (r + seed) * 5 + C = r * 5 + (seed * 5 + C) mod 2^64, so the seed rides
     // on the multiply-add's addend (a loop invariant of the scan kernels) instead of a 64-bit add per hash
     const uint64_t s5 = (uint64_t)seed * 5u + 0x52dce729u;
 #pragma unroll
     for (int b = 0; b < NB; b++) {
-        u64x2 k1{a[4 * b], a[4 * b + 1]}, k2{a[4 * b + 2], a[4 * b + 3]};
-        k1 = mul_const(k1, c1); k1 = rotl<31>(k1); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
+        u64x2 k1 = rotl<31>(p1[b]); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
         h1 = rotl<27>(h1);
         if (b == 0) h1 = mul5_add64(h1, u64x2{(uint32_t)s5, (uint32_t)(s5 >> 32)});
         else { h1 = add64(h1, h2); h1 = mul5_add(h1, 0x52dce729u); }
-        k2 = mul_const(k2, c2); k2 = rotl<33>(k2); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
+        u64x2 k2 = rotl<33>(p2[b]); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
         h2 = rotl<31>(h2); h2 = add64(h2, h1); h2 = mul5_add(h2, 0x38495ab5u);
     }
     if constexpr (TAIL > 8) {
-        u64x2 k2{a[4 * NB + 2], a[4 * NB + 3]};
-        k2 = mul_const(k2, c2); k2 = rotl<33>(k2); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
+        u64x2 k2 = rotl<33>(p2[NB < MurmurShape<K>::NP ? NB : 0]); k2 = mul_const(k2, c1); h2 = xor64(h2, k2);
     }
     static_assert(!K1_GIVEN || (TAIL > 0 && TAIL <= 8), "a given k1 replaces the whole tail");
     if constexpr (K1_GIVEN) {
         h1 = xor64(h1, k1_tail);
     } else if constexpr (TAIL > 0) {
-        u64x2 k1{a[4 * NB], a[4 * NB + 1]};
-        k1 = mul_const(k1, c1); k1 = rotl<31>(k1); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
+        u64x2 k1 = rotl<31>(p1[NB < MurmurShape<K>::NP ? NB : 0]); k1 = mul_const(k1, c2); h1 = xor64(h1, k1);
     }
     h1.lo ^= (uint32_t)K; h2.lo ^= (uint32_t)K;
     h1 = add64(h1, h2); h2 = add64(h2, h1);
     h1_out = h1; h2_out = h2;
 }
 
+// The body from the key's ASCII words: the first multiply of every block lane, then murmur3_mix.
+template <int K, int NA, bool K1_GIVEN = false>
+__device__ __forceinline__ void murmur3_body(const uint32_t (&a)[NA], uint32_t seed, u64x2 &h1_out, u64x2 &h2_out,
+                                             u64x2 k1_tail = u64x2{0u, 0u})
+{
+    constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
+    using M = MurmurShape<K>;
+    u64x2 p1[M::NP], p2[M::NP];
+#pragma unroll
+    for (int b = 0; b < M::NP; b++) {
+        const bool tail = b == M::NB;
+        // (indices clamped for the tail lanes the key does not have, which are not read)
+        const int i1 = 4 * b + 1 < NA ? 4 * b : 0, i2 = 4 * b + 3 < NA ? 4 * b + 2 : 0;
+        p1[b] = tail && K1_GIVEN ? u64x2{0u, 0u} : mul_const(u64x2{a[i1], a[i1 + 1]}, c1);
+        p2[b] = tail && M::TAIL <= 8 ? u64x2{0u, 0u} : mul_const(u64x2{a[i2], a[i2 + 1]}, c2);
+    }
+    murmur3_mix<K, K1_GIVEN>(p1, p2, seed, h1_out, h2_out, k1_tail);
+}
+
 // a[i] = ASCII bytes 4i..4i+3 of the k-mer (little endian, byte 0 = first base), bytes >= K zeroed.
 // NA = 2*ceil(K/8) words.  Returns h1 (the first 8 bytes of the 128-bit digest).
-template <int K, int NA>
-__device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t seed)
+// K1_GIVEN: as murmur3_body (the tail's words of `a` are not read).
+template <int K, int NA, bool K1_GIVEN = false>
+__device__ __forceinline__ u64x2 murmur3_h1(const uint32_t (&a)[NA], uint32_t seed, u64x2 k1_tail = u64x2{0u, 0u})
 {
     u64x2 h1, h2;
-    murmur3_body<K, NA>(a, seed, h1, h2);
+    murmur3_body<K, NA, K1_GIVEN>(a, seed, h1, h2, k1_tail);
     h1 = fmix(h1); h2 = fmix(h2);
     h1 = add64(h1, h2);
     return h1;
@@ -167,6 +191,16 @@ __device__ __forceinline__ uint32_t murmur3_h1_filter(const uint32_t (&a)[NA], u
 {
     u64x2 h1, h2;
     murmur3_body<K, NA, K1_GIVEN>(a, seed, h1, h2, k1_tail);
+    return fmix_hi(h1) + fmix_hi(h2) + 1u;
+}
+
+// The same filter word from the blocks' first products (murmur3_mix)
+template <int K, bool K1_GIVEN = false>
+__device__ __forceinline__ uint32_t murmur3_filter_mix(const u64x2 (&p1)[MurmurShape<K>::NP], const u64x2 (&p2)[MurmurShape<K>::NP],
+                                                       uint32_t seed, u64x2 k1_tail = u64x2{0u, 0u})
+{
+    u64x2 h1, h2;
+    murmur3_mix<K, K1_GIVEN>(p1, p2, seed, h1, h2, k1_tail);
     return fmix_hi(h1) + fmix_hi(h2) + 1u;
 }
 

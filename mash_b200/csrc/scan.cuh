@@ -12,7 +12,10 @@
 // reverse-complement k-mer with funnel shifts, picks the canonical one by an integer compare of the
 // little-endian nibble words (equivalent to the reference's memcmp because complementing reverses the
 // base order, see DESIGN.md), expands it to ASCII with one PRMT per 4 bases and runs MurmurHash3_x64_128.
-// Only hashes at or below the tile's coarse threshold leave the fast path.
+// Only hashes at or below the tile's coarse threshold leave the fast path.  That is the layout of the FULL kernels
+// (k <= 16 and the screen's probing kernels); the filter-word kernels (k = 17..32) stage 2-bit codes instead and take the
+// first multiplies of MurmurHash3 from tables indexed by bytes of the canonical k-mer (CodeTables below), building no
+// ASCII in the fast path.
 #pragma once
 #include <cstdint>
 #include <utility>
@@ -272,11 +275,12 @@ __device__ __forceinline__ uint32_t nibble_reverse(uint32_t x)
     return ((x & 0x0F0F0F0Fu) << 4) | ((x >> 4) & 0x0F0F0F0Fu);
 }
 
-// word i of (block >> 4*OFF nibbles), block = BW little-endian words
-template <int OFF, int BW>
+// word i of (block >> BITS*OFF), block = BW little-endian words of BITS-bit digits (nibbles, or 2-bit codes)
+template <int OFF, int BW, int BITS = 4>
 __device__ __forceinline__ uint32_t block_word(const uint32_t (&b)[BW], int i)
 {
-    constexpr int WS = OFF / 8, SH = 4 * (OFF % 8);
+    constexpr int DIGITS = 32 / BITS;
+    constexpr int WS = OFF / DIGITS, SH = BITS * (OFF % DIGITS);
     const int lo_i = i + WS, hi_i = i + WS + 1;
     const uint32_t lo = lo_i < BW ? b[lo_i < BW ? lo_i : 0] : 0u;
     if (SH == 0) return lo;
@@ -295,17 +299,17 @@ struct KmerShape {
     // masking and padding are one OR.  Both strands carry the same padding in their most significant nibbles, so the
     // canonical compare is decided by the k-mer's own nibbles.
     static constexpr uint32_t LAST_PAD = ~LAST_MASK;
-    // 17 <= K <= 21 (a tail block of 1..5 bases): the filter-word kernels take the tail's k1 from a table (TailTable)
+    // 17 <= K <= 21 (a tail block of 1..5 bases): the FULL kernels take the tail's k1 from a table (TailTable)
     static constexpr bool TAIL_TABLE = K >= 17 && K <= 21;
 };
 
 // Tail block by table.  For 17 <= K <= 21 the tail block of MurmurHash3 is bases 16..K-1 of the canonical k-mer, and its k1
-// (murmur3_tail_k1 of their ASCII bytes) takes at most 4^5 values and does not depend on the seed.  The filter-word kernels
-// keep the 1024 values in shared memory and replace the tail's two PRMT, two multiplies and rotate by one IMAD, one shift
+// (murmur3_tail_k1 of their ASCII bytes) takes at most 4^5 values and does not depend on the seed.  The FULL kernels (the
+// screen's probing kernels at these k) keep the 1024 values in shared memory and replace the tail's two PRMT, two multiplies and rotate by one IMAD, one shift
 // and one 8-byte LDS.  The index is computed from the canonical k-mer's last nibble word with bit 3 and bit 2 of every
 // nibble cleared (codes c0..c4 at bits 0, 4, 8, 12, 16): w * (2^10 + 1) puts c0, c3, c1, c4, c2 side by side at bits
 // 10..19 without overlap and without a carry, and the shift keeps those ten bits.  Windows with a base outside the
-// alphabet read some entry and are rejected by the exact rebuild, as before.
+// alphabet read some entry and are rejected by the slow path's validity test.
 constexpr uint32_t TAIL_IDX_MUL = 0x401000u;   // (2^10 + 1) << 12
 constexpr int TAIL_IDX_SHIFT = 22;
 constexpr int TAIL_TAB_SIZE = 1024;
@@ -323,28 +327,27 @@ __device__ __forceinline__ void expand_ascii(const uint32_t (&c)[KmerShape<K>::N
 }
 
 // canonical k-mer of a window: c = rc when rc < fwd as little-endian multi-word integers  <=>  memcmp(fwd, rc, k) > 0
-// (Sketch.cpp:569-571): borrow out of rc - fwd.  m = all-ones when the reverse complement is the canonical k-mer.
-template <int K>
-__device__ __forceinline__ void canonical_words(const uint32_t (&f)[KmerShape<K>::NW], const uint32_t (&r)[KmerShape<K>::NW],
-                                                uint32_t (&c)[KmerShape<K>::NW])
+// (Sketch.cpp:569-571): borrow out of rc - fwd.  m = all-ones when the reverse complement is the canonical k-mer.  The
+// argument (DESIGN.md §2.2) holds for any digit width, so N words of nibbles or of 2-bit codes.
+template <int N>
+__device__ __forceinline__ void canonical_words(const uint32_t (&f)[N], const uint32_t (&r)[N], uint32_t (&c)[N])
 {
-    using S = KmerShape<K>;
     uint32_t m;
-    if (S::NW == 1) {
+    if (N == 1) {
         asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.u32 %0, 0, 0;\n\t}" : "=r"(m) : "r"(r[0]), "r"(f[0]));
-    } else if (S::NW == 2) {
+    } else if (N == 2) {
         asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.u32 %0, 0, 0;\n\t}"
-            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]));
-    } else if (S::NW == 3) {
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[N > 1 ? 1 : 0]), "r"(f[N > 1 ? 1 : 0]));
+    } else if (N == 3) {
         asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.u32 %0, 0, 0;\n\t}"
-            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]));
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[N > 1 ? 1 : 0]), "r"(f[N > 1 ? 1 : 0]), "r"(r[N > 2 ? 2 : 0]), "r"(f[N > 2 ? 2 : 0]));
     } else {
         asm("{\n\t.reg .u32 t;\n\tsub.cc.u32 t, %1, %2;\n\tsubc.cc.u32 t, %3, %4;\n\tsubc.cc.u32 t, %5, %6;\n\tsubc.cc.u32 t, %7, %8;\n\tsubc.u32 %0, 0, 0;\n\t}"
-            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[S::NW > 1 ? 1 : 0]), "r"(f[S::NW > 1 ? 1 : 0]), "r"(r[S::NW > 2 ? 2 : 0]), "r"(f[S::NW > 2 ? 2 : 0]),
-              "r"(r[S::NW > 3 ? 3 : 0]), "r"(f[S::NW > 3 ? 3 : 0]));
+            : "=r"(m) : "r"(r[0]), "r"(f[0]), "r"(r[N > 1 ? 1 : 0]), "r"(f[N > 1 ? 1 : 0]), "r"(r[N > 2 ? 2 : 0]), "r"(f[N > 2 ? 2 : 0]),
+              "r"(r[N > 3 ? 3 : 0]), "r"(f[N > 3 ? 3 : 0]));
     }
 #pragma unroll
-    for (int i = 0; i < S::NW; i++) c[i] = (f[i] & ~m) | (r[i] & m);
+    for (int i = 0; i < N; i++) c[i] = (f[i] & ~m) | (r[i] & m);
 }
 
 __device__ __forceinline__ uint32_t lds_u32(uint32_t addr)
@@ -360,48 +363,191 @@ __device__ __forceinline__ uint64_t lds_u64(uint32_t addr)
     return v;
 }
 
-// Exact hash of the window at nibble `lp` of a warp tile (shared-memory address sm_addr), rebuilt from the tile's nibble
-// words alone: forward words by funnel shifts, reverse complement by nibble reversal of those.  Returns false when the
-// window holds a base outside the alphabet (bit 3 of a nibble).
+// ---------------------------------------------------------------------------------------------------------------
+// 2-bit tiles of the filter-word kernels.  A warp tile's 1088 bases (1024 window starts + 64 halo) are staged as 68 words
+// of 16 bases (base i of a word at bits 2i, codes A0 C1 G2 T3 as the packed source has them), beside a reverse-complement
+// image (word j = word 67 - j with its codes in reverse order and complemented, so reverse-complement base q is the
+// complement of forward base 1087 - q) and a validity bitmap (1 bit per base, set = outside the alphabet) that only the
+// slow path reads.  A k-mer (17 <= k <= 32) is 2 words per strand; the first multiply of every MurmurHash3 block lane
+// comes from tables indexed by single bytes of those words (CodeTables), so the fast path builds no ASCII.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int SCAN_C2_IMAGE = 68;      // code words per warp tile image
+constexpr int SCAN_C2_WORDS = 72;      // padded: a block's reverse-complement load of an even lane reads word 68 (unused bits)
+constexpr int SCAN_INV_WORDS = 36;     // 34 validity words, padded
+
+template <int K>
+struct CodeShape {
+    static_assert(K > 16 && K <= 32, "2-bit tiles serve the filter-word kernels");
+    static constexpr int NB = (K + 7 + 15) / 16;     // normalised code words per block of 8 window starts: 2 (k <= 25) or 3
+    static constexpr uint32_t M1 = K == 32 ? 0xFFFFFFFFu : (1u << (2 * (K - 16) & 31)) - 1u;   // bases 16..K-1 of word 1
+    // tail block (bases 16..K-1): k = 17..21 take its k1 whole from a 1024-entry table indexed by word 1 (TAIL_TABLE).  For
+    // k = 22..31 its whole 4-base groups use the block tables, and the one group that K cuts short, starting at base GS,
+    // has a K-specific table of 256 products with zero bytes past K: an H-lane group (bases 4..7 of a lane: GS = 20, 28)
+    // or an L-lane group (GS = 24).
+    static constexpr bool TAIL_TABLE = K <= 21;
+    static constexpr int GS = (K <= 21 || K % 4 == 0) ? 0 : K / 4 * 4;
+    static constexpr int TAIL_SIZE = TAIL_TABLE ? TAIL_TAB_SIZE : GS ? 256 : 1;
+};
+
+// First multiplies of a MurmurHash3 block lane.  A lane (k1 or k2) is 8 ASCII bytes, L + H 2^32 with L the bytes of its
+// bases 0..3 and H of bases 4..7, so lane * c mod 2^64 = L c + ((H c_lo) mod 2^32) 2^32: a 64-bit value that depends on
+// 4 bases and a 32-bit one that depends on 4 others, 256 values each, indexed by the byte of 2-bit codes of those bases.
+// They depend neither on the seed nor on k.  a/b: k1 (c1), c/d: k2 (c2); tail: CodeShape<K>'s tail table.  One object, so
+// that the hot loop addresses every table from one register with immediate offsets.
+template <int K>
+struct CodeTables {
+    uint64_t a[256], c[256], tail[CodeShape<K>::TAIL_SIZE];
+    uint32_t b[256], d[256];
+    static constexpr uint32_t A = 0, C = 8 * 256, TAIL = 16 * 256, B = TAIL + 8 * CodeShape<K>::TAIL_SIZE, D = B + 4 * 256;
+};
+
+// ASCII bytes of the first n codes of v (2 bits each), zero bytes after
+__device__ __forceinline__ uint64_t codes_ascii(uint32_t v, int n)
+{
+    uint64_t t = 0;
+    for (int i = 0; i < n; i++) t |= (uint64_t)((0x54474341u >> (8 * ((v >> (2 * i)) & 3u))) & 0xFFu) << (8 * i);   // A C G T
+    return t;
+}
+
+// Fill the CTA's tables (CodeShape<K>); the caller synchronises
+template <int K>
+__device__ __forceinline__ void fill_code_tables(CodeTables<K> &t)
+{
+    using C = CodeShape<K>;
+    constexpr uint64_t c1 = 0x87c37b91114253d5ULL, c2 = 0x4cf5ad432745937fULL;
+    for (uint32_t v = threadIdx.x; v < 256; v += blockDim.x) {
+        const uint64_t l = codes_ascii(v, 4);
+        t.a[v] = l * c1;
+        t.c[v] = l * c2;
+        t.b[v] = (uint32_t)l * (uint32_t)c1;
+        t.d[v] = (uint32_t)l * (uint32_t)c2;
+    }
+    if (C::TAIL_TABLE) {
+        for (uint32_t v = threadIdx.x; v < TAIL_TAB_SIZE; v += blockDim.x) t.tail[v] = murmur3_tail_k1(codes_ascii(v, K - 16));
+    } else if (C::GS) {
+        const uint64_t c = C::GS < 24 ? c1 : c2;
+        for (uint32_t v = threadIdx.x; v < 256; v += blockDim.x) {
+            const uint64_t l = codes_ascii(v, K - C::GS);
+            t.tail[v] = C::GS % 8 == 4 ? (uint64_t)((uint32_t)l * (uint32_t)c) : l * c;
+        }
+    }
+}
+
+// Table lookups: the address idx * SCALE + tab is one IMAD (written in C, ptxas makes each a shift and a mask on the ALU
+// pipe), and the table's offset in CodeTables is the LDS immediate
+template <uint32_t OFF>
+__device__ __forceinline__ uint64_t tab_u64(uint32_t tab, uint32_t idx)
+{
+    uint32_t at;
+    uint64_t v;
+    asm("mad.lo.u32 %0, %1, 8, %2;" : "=r"(at) : "r"(idx), "r"(tab));
+    asm("ld.shared.u64 %0, [%1+%2];" : "=l"(v) : "r"(at), "n"(OFF));
+    return v;
+}
+template <uint32_t OFF>
+__device__ __forceinline__ uint32_t tab_u32(uint32_t tab, uint32_t idx)
+{
+    uint32_t at, v;
+    asm("mad.lo.u32 %0, %1, 4, %2;" : "=r"(at) : "r"(idx), "r"(tab));
+    asm("ld.shared.u32 %0, [%1+%2];" : "=r"(v) : "r"(at), "n"(OFF));
+    return v;
+}
+// one byte of a word, as one ALU instruction
+template <int I>
+__device__ __forceinline__ uint32_t byte_of(uint32_t x)
+{
+    if (I == 0) return x & 0xFFu;
+    if (I == 3) return x >> 24;
+    return __byte_perm(x, 0u, 0x4440u + I);
+}
+__device__ __forceinline__ u64x2 lane_product(uint64_t lo, uint32_t hi)
+{
+    return u64x2{(uint32_t)lo, (uint32_t)(lo >> 32) + hi};
+}
+
+// The filter word of the canonical k-mer whose 2-bit words are c[0] (bases 0..15) and c[1] (bases 16..K-1, masked); tab:
+// the shared address of the CTA's CodeTables<K>
+template <int K>
+__device__ __forceinline__ uint32_t code_filter_word(const ScanArgs &a, const uint32_t (&c)[2], uint32_t tab)
+{
+    using C = CodeShape<K>;
+    using T = CodeTables<K>;
+    constexpr int NP = MurmurShape<K>::NP;
+    u64x2 p1[NP], p2[NP];
+    p1[0] = lane_product(tab_u64<T::A>(tab, byte_of<0>(c[0])), tab_u32<T::B>(tab, byte_of<1>(c[0])));
+    p2[0] = lane_product(tab_u64<T::C>(tab, byte_of<2>(c[0])), tab_u32<T::D>(tab, byte_of<3>(c[0])));
+    if constexpr (C::TAIL_TABLE) {
+        const uint64_t k1 = tab_u64<T::TAIL>(tab, c[1]);
+        return murmur3_filter_mix<K, true>(p1, p2, a.seed, u64x2{(uint32_t)k1, (uint32_t)(k1 >> 32)});
+    } else {
+        // bases 16..23 (k1 of block 1 or of the tail): bases 16..19 are always whole for k >= 22
+        const uint32_t b1 = byte_of<1>(c[1]);
+        p1[NP - 1] = lane_product(tab_u64<T::A>(tab, byte_of<0>(c[1])), K >= 24 ? tab_u32<T::B>(tab, b1) : tab_u32<T::TAIL>(tab, 2 * b1));
+        if constexpr (K >= 25) {   // bases 24..31 (k2 of block 1 or of the tail)
+            const uint32_t b2 = byte_of<2>(c[1]), b3 = byte_of<3>(c[1]);
+            const uint32_t hi = K == 32 ? tab_u32<T::D>(tab, b3) : K >= 29 ? tab_u32<T::TAIL>(tab, 2 * b3) : 0u;
+            p2[NP - 1] = lane_product(K >= 28 ? tab_u64<T::C>(tab, b2) : tab_u64<T::TAIL>(tab, b2), hi);
+        } else {
+            p2[NP - 1] = u64x2{0u, 0u};
+        }
+        return murmur3_filter_mix<K>(p1, p2, a.seed);
+    }
+}
+
+// reverse complement of the 16 codes of a word: code order reversed, every code complemented (xor 3)
+__device__ __forceinline__ uint32_t revcomp16(uint32_t x)
+{
+    x = __brev(x);                          // code order reversed, the two bits of each code swapped
+    return ~(((x >> 1) & 0x55555555u) | ((x << 1) & 0xAAAAAAAAu));
+}
+
+// 8 two-bit codes (16 bits) -> 8 nibbles
+__device__ __forceinline__ uint32_t spread_codes8(uint32_t x)
+{
+    x = (x | (x << 8)) & 0x00FF00FFu;
+    x = (x | (x << 4)) & 0x0F0F0F0Fu;
+    x = (x | (x << 2)) & 0x33333333u;
+    return x;
+}
+
+// Exact hash of the window at base `lp` of a warp tile, rebuilt from its code images (shared addresses c2 forward, rc2
+// reverse complement) and its validity bitmap (inv).  Returns false when the window holds a base outside the alphabet.
 template <int K, bool CANON>
-__device__ __forceinline__ bool window_hash(const ScanArgs &a, uint32_t sm_addr, uint32_t lp, uint64_t &hash)
+__device__ __forceinline__ bool window_hash(const ScanArgs &a, uint32_t c2, uint32_t rc2, uint32_t inv, uint32_t lp, uint64_t &hash)
 {
     using S = KmerShape<K>;
-    uint32_t x[S::NW + 1], f[S::NW], c[S::NW];
-    const uint32_t w = sm_addr + 4 * (lp >> 3), sh = 4 * (lp & 7);
-#pragma unroll
-    for (int i = 0; i <= S::NW; i++) x[i] = lds_u32(w + 4 * i);     // word index <= 127 + 4 < SCAN_WARP_WORDS
-    uint32_t bad = 0;
+    using C = CodeShape<K>;
+    uint32_t f[2], c[2];
+    {
+        const uint32_t w = c2 + 4 * (lp >> 4), sh = 2 * (lp & 15);      // word index <= 63 + 2
+        const uint32_t x0 = lds_u32(w), x1 = lds_u32(w + 4), x2 = lds_u32(w + 8);
+        f[0] = __funnelshift_r(x0, x1, sh);
+        f[1] = __funnelshift_r(x1, x2, sh) & C::M1;
+    }
+    const uint32_t v = inv + 4 * (lp >> 5);
+    const uint32_t bad = __funnelshift_r(lds_u32(v), lds_u32(v + 4), lp & 31) & (K == 32 ? 0xFFFFFFFFu : (1u << (K & 31)) - 1u);
+    if (CANON) {
+        const uint32_t q = 16 * SCAN_C2_IMAGE - lp - K;                 // the reverse complement's first base, word <= 66 + 2
+        const uint32_t w = rc2 + 4 * (q >> 4), sh = 2 * (q & 15);
+        const uint32_t y0 = lds_u32(w), y1 = lds_u32(w + 4), y2 = lds_u32(w + 8);
+        const uint32_t r[2] = {__funnelshift_r(y0, y1, sh), __funnelshift_r(y1, y2, sh) & C::M1};
+        canonical_words(f, r, c);
+    } else {
+        c[0] = f[0]; c[1] = f[1];
+    }
+    uint32_t n[S::NW];
 #pragma unroll
     for (int i = 0; i < S::NW; i++) {
-        f[i] = __funnelshift_r(x[i], x[i + 1], sh);
-        if (i == S::NW - 1) f[i] = (f[i] & S::LAST_MASK) | S::LAST_PAD;
-        bad |= i == S::NW - 1 ? f[i] & S::LAST_MASK : f[i];
-    }
-    if (CANON) {
-        // rr = the 8 NW nibbles of f reversed and complemented; the reverse complement starts P = 8 NW - K nibbles in
-        constexpr int P = 8 * S::NW - K;
-        uint32_t rr[S::NW + 1], r[S::NW];
-#pragma unroll
-        for (int i = 0; i < S::NW; i++) rr[i] = nibble_reverse(f[S::NW - 1 - i]) ^ 0x33333333u;
-        rr[S::NW] = 0;
-#pragma unroll
-        for (int i = 0; i < S::NW; i++) {
-            r[i] = P ? __funnelshift_r(rr[i], rr[i + 1], 4 * P) : rr[i];
-            if (i == S::NW - 1) r[i] = (r[i] & S::LAST_MASK) | S::LAST_PAD;
-        }
-        canonical_words<K>(f, r, c);
-    } else {
-#pragma unroll
-        for (int i = 0; i < S::NW; i++) c[i] = f[i];
+        n[i] = spread_codes8((c[i >> 1] >> (16 * (i & 1))) & 0xFFFFu);
+        if (i == S::NW - 1) n[i] = (n[i] & S::LAST_MASK) | S::LAST_PAD;
     }
     uint32_t pool;
     asm("mov.u32 %0, 0x54474341;" : "=r"(pool));
     uint32_t asc[S::NA];
-    expand_ascii<K>(c, asc, pool);
+    expand_ascii<K>(n, asc, pool);
     const u64x2 h = murmur3_h1<K, S::NA>(asc, a.seed);
-    hash = K <= 16 ? (uint64_t)h.lo : (((uint64_t)h.hi << 32) | h.lo);
-    return !(bad & 0x88888888u);
+    hash = ((uint64_t)h.hi << 32) | h.lo;
+    return bad == 0;
 }
 
 // Survivor queue of the filter-word kernels: per warp, up to SCAN_SQ exact survivors {hash, stream position} waiting for
@@ -423,7 +569,8 @@ __shared__ uint32_t scan_sq_n[SCAN_WARPS];   // entries appended since the last 
 // tile, and queue the valid ones at or below the tile threshold for their table work.  Out of line: inlined into scan_kernel
 // it measured slower (DESIGN.md §2.4).
 template <int K, bool CANON>
-static __device__ __noinline__ void scan_resolve(const ScanArgs &a, uint32_t pm, uint32_t sm_addr, uint64_t tile_base, uint64_t tmax)
+static __device__ __noinline__ void scan_resolve(const ScanArgs &a, uint32_t pm, uint32_t c2, uint32_t rc2, uint32_t inv, uint64_t tile_base,
+                                                uint64_t tmax)
 {
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     while (__any_sync(0xFFFFFFFFu, pm != 0)) {
@@ -432,7 +579,7 @@ static __device__ __noinline__ void scan_resolve(const ScanArgs &a, uint32_t pm,
             pm &= pm - 1;
             const uint32_t lp = 8 * (lane + 32 * (bit >> 3)) + (bit & 7);
             uint64_t hash;
-            if (window_hash<K, CANON>(a, sm_addr, lp, hash) && hash <= tmax) {
+            if (window_hash<K, CANON>(a, c2, rc2, inv, lp, hash) && hash <= tmax) {
                 const uint32_t at = atomicAdd(&scan_sq_n[warp], 1u);
                 if (at < SCAN_SQ) {
                     scan_sq_hash[warp][at] = hash;
@@ -500,7 +647,7 @@ __device__ __forceinline__ void window_words(const uint32_t (&b)[KmerShape<K>::B
             r[i] = block_word<RO, S::BW>(rb, i);
             if (i == S::NW - 1) r[i] = (r[i] & LM) | LP;
         }
-        canonical_words<K>(f, r, c);
+        canonical_words(f, r, c);
     } else {
 #pragma unroll
         for (int i = 0; i < S::NW; i++) c[i] = f[i];
@@ -541,28 +688,14 @@ __device__ __forceinline__ uint32_t scan_mb_extra(const ScanArgs &a, uint32_t x)
 }
 
 // Full-hash fast path (k <= 16, and the screen's probing kernels: every lane probes the reference table with its own hash)
-template <int K, bool CANON, int J>
-__device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
-                                            const uint32_t (&rb)[KmerShape<K>::BW], uint64_t tmax, uint32_t pool, u64x2 &h_out)
-{
-    using S = KmerShape<K>;
-    uint32_t asc[S::NA];
-    window_ascii<K, CANON, J>(b, rb, pool, asc);
-    u64x2 h = murmur3_h1<K, S::NA>(asc, a.seed);
-    if (K <= 16) h.hi = 0;        // 32-bit hashes: |{A,C,G,T}|^k <= 2^32 (reference Sketch.cpp:1136, hash.cpp:31-35)
-    // coarse filter on one 32-bit word; validity and the exact threshold are checked in the slow path
-    h_out = h;
-    return (K <= 16) ? (h.lo <= (uint32_t)tmax) : (h.hi <= (uint32_t)(tmax >> 32));
-}
-
-// Filter-word fast path (k > 16): only murmur3_h1_filter's word, to be tested against filter_threshold(tmax >> 32)
 // (tail_tab: the CTA's tail table in shared memory, used when KmerShape<K>::TAIL_TABLE)
 template <int K, bool CANON, int J>
-__device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
-                                                       const uint32_t (&rb)[KmerShape<K>::BW], uint32_t pool, const uint64_t *tail_tab)
+__device__ __forceinline__ bool scan_window(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW],
+                                            const uint32_t (&rb)[KmerShape<K>::BW], uint64_t tmax, uint32_t pool, const uint64_t *tail_tab,
+                                            u64x2 &h_out)
 {
     using S = KmerShape<K>;
-    uint32_t x;
+    u64x2 h;
     if constexpr (S::TAIL_TABLE) {
         // the last word keeps the two code bits of the tail's nibbles (both strands alike, so the compare is unchanged for
         // windows in the alphabet); it becomes the table index instead of ASCII words
@@ -573,26 +706,79 @@ __device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const 
             asc[2 * i] = prmt(pool, 0, c[i]);
             asc[2 * i + 1] = prmt(pool, 0, c[i] >> 16);
         }
-        uint32_t at;   // base + 8 index as one IMAD: written in C, ptxas makes it a shift, a mask and an add
-        asm("mad.lo.u32 %0, %1, 8, %2;" : "=r"(at) : "r"(tail_index(c[S::NW - 1])), "r"((uint32_t)__cvta_generic_to_shared(tail_tab)));
-        const uint64_t k1 = lds_u64(at);
-        x = murmur3_h1_filter<K, S::NA - 2, true>(asc, a.seed, u64x2{(uint32_t)k1, (uint32_t)(k1 >> 32)});
+        const uint64_t k1 = tail_tab[tail_index(c[S::NW - 1])];
+        h = murmur3_h1<K, S::NA - 2, true>(asc, a.seed, u64x2{(uint32_t)k1, (uint32_t)(k1 >> 32)});
     } else {
         uint32_t asc[S::NA];
         window_ascii<K, CANON, J>(b, rb, pool, asc);
-        x = murmur3_h1_filter<K, S::NA>(asc, a.seed);
+        h = murmur3_h1<K, S::NA>(asc, a.seed);
     }
-    return scan_mb_extra(a, x);
+    if (K <= 16) h.hi = 0;        // 32-bit hashes: |{A,C,G,T}|^k <= 2^32 (reference Sketch.cpp:1136, hash.cpp:31-35)
+    // coarse filter on one 32-bit word; validity and the exact threshold are checked in the slow path
+    h_out = h;
+    return (K <= 16) ? (h.lo <= (uint32_t)tmax) : (h.hi <= (uint32_t)(tmax >> 32));
+}
+
+// Filter-word fast path (k > 16): only murmur3_h1_filter's word, to be tested against filter_threshold(tmax >> 32).  b, rb:
+// the block's normalised code words (forward from the block's first base, reverse complement ending at its last), so window
+// J's forward k-mer starts J bases into b and its reverse complement 16 NB - K - J bases into rb; both offsets are immediates.
+template <int K, bool CANON, int J>
+__device__ __forceinline__ uint32_t scan_window_filter(const ScanArgs &a, const uint32_t (&b)[CodeShape<K>::NB],
+                                                       const uint32_t (&rb)[CodeShape<K>::NB], uint32_t tab)
+{
+    using C = CodeShape<K>;
+    uint32_t f[2], c[2];
+    f[0] = block_word<J, C::NB, 2>(b, 0);
+    f[1] = block_word<J, C::NB, 2>(b, 1) & C::M1;
+    if (CANON) {
+        constexpr int RO = 16 * C::NB - K - J;
+        const uint32_t r[2] = {block_word<RO, C::NB, 2>(rb, 0), block_word<RO, C::NB, 2>(rb, 1) & C::M1};
+        canonical_words(f, r, c);
+    } else {
+        c[0] = f[0]; c[1] = f[1];
+    }
+    return scan_mb_extra(a, code_filter_word<K>(a, c, tab));
 }
 
 // The 8 windows of a block hashed back to back (independent multiply chains that ptxas can interleave), their pass flags
 // at bits 24..31 of the result (bit 24 + j = window j).  No vote and no branch: the hot loop shifts the block's flags into
 // the lane's pass mask, and the mask is resolved once per tile (scan_resolve).
 template <int K, bool CANON, int... J>
-__device__ __forceinline__ uint32_t scan_block_filter(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
-                                                      uint32_t tf, uint32_t pool, const uint64_t *tail_tab, std::integer_sequence<int, J...>)
+__device__ __forceinline__ uint32_t scan_block_filter(const ScanArgs &a, const uint32_t (&b)[CodeShape<K>::NB], const uint32_t (&rb)[CodeShape<K>::NB],
+                                                      uint32_t tf, uint32_t tab, std::integer_sequence<int, J...>)
 {
-    return (((scan_window_filter<K, CANON, J>(a, b, rb, pool, tail_tab) <= tf ? 1u : 0u) << (24 + J)) | ...);
+    return (((scan_window_filter<K, CANON, J>(a, b, rb, tab) <= tf ? 1u : 0u) << (24 + J)) | ...);
+}
+
+// The lane's pass mask of a warp tile (filter-word kernels): block i = (g - lane) / 32 ends at bits 8 i .. 8 i + 7 after the
+// tile's 4 trips.  Block g starts at base 8 g, bits 16 (g & 1) of code word g / 2, and a lane's g all have its parity, so
+// one funnel shift per word by a per-lane amount normalises the block to start at bit 0 of b[0] (and its reverse
+// complement, which ends at base 1087 - 8 g of the reverse-complement image, to end at the top of rb[NB - 1]).
+template <int K, bool CANON>
+__device__ __forceinline__ uint32_t scan_tile_filter(const ScanArgs &a, uint32_t c2, uint32_t rc2, uint32_t tab, uint32_t tf)
+{
+    using C = CodeShape<K>;
+    const int lane = threadIdx.x & 31;
+    const uint32_t par = 16u * (lane & 1);
+    const uint32_t rc_lane = rc2 + 4u * (SCAN_C2_IMAGE - C::NB - (lane & 1));
+    uint32_t pmask = 0;
+#pragma unroll 1
+    for (int g = lane; g < SCAN_WARP_TILE / 8; g += 32) {
+        const uint32_t h = (uint32_t)g >> 1;
+        uint32_t w[C::NB + 1], b[C::NB], rb[C::NB];
+#pragma unroll
+        for (int i = 0; i <= C::NB; i++) w[i] = lds_u32(c2 + 4u * (h + i));
+#pragma unroll
+        for (int i = 0; i < C::NB; i++) b[i] = __funnelshift_r(w[i], w[i + 1], par);
+        if (CANON) {
+#pragma unroll
+            for (int i = 0; i <= C::NB; i++) w[i] = lds_u32(rc_lane - 4u * h + 4u * i);
+#pragma unroll
+            for (int i = 0; i < C::NB; i++) rb[i] = __funnelshift_r(w[i], w[i + 1], par);
+        }
+        pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, tab, std::make_integer_sequence<int, 8>());
+    }
+    return pmask;
 }
 
 // Fill the CTA's tail table (KmerShape<K>::TAIL_TABLE): entry tail_index(w) = murmur3_tail_k1 of the ASCII bytes of bases
@@ -618,11 +804,12 @@ __device__ __forceinline__ void fill_tail_table(uint64_t *tab)
 // DESIGN.md §2.4).
 template <int K, bool CANON, int J0>
 __device__ __forceinline__ void scan_group(const ScanArgs &a, const uint32_t (&b)[KmerShape<K>::BW], const uint32_t (&rb)[KmerShape<K>::BW],
-                                           uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t pool, const uint32_t *sm_tile)
+                                           uint64_t tile_base, uint32_t local0, uint64_t tmax, uint32_t pool, const uint32_t *sm_tile,
+                                           const uint64_t *tail_tab)
 {
     u64x2 h0, h1;
-    const bool p0 = scan_window<K, CANON, J0>(a, b, rb, tmax, pool, h0);
-    const bool p1 = scan_window<K, CANON, J0 + 1>(a, b, rb, tmax, pool, h1);
+    const bool p0 = scan_window<K, CANON, J0>(a, b, rb, tmax, pool, tail_tab, h0);
+    const bool p1 = scan_window<K, CANON, J0 + 1>(a, b, rb, tmax, pool, tail_tab, h1);
     if (__any_sync(0xFFFFFFFFu, p0 | p1)) {
         if (__any_sync(0xFFFFFFFFu, p0)) scan_emit_warp(a, p0, h0.lo, h0.hi, tile_base, local0 + J0, sm_tile, K, tmax);
         if (__any_sync(0xFFFFFFFFu, p1)) scan_emit_warp(a, p1, h1.lo, h1.hi, tile_base, local0 + J0 + 1, sm_tile, K, tmax);
@@ -668,19 +855,56 @@ __device__ __forceinline__ uint32_t clip_word(uint32_t w, uint64_t off, uint64_t
     return w;
 }
 
-// Filter-word kernels, ASCII source: a lane's staged words -- words 2 lane, 2 lane + 1 (w0, w1), 64 + 2 lane, 65 + 2 lane
-// (w2, w3) and halo word 128 + hw (w4) -- into a forward image and, canonical, its reverse-complement image
-template <bool CANON>
-__device__ __forceinline__ void stage_words(uint32_t *sm, uint32_t *smr, int lane, int hw, uint32_t w0, uint32_t w1, uint32_t w2,
-                                            uint32_t w3, uint32_t w4)
+// 4 byte codes (bits 0-1 of each byte) -> one byte of 2-bit codes at bits 24..31: of the products of the multiply by
+// 2^24 + 2^18 + 2^12 + 2^6, those that fall below bit 24 land in disjoint 2-bit fields, so nothing carries into bits 24..31
+__device__ __forceinline__ uint32_t gather_codes4(uint32_t x) { return x * 0x01041040u; }
+
+// 8 ASCII bytes -> 16 bits of 2-bit codes (the low half of the result; the high half is not zero), the codes of
+// ascii8_to_code_word, which also tests the bytes into `diff`
+__device__ __forceinline__ uint32_t ascii8_to_codes16(uint32_t lo, uint32_t hi, uint32_t fold, uint32_t pool, uint32_t &diff)
 {
-    *reinterpret_cast<uint2 *>(sm + 2 * lane) = make_uint2(w0, w1);
-    *reinterpret_cast<uint2 *>(sm + 2 * (lane + 32)) = make_uint2(w2, w3);
-    sm[128 + hw] = w4;
+    ascii8_to_code_word(lo, hi, fold, pool, diff);
+    const uint32_t x0 = ((lo >> 1) ^ (lo >> 2)) & 0x03030303u, x1 = ((hi >> 1) ^ (hi >> 2)) & 0x03030303u;
+    return __byte_perm(gather_codes4(x0), gather_codes4(x1), 0x0073);
+}
+
+// nibble word (codes 0..3 in bits 0-1 of each nibble, bit 3 = outside the alphabet) -> 16 bits of 2-bit codes / 8 flag bits
+__device__ __forceinline__ uint32_t nibbles_to_codes16(uint32_t w)
+{
+    w &= 0x33333333u;
+    w = (w | (w >> 2)) & 0x0F0F0F0Fu;
+    w = (w | (w >> 4)) & 0x00FF00FFu;
+    return (w | (w >> 8)) & 0xFFFFu;
+}
+__device__ __forceinline__ uint32_t nibbles_to_flags8(uint32_t w)
+{
+    w = (w >> 3) & 0x11111111u;
+    w = (w | (w >> 3)) & 0x03030303u;
+    w = (w | (w >> 6)) & 0x000F000Fu;
+    return (w | (w >> 12)) & 0xFFu;
+}
+
+__device__ __forceinline__ void sts_u16(uint32_t addr, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" :: "r"(addr), "h"((unsigned short)v) : "memory"); }
+__device__ __forceinline__ void sts_u8(uint32_t addr, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" :: "r"(addr), "h"((unsigned short)v) : "memory"); }
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
+
+// Filter-word kernels, ASCII source: a lane's staged code words -- word lane (w0), word lane + 32 (w1) and halo half-word
+// 128 + hw (h, bases 1024 + 8 hw ..) -- and their validity bits (v0, v1: 16 bits, vh: 8 bits) into the forward image, the
+// validity bitmap and, canonical, the reverse-complement image (half-word H of the forward image is half-word 135 - H there)
+template <bool CANON>
+__device__ __forceinline__ void stage_codes(uint32_t c2, uint32_t rc2, uint32_t inv, int lane, int hw, uint32_t w0, uint32_t w1, uint32_t h,
+                                            uint32_t v0, uint32_t v1, uint32_t vh)
+{
+    sts_u32(c2 + 4 * lane, w0);
+    sts_u32(c2 + 4 * (lane + 32), w1);
+    sts_u16(c2 + 2 * (128 + hw), h);
+    sts_u16(inv + 2 * lane, v0);
+    sts_u16(inv + 2 * (lane + 32), v1);
+    sts_u8(inv + 128 + hw, vh);
     if (CANON) {
-        *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * lane)) = make_uint2(nibble_reverse(w1) ^ 0x33333333u, nibble_reverse(w0) ^ 0x33333333u);
-        *reinterpret_cast<uint2 *>(smr + (SCAN_WARP_WORDS - 2 - 2 * (lane + 32))) = make_uint2(nibble_reverse(w3) ^ 0x33333333u, nibble_reverse(w2) ^ 0x33333333u);
-        smr[SCAN_WARP_WORDS - 1 - 128 - hw] = nibble_reverse(w4) ^ 0x33333333u;
+        sts_u32(rc2 + 4 * (SCAN_C2_IMAGE - 1 - lane), revcomp16(w0));
+        sts_u32(rc2 + 4 * (SCAN_C2_IMAGE - 1 - 32 - lane), revcomp16(w1));
+        sts_u16(rc2 + 2 * (2 * SCAN_C2_IMAGE - 1 - 128 - hw), revcomp16(h) >> 16);
     }
 }
 
@@ -763,13 +987,6 @@ __device__ __forceinline__ void scan_prefetch_land(const ScanArgs &a, uint64_t w
 }
 
 // 32 packed positions (2-bit codes + invalid bits) -> 4 nibble words
-__device__ __forceinline__ uint32_t spread_codes8(uint32_t x)   // 8 two-bit codes (16 bits) -> 8 nibbles
-{
-    x = (x | (x << 8)) & 0x00FF00FFu;
-    x = (x | (x << 4)) & 0x0F0F0F0Fu;
-    x = (x | (x << 2)) & 0x33333333u;
-    return x;
-}
 __device__ __forceinline__ uint32_t spread_bits8(uint32_t y)    // 8 bits -> bit 3 of 8 nibbles
 {
     y = (y | (y << 12)) & 0x000F000Fu;
@@ -800,44 +1017,61 @@ __device__ __forceinline__ uint4 expand32(uint64_t c, uint32_t m)
 #ifndef SCAN_MIN_BLOCKS_FULL
 #define SCAN_MIN_BLOCKS_FULL 3 // FULL kernels (=> 80 registers, no spills; 4 => 64 registers and spills)
 #endif
+__device__ __forceinline__ void sts_u64(uint32_t addr, uint32_t lo, uint32_t hi)
+{
+    asm volatile("st.shared.v2.u32 [%0], {%1, %2};" :: "r"(addr), "r"(lo), "r"(hi) : "memory");
+}
+
 // FULL: the fast path computes the whole 64-bit hash (k <= 16, where the filter is on the low word, and SCAN_SCREEN, where
-// every lane probes the reference table with it); otherwise only murmur3_h1_filter's word and the slow path recomputes.
+// every lane probes the reference table with it) from nibble tiles; otherwise only murmur3_h1_filter's word, from 2-bit
+// tiles, and the slow path recomputes.
 template <int K, bool CANON, bool PACKED, bool FULL>
 __global__ void __launch_bounds__(SCAN_THREADS, FULL ? ((K > 24 && SCAN_MIN_BLOCKS_FULL > 3) ? 3 : SCAN_MIN_BLOCKS_FULL) : SCAN_MIN_BLOCKS)
 scan_kernel(const __grid_constant__ ScanArgs a)
 {
     using S = KmerShape<K>;
+    using C = CodeShape<(K > 16 ? K : 17)>;
     static_assert(FULL || K > 16, "the filter word is the high word of the hash");
-    __shared__ __align__(16) uint32_t sm_all[SCAN_WARPS][SCAN_WARP_WORDS];
+    constexpr int NWARPS = FULL ? SCAN_WARPS : 1;    // nibble tiles (FULL kernels)
+    constexpr int CWARPS = FULL ? 1 : SCAN_WARPS;    // code tiles and landing buffers (filter-word kernels)
+    __shared__ __align__(16) uint32_t sm_all[NWARPS][SCAN_WARP_WORDS];
     // reverse-complement image of the tile (word i = nibble-reversed, complemented word NW-1-i), written once at staging so
     // that a block's reverse-complement words are 4 more LDS (the LSU is idle) instead of ~16 ALU instructions per block
-    __shared__ __align__(16) uint32_t smr_all[CANON ? SCAN_WARPS : 1][SCAN_WARP_WORDS];
-    __shared__ __align__(16) uint4 land_all[FULL ? 1 : SCAN_WARPS][FULL ? 1 : SCAN_WARP_VECS];   // next tile's raw bytes
-    constexpr bool TAB = !FULL && S::TAIL_TABLE;
-    __shared__ __align__(16) uint64_t tail_tab[TAB ? TAIL_TAB_SIZE : 1];
-    if (TAB) {
+    __shared__ __align__(16) uint32_t smr_all[CANON ? NWARPS : 1][SCAN_WARP_WORDS];
+    __shared__ __align__(16) uint32_t c2_all[CWARPS][SCAN_C2_WORDS];
+    __shared__ __align__(16) uint32_t rc2_all[CANON ? CWARPS : 1][SCAN_C2_WORDS];
+    __shared__ __align__(16) uint32_t inv_all[CWARPS][SCAN_INV_WORDS];
+    __shared__ __align__(16) uint4 land_all[CWARPS][FULL ? 1 : SCAN_WARP_VECS];   // next tile's raw bytes
+    __shared__ __align__(16) uint8_t code_tab[FULL ? 16 : sizeof(CodeTables<(K > 16 ? K : 17)>)];
+    __shared__ __align__(16) uint64_t tail_tab[FULL && S::TAIL_TABLE ? TAIL_TAB_SIZE : 1];
+    if constexpr (!FULL) {
+        fill_code_tables<K>(*reinterpret_cast<CodeTables<K> *>(code_tab));
+        __syncthreads();
+    } else if constexpr (S::TAIL_TABLE) {
         fill_tail_table<K>(tail_tab);
         __syncthreads();
     }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t *sm = sm_all[warp];
-    uint32_t *smr = smr_all[CANON ? warp : 0];
+    uint32_t *sm = sm_all[FULL ? warp : 0];
+    uint32_t *smr = smr_all[CANON && FULL ? warp : 0];
     // the hot loop and the slow path address the tiles as 32-bit shared-memory addresses, passed through a shuffle (they are
     // warp-uniform) so that ptxas keeps them in registers: it otherwise re-derives them (S2R SR_CgaCtaId, LEA, IMAD) on every
     // iteration of the hot loop to save a register
-    const uint32_t sm_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(sm), 0);
-    const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(smr), 0);
+    const uint32_t sm_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(FULL ? sm : c2_all[FULL ? 0 : warp]), 0);
+    const uint32_t smr_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(FULL ? smr : rc2_all[CANON && !FULL ? warp : 0]), 0);
+    const uint32_t inv_addr = (uint32_t)__cvta_generic_to_shared(inv_all[FULL ? 0 : warp]);
+    const uint32_t tab_addr = __shfl_sync(0xFFFFFFFFu, (uint32_t)__cvta_generic_to_shared(code_tab), 0);
     const uint32_t land = (uint32_t)__cvta_generic_to_shared(land_all[FULL ? 0 : warp]);
     const uint32_t fold = a.preserve_case ? 0xFFFFFFFFu : 0xDFDFDFDFu;
     // the bytes 'A','C','G','T' for PRMT.  Filter-word kernels: each lane reads the pool back from its own word of the warp's
-    // tile (word 2 lane, which only this lane stages later), so that ptxas keeps it in one register for the whole kernel.  A
+    // tile (word lane, which only this lane stages later), so that ptxas keeps it in one register for the whole kernel.  A
     // constant, even through a shuffle or %laneid arithmetic, is rebuilt before every PRMT instead (an IMAD.U32 each).  The
     // FULL kernels keep the constant.
     uint32_t pool;
     if (FULL) {
         asm volatile("mov.u32 %0, 0x54474341;" : "=r"(pool));
     } else {
-        const uint32_t at = (uint32_t)__cvta_generic_to_shared(sm) + 8u * lane;
+        const uint32_t at = sm_addr + 4u * lane;
         asm volatile("st.shared.u32 [%0], %1;" :: "r"(at), "r"(0x54474341u) : "memory");
         asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(pool) : "r"(at) : "memory");
     }
@@ -850,7 +1084,8 @@ scan_kernel(const __grid_constant__ ScanArgs a)
 
     // FULL kernels: each lane stages vectors lane, lane+32 and one of the 4 halo vectors (64 + lane%4: eight lanes write the
     // same words with the same values -- no lane-dependent branch, the warp never splits): 16 bytes -> 2 words each.
-    // Filter-word kernels: vectors lane and lane+32, and halo word 128 + lane%8 (8 bytes -> 1 word, four lanes alike).
+    // Filter-word kernels: vectors lane and lane+32 (16 bytes -> one code word), and halo half-word 128 + lane%8 (8 bytes ->
+    // 16 bits, four lanes alike).
     static_assert(SCAN_WARP_VECS - 64 == 4 && SCAN_HALO_WORDS == 8, "halo = 4 vectors = 8 words");
     const int v2 = 64 + (lane & 3);
     const int hw = lane & 7;
@@ -894,6 +1129,16 @@ scan_kernel(const __grid_constant__ ScanArgs a)
         }
         if (SCAN_MB_STAGE_ONCE && wt != wt_first) {
             // microbenchmark only: hash the first tile again
+        } else if (PACKED && !FULL) {
+            // the packed words are the code images' words as they stand: group g is code words 2g, 2g + 1 and validity word g
+            sts_u64(sm_addr + 8 * lane, (uint32_t)pc0, (uint32_t)(pc0 >> 32));
+            sts_u64(sm_addr + 8 * hg, (uint32_t)pc1, (uint32_t)(pc1 >> 32));
+            sts_u32(inv_addr + 4 * lane, pm0);
+            sts_u32(inv_addr + 4 * hg, pm1);
+            if (CANON) {
+                sts_u64(smr_addr + 4 * (SCAN_C2_IMAGE - 2 - 2 * lane), revcomp16((uint32_t)(pc0 >> 32)), revcomp16((uint32_t)pc0));
+                sts_u64(smr_addr + 4 * (SCAN_C2_IMAGE - 2 - 2 * hg), revcomp16((uint32_t)(pc1 >> 32)), revcomp16((uint32_t)pc1));
+            }
         } else if (PACKED) {
             const uint4 e0 = expand32(pc0, pm0), e1 = expand32(pc1, pm1);
             *reinterpret_cast<uint4 *>(sm + 4 * lane) = e0;
@@ -910,26 +1155,32 @@ scan_kernel(const __grid_constant__ ScanArgs a)
             // preserve_case) is converted again with the validity test, as is the last tile of a launch, which reaches
             // past stream_len (warp-uniform); bit 3 of a nibble marks a base outside the alphabet as before.
             const bool ragged = base + 16ull * SCAN_WARP_VECS > a.stream_len;
-            uint32_t w0, w1, w2, w3, w4, diff = 0;
+            uint32_t w0, w1, h, v0 = 0, v1 = 0, vh = 0, diff = 0;
             if (!ragged) {
-                w0 = ascii8_to_code_word(q0.x, q0.y, fold, pool, diff); w1 = ascii8_to_code_word(q0.z, q0.w, fold, pool, diff);
-                w2 = ascii8_to_code_word(q1.x, q1.y, fold, pool, diff); w3 = ascii8_to_code_word(q1.z, q1.w, fold, pool, diff);
-                w4 = ascii8_to_code_word(q2.x, q2.y, fold, pool, diff);
+                w0 = __byte_perm(ascii8_to_codes16(q0.x, q0.y, fold, pool, diff), ascii8_to_codes16(q0.z, q0.w, fold, pool, diff), 0x5410);
+                w1 = __byte_perm(ascii8_to_codes16(q1.x, q1.y, fold, pool, diff), ascii8_to_codes16(q1.z, q1.w, fold, pool, diff), 0x5410);
+                h = ascii8_to_codes16(q2.x, q2.y, fold, pool, diff);
             }
             if (ragged || __any_sync(0xFFFFFFFFu, diff != 0)) {
-                w0 = ascii8_to_word(q0.x, q0.y, fold), w1 = ascii8_to_word(q0.z, q0.w, fold);
-                w2 = ascii8_to_word(q1.x, q1.y, fold), w3 = ascii8_to_word(q1.z, q1.w, fold);
-                w4 = ascii8_to_word(q2.x, q2.y, fold);
+                uint32_t n0 = ascii8_to_word(q0.x, q0.y, fold), n1 = ascii8_to_word(q0.z, q0.w, fold);
+                uint32_t n2 = ascii8_to_word(q1.x, q1.y, fold), n3 = ascii8_to_word(q1.z, q1.w, fold);
+                uint32_t n4 = ascii8_to_word(q2.x, q2.y, fold);
                 if (ragged) {
                     const uint64_t o0 = base + 16ull * lane, o1 = o0 + 16ull * 32;
-                    w0 = clip_word(w0, o0, a.stream_len);
-                    w1 = clip_word(w1, o0 + 8, a.stream_len);
-                    w2 = clip_word(w2, o1, a.stream_len);
-                    w3 = clip_word(w3, o1 + 8, a.stream_len);
-                    w4 = clip_word(w4, base + 16ull * 64 + 8ull * hw, a.stream_len);
+                    n0 = clip_word(n0, o0, a.stream_len);
+                    n1 = clip_word(n1, o0 + 8, a.stream_len);
+                    n2 = clip_word(n2, o1, a.stream_len);
+                    n3 = clip_word(n3, o1 + 8, a.stream_len);
+                    n4 = clip_word(n4, base + 16ull * 64 + 8ull * hw, a.stream_len);
                 }
+                w0 = nibbles_to_codes16(n0) | (nibbles_to_codes16(n1) << 16);
+                w1 = nibbles_to_codes16(n2) | (nibbles_to_codes16(n3) << 16);
+                h = nibbles_to_codes16(n4);
+                v0 = nibbles_to_flags8(n0) | (nibbles_to_flags8(n1) << 8);
+                v1 = nibbles_to_flags8(n2) | (nibbles_to_flags8(n3) << 8);
+                vh = nibbles_to_flags8(n4);
             }
-            stage_words<CANON>(sm, smr, lane, hw, w0, w1, w2, w3, w4);
+            stage_codes<CANON>(sm_addr, smr_addr, inv_addr, lane, hw, w0, w1, h, v0, v1, vh);
         } else {
             const uint2 s0 = stage16(q0, base + 16ull * lane, a.stream_len, fold);
             const uint2 s1 = stage16(q1, base + 16ull * (lane + 32), a.stream_len, fold);
@@ -965,6 +1216,8 @@ scan_kernel(const __grid_constant__ ScanArgs a)
         const long long c0 = SCAN_MB_CLOCK ? clock64() : 0;
         static_assert(SCAN_WARP_TILE / 8 == 4 * 32, "a lane's pass mask holds 4 blocks of 8 windows");
         uint32_t pmask = 0;   // filter-word kernels: the lane's pass flags of this tile, see scan_resolve
+        if constexpr (!FULL) pmask = scan_tile_filter<K, CANON>(a, sm_addr, smr_addr, tab_addr, tf);
+        else
 #pragma unroll 1
         for (int g = lane; g < SCAN_WARP_TILE / 8; g += 32) {
             uint32_t b[S::BW], rb[S::BW];
@@ -975,20 +1228,15 @@ scan_kernel(const __grid_constant__ ScanArgs a)
                 for (int i = 0; i < S::BW; i++) rb[i] = lds_u32(smr_addr + 4u * (SCAN_WARP_WORDS - S::BW - g + i));
             }
             const uint32_t local0 = 8u * g;
-            if constexpr (!FULL) {
-                // block i = (g - lane) / 32 ends at bits 8 i .. 8 i + 7 after the tile's 4 trips
-                pmask = (pmask >> 8) | scan_block_filter<K, CANON>(a, b, rb, tf, pool, tail_tab, std::make_integer_sequence<int, 8>());
-            } else {
-                scan_group<K, CANON, 0>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 2>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 4>(a, b, rb, base, local0, tmax, pool, sm);
-                scan_group<K, CANON, 6>(a, b, rb, base, local0, tmax, pool, sm);
-            }
+            scan_group<K, CANON, 0>(a, b, rb, base, local0, tmax, pool, sm, tail_tab);
+            scan_group<K, CANON, 2>(a, b, rb, base, local0, tmax, pool, sm, tail_tab);
+            scan_group<K, CANON, 4>(a, b, rb, base, local0, tmax, pool, sm, tail_tab);
+            scan_group<K, CANON, 6>(a, b, rb, base, local0, tmax, pool, sm, tail_tab);
         }
         if (SCAN_MB_CLOCK) mb_cycles += clock64() - c0;
-        if (!FULL) {
+        if constexpr (!FULL) {
             if (SCAN_MB_NO_SURVIVORS) mb_acc ^= pmask;
-            else if (__any_sync(0xFFFFFFFFu, pmask != 0)) scan_resolve<K, CANON>(a, pmask, sm_addr, base, tmax);
+            else if (__any_sync(0xFFFFFFFFu, pmask != 0)) scan_resolve<K, CANON>(a, pmask, sm_addr, smr_addr, inv_addr, base, tmax);
         }
         __syncwarp();
         if (!FULL && scan_sq_n[warp] >= SCAN_SQ_FLUSH) scan_sq_flush(a);
