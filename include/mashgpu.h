@@ -335,6 +335,29 @@ int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row, uint32_t 
 int mashgpu_dist_spanning_forest_dev(mashgpu_dist_job *job, uint32_t *d_row, uint32_t *d_col, uint32_t *d_numer, uint32_t *d_denom,
                                      double *d_distance, double *d_pvalue, uint64_t *n_edges, uint64_t *n_rounds, void *stream);
 
+/* Greedy dereplication of the component graph above (DESIGN.md 3.12); no counterpart in the reference.  Self jobs (qry == NULL) only;
+ * the lower triangle whatever mashgpu_dist_set_triangle says.  The graph is the one of mashgpu_dist_components: an edge {i, j}, j < i,
+ * for every pair (q = i, r = j) with pass == 1 and numer > 0.  The greedy order is the index order (a caller that wants another order
+ * opens the job over a permuted set):
+ *   representatives: for v = 0 .. n-1, v is a representative iff no representative u < v has an edge {u, v} (the lexicographically
+ *   first maximal independent set);
+ *   assignment: a member m goes to the representative r adjacent to it with the least (distance as a double, min(m, r), max(m, r)),
+ *   the spanning forest's edge order -- its nearest one, ties to the smaller index, later representatives included.  An earlier
+ *   representative is always adjacent, so every member has one.
+ * Outputs of n_qry entries: rep[i] = sketch i's representative, i itself for a representative; for a member, numer, denom, distance
+ * and pvalue bit-identical to what mashgpu_dist_run returns for (q = max(i, rep[i]), r = min(i, rep[i])), for a representative zeros.
+ * *n_reps = number of representatives, *n_rounds = resolution rounds over all blocks (at most the rows of each block).  The result
+ * depends only on the grid: not on the merge path, the prefilter, the block size or the run.  Memory: O(n) plus one block's
+ * rows x rows bit matrix.  0 or 1 sketches give the identity and 0 rounds.  A job with a separate query set and NULL outputs are
+ * MASHGPU_ERR_INVALID, an encoded job MASHGPU_ERR_UNSUPPORTED.  Synchronises the stream. */
+int mashgpu_dist_representatives(mashgpu_dist_job *job, uint32_t *rep, uint32_t *numer, uint32_t *denom, double *distance, double *pvalue,
+                                 uint64_t *n_reps, uint64_t *n_rounds);
+int mashgpu_dist_representatives_dev(mashgpu_dist_job *job, uint32_t *d_rep, uint32_t *d_numer, uint32_t *d_denom, double *d_distance,
+                                     double *d_pvalue, uint64_t *n_reps, uint64_t *n_rounds, void *stream);
+/* Rows of one block of the representatives' first pass (each block is one lower-triangle run followed by its resolve rounds).
+ * 0 = default, min(2^31 / n, 32768); larger values are cut to 32768 (a 128 MiB bit matrix).  The result does not depend on it. */
+int mashgpu_dist_set_representative_block(mashgpu_dist_job *job, uint64_t rows);
+
 /* Neighbor joining (DESIGN.md 3.10); no counterpart in the reference.  Canonical Saitou-Nei / Studier-Keppler NJ over a symmetric
  * n x n float64 matrix D of which only the lower triangle (j < i) is read, with the operation order fixed so that it is
  * reproducible bit for bit (tests/nj_model.py):

@@ -128,6 +128,10 @@ def load_library():
     L.mashgpu_dist_spanning_forest.argtypes = [C.c_void_p, u32p, u32p, u32p, u32p, f64p, f64p, u64p, u64p]
     L.mashgpu_dist_spanning_forest_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    u64p, u64p, C.c_void_p]
+    L.mashgpu_dist_representatives.argtypes = [C.c_void_p, u32p, u32p, u32p, f64p, f64p, u64p, u64p]
+    L.mashgpu_dist_representatives_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, u64p, u64p,
+                                                   C.c_void_p]
+    L.mashgpu_dist_set_representative_block.argtypes = [C.c_void_p, C.c_uint64]
     L.mashgpu_dist_neighbor_joining.argtypes = [C.c_void_p, u32p, f64p]
     L.mashgpu_neighbor_joining_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, u32p, f64p, C.c_void_p]
     L.mashgpu_dist_linkage.argtypes = [C.c_void_p, C.c_int, u32p, u32p, f64p, u32p, u64p]
@@ -579,6 +583,34 @@ class DistJob:
         self.eng._check(self.eng.lib.mashgpu_dist_spanning_forest_dev(self.h, d_row, d_col, d_numer, d_denom, d_distance, d_pvalue,
                                                                       C.byref(n), C.byref(rounds), stream))
         return n.value, rounds.value
+
+    def representatives(self):
+        """Greedy dereplication (DESIGN.md 3.12) of the graph of components(), in index order: sketch v is a representative iff no
+        representative u < v has an edge {u, v}, and every other sketch goes to its adjacent representative of least (distance, smaller
+        index, larger index).  A dict of rep (uint32, i itself for a representative), numer, denom, distance, pvalue (run()'s values for
+        (q = max(i, rep), r = min(i, rep)), zeros for a representative), plus "n_reps" and "rounds".  Self jobs only."""
+        n = self.n_qry
+        out = {"rep": np.zeros(n, np.uint32), "numer": np.zeros(n, np.uint32), "denom": np.zeros(n, np.uint32),
+               "distance": np.zeros(n, np.float64), "pvalue": np.zeros(n, np.float64)}
+        reps, rounds = C.c_uint64(0), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_representatives(self.h, _p(out["rep"], u32p), _p(out["numer"], u32p), _p(out["denom"], u32p),
+                                                                  _p(out["distance"], f64p), _p(out["pvalue"], f64p), C.byref(reps),
+                                                                  C.byref(rounds)))
+        out["n_reps"] = reps.value
+        out["rounds"] = rounds.value
+        return out
+
+    def representatives_dev(self, d_rep, d_numer, d_denom, d_distance, d_pvalue, stream=None):
+        """representatives() into device arrays of n_qry entries (uint32 rep, numer, denom; float64 distance, pvalue); returns
+        (n_reps, rounds)."""
+        reps, rounds = C.c_uint64(0), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_representatives_dev(self.h, d_rep, d_numer, d_denom, d_distance, d_pvalue, C.byref(reps),
+                                                                      C.byref(rounds), stream))
+        return reps.value, rounds.value
+
+    def set_representative_block(self, rows):
+        """Rows of one first-pass block of representatives() (0 = default, at most 32768); the result does not depend on it."""
+        self.eng._check(self.eng.lib.mashgpu_dist_set_representative_block(self.h, int(rows)))
 
     def neighbor_joining(self):
         """Neighbor-joining tree (DESIGN.md 3.10) of every pair's distance of a self job, D(i, j) = run()'s distance at (q = i, r = j),

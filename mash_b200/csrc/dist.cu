@@ -24,6 +24,9 @@
 // of every hit of the lower triangle into a forest, whose roots become the components' labels.
 // A spanning-forest run (mashgpu_dist_spanning_forest, DESIGN.md 3.9) repeats such runs in Boruvka rounds: at the same places
 // dist_msf.cuh offers every hit to the cheapest-edge slots of its two components.
+// Greedy dereplication (mashgpu_dist_representatives, DESIGN.md 3.12) runs the query rows in blocks, strictly in order: at the same
+// places dist_greedy.cuh marks rows covered by earlier representatives and records each block's own edges in a bit matrix, which
+// greedy_resolve_kernel decides in rounds; one more run offers each member its nearest representative.
 // Neighbor joining (mashgpu_dist_neighbor_joining, DESIGN.md 3.10) and average / complete linkage (mashgpu_dist_linkage, 3.11)
 // fill an n x n matrix with plain lower-triangle runs (distance output only) and hand it to nj.cu or linkage.cu.
 #include <algorithm>
@@ -42,6 +45,7 @@
 #include "dist_best.cuh"
 #include "dist_cc.cuh"
 #include "dist_msf.cuh"
+#include "dist_greedy.cuh"
 
 namespace mashgpu {
 
@@ -673,19 +677,50 @@ __global__ void __launch_bounds__(256) dist_kernel_general(const DistArgs a)
     dist_emit(a, q, r, cd.x, cd.y, a.ref_len[r]);
 }
 
-// Values of the spanning forest's edges, once after its last round: the sequential merge of dist_kernel_general and the arithmetic
-// of dist_emit / dist_fix_kernel, so every value is the one a dense run returns for (q = i, r = j - tri_r0).  Every forest edge
-// shares a hash, so its p-value is the binomial tail.  `lo` holds the edges (j << 32 | i) in forest order.
+// The values of a graph edge (q, r) recomputed on its own: the sequential merge of dist_kernel_general and the arithmetic of dist_emit /
+// dist_fix_kernel, so every value is the one a dense run returns for (q, r).  Every edge shares a hash, so its p-value is the binomial
+// tail.
+__device__ __forceinline__ void dist_edge_values(const DistArgs &a, uint32_t q, uint32_t r, uint32_t *numer, uint32_t *denom, double *distance,
+                                                 double *pvalue)
+{
+    const uint2 cd = dist_merge_pair(a, q, r);
+    *numer = cd.x; *denom = cd.y;
+    *distance = (cd.y == a.S) ? a.dist_lut[cd.x] : mash_distance(cd.x, cd.y, a.kmer_size);
+    *pvalue = mash_pvalue(cd.x, a.ref_len[r], a.qry_len[q], a.kmer_space, cd.y, &a.binom);
+}
+
+// Values of the spanning forest's edges, once after its last round, for (q = i, r = j - tri_r0).  `lo` holds the edges (j << 32 | i)
+// in forest order.
 __global__ void __launch_bounds__(256) msf_values_kernel(const DistArgs a, const unsigned long long *lo, uint64_t m, uint32_t *row,
                                                          uint32_t *col, uint32_t *numer, uint32_t *denom, double *distance, double *pvalue)
 {
     const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (t >= m) return;
-    const uint32_t q = (uint32_t)lo[t], j = (uint32_t)(lo[t] >> 32), r = j - a.tri_r0;
-    const uint2 cd = dist_merge_pair(a, q, r);
-    row[t] = q; col[t] = j; numer[t] = cd.x; denom[t] = cd.y;
-    distance[t] = (cd.y == a.S) ? a.dist_lut[cd.x] : mash_distance(cd.x, cd.y, a.kmer_size);
-    pvalue[t] = mash_pvalue(cd.x, a.ref_len[r], a.qry_len[q], a.kmer_space, cd.y, &a.binom);
+    const uint32_t q = (uint32_t)lo[t], j = (uint32_t)(lo[t] >> 32);
+    row[t] = q; col[t] = j;
+    dist_edge_values(a, q, j - a.tri_r0, numer + t, denom + t, distance + t, pvalue + t);
+}
+
+// The outputs of greedy dereplication, one thread per sketch of a self job: a representative is its own with zero values; a member's
+// representative is the other end of the key in its slot, and its values are those of that edge.  counters[1] counts the
+// representatives; counters[2] |= 2 for a member without a slot (cannot happen: an earlier representative is always adjacent).
+__global__ void __launch_bounds__(256) greedy_values_kernel(const DistArgs a, const uint32_t *status, const MsfKey *slot, uint64_t n, uint32_t *rep,
+                                                           uint32_t *numer, uint32_t *denom, double *distance, double *pvalue,
+                                                           unsigned long long *counters)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const MsfKey k = slot[t];
+    const bool is_rep = status[t] & GREEDY_REP;
+    if (is_rep || k.hi == MSF_NONE) {
+        rep[t] = (uint32_t)t; numer[t] = 0; denom[t] = 0; distance[t] = 0.0; pvalue[t] = 0.0;
+        if (is_rep) atomicAdd(counters + 1, 1ull);
+        else atomicOr(counters + 2, 2ull);
+        return;
+    }
+    const uint32_t q = (uint32_t)k.lo, r = (uint32_t)(k.lo >> 32);
+    rep[t] = q == (uint32_t)t ? r : q;
+    dist_edge_values(a, q, r, numer + t, denom + t, distance + t, pvalue + t);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -803,6 +838,7 @@ struct mashgpu_dist_job {
     double best_select_ms = 0;
     std::vector<EventPair> best_events;
     DevBuf<unsigned long long> cc_edges;        // edge counter of mashgpu_dist_components_dev
+    uint64_t greedy_block = 0;          // mashgpu_dist_set_representative_block; 0 = default
     // prefilter (dist_probe_kernel): -1 = auto (on; switched off when most combinations turn out to share hashes), 0 = off, 1 = on
     int prefilter_mode = -1;
     bool triangle = false;
@@ -1588,22 +1624,36 @@ static int need_self_or_encoded(mashgpu_dist_job *job, const char *what)
     return job->self || job->encoded ? MASHGPU_OK : fail(job->ctx, MASHGPU_ERR_INVALID, "%s a self comparison (qry == NULL) or an encoded job", what);
 }
 
-// Runs every pair of the lower triangle of a self or encoded job once, in blocks of TRIANGLE_RUN_PAIRS / n_ref queries, with the capture
-// that set_target puts into each run's arguments.  Lower triangle whatever the job's own setting: query q meets the rows below it
-// only, so the queries up to the first reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
-template <class SetTarget>
-static int enqueue_lower_triangle(mashgpu_dist_job *job, cudaStream_t st, SetTarget set_target)
+// Queries of one lower-triangle run by default
+static uint64_t triangle_block(const mashgpu_dist_job *job)
+{
+    return std::max<uint64_t>(1, TRIANGLE_RUN_PAIRS / std::max<uint64_t>(job->n_ref, 1));
+}
+
+// Runs every pair of the lower triangle of a self or encoded job once, in blocks of `block` queries (0: triangle_block), with the capture
+// that set_target puts into each run's arguments; after_run(a) enqueues what follows each block's run (greedy dereplication resolves the
+// block there).  Lower triangle whatever the job's own setting: query q meets the rows below it only, so the queries up to the first
+// reference row have no pair at all.  Nothing can overflow, so no block is ever run twice.
+template <class SetTarget, class AfterRun>
+static int enqueue_lower_triangle(mashgpu_dist_job *job, cudaStream_t st, SetTarget set_target, uint64_t block, AfterRun after_run)
 {
     const uint64_t n = job->n_qry, n_ref = job->n_ref;
     const uint64_t q_first = job->self ? 1 : job->ref_row0 + 1;
-    const uint64_t block = std::max<uint64_t>(1, TRIANGLE_RUN_PAIRS / std::max<uint64_t>(n_ref, 1));
+    if (block == 0) block = triangle_block(job);
     for (uint64_t q0 = q_first; n_ref && q0 < n; q0 += block) {
         DistArgs a = dist_args(job, q0, std::min(block, n - q0));
         a.triangle = 1;
         set_target(a);
         MG_TRY(dist_enqueue(job, a, st));
+        MG_TRY(after_run(a));
     }
     return MASHGPU_OK;
+}
+
+template <class SetTarget>
+static int enqueue_lower_triangle(mashgpu_dist_job *job, cudaStream_t st, SetTarget set_target)
+{
+    return enqueue_lower_triangle(job, st, set_target, 0, [](const DistArgs &) { return (int)MASHGPU_OK; });
 }
 
 extern "C" int mashgpu_dist_components_dev(mashgpu_dist_job *job, uint32_t *d_labels, uint64_t *n_edges, void *stream)
@@ -1741,6 +1791,111 @@ extern "C" int mashgpu_dist_spanning_forest(mashgpu_dist_job *job, uint32_t *row
     MG_CUDA(ctx, cudaMemcpyAsync(denom, d32.p + 3 * cap, m * 4, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaMemcpyAsync(distance, d64.p, m * 8, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaMemcpyAsync(pvalue, d64.p + cap, m * 8, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    return MASHGPU_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Greedy dereplication (DESIGN.md 3.12)
+// ---------------------------------------------------------------------------------------------------------
+extern "C" int mashgpu_dist_set_representative_block(mashgpu_dist_job *job, uint64_t rows)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    job->greedy_block = std::min<uint64_t>(rows, GREEDY_MAX_BLOCK);
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_representatives_dev(mashgpu_dist_job *job, uint32_t *d_rep, uint32_t *d_numer, uint32_t *d_denom, double *d_distance,
+                                                double *d_pvalue, uint64_t *n_reps, uint64_t *n_rounds, void *stream)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "representatives of an encoded (sharded) job");
+    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "representatives need a self comparison (qry == NULL)");
+    if (!d_rep || !d_numer || !d_denom || !d_distance || !d_pvalue || !n_reps || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_reps = 0; *n_rounds = 0;
+    const uint64_t n = job->n_qry;
+    if (n == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = stream ? (cudaStream_t)stream : ctx->stream;
+    // pass-1 blocks of `block` rows from row 1 (sketch 0 is a representative from the start), each with its GreedyRun header; one
+    // header more for pass 2
+    const uint64_t block = std::min<uint64_t>({job->greedy_block ? job->greedy_block : triangle_block(job), GREEDY_MAX_BLOCK, std::max<uint64_t>(n - 1, 1)});
+    const uint64_t pitch = (block + 31) / 32, n_blocks = (n - 1 + block - 1) / block;
+    // O(n) state plus one block's bit matrix, its two pairs of row sets and the rows' extents
+    DevBuf<uint32_t> status, bits, masks, extent; DevBuf<MsfKey> slot; DevBuf<GreedyRun> runs; DevBuf<int> ctl; DevBuf<unsigned long long> counters;
+    if (status.alloc(n) != cudaSuccess || slot.alloc(n) != cudaSuccess || runs.alloc(n_blocks + 1) != cudaSuccess || counters.alloc(3) != cudaSuccess ||
+        (n_blocks && (bits.alloc(block * pitch) != cudaSuccess || masks.alloc(4 * pitch) != cudaSuccess || extent.alloc(2 * block) != cudaSuccess ||
+                      ctl.alloc(6) != cudaSuccess)))
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (representatives of %llu sketches in blocks of %llu)", (unsigned long long)n,
+                    (unsigned long long)block);
+    std::vector<GreedyRun> h_runs(n_blocks + 1);
+    for (uint64_t b = 0; b < n_blocks; b++) h_runs[b] = GreedyRun{status.p, bits.p, nullptr, (uint32_t)(1 + b * block), (uint32_t)pitch};
+    h_runs[n_blocks] = GreedyRun{status.p, nullptr, slot.p, 0, 0};
+    MG_CUDA(ctx, cudaMemcpyAsync(runs.p, h_runs.data(), h_runs.size() * sizeof(GreedyRun), cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemsetAsync(counters.p, 0, 3 * 8, st));
+    MG_CUDA(ctx, cudaMemsetAsync(slot.p, 0xFF, n * sizeof(MsfKey), st));
+    if (n_blocks) MG_CUDA(ctx, cudaMemsetAsync(bits.p, 0, block * pitch * 4, st));
+    greedy_init_kernel<<<blocks_for(n), 256, 0, st>>>(status.p, n);
+    MG_CUDA(ctx, cudaGetLastError());
+    ctx->kernel_launches++;
+    int per_sm = 0;
+    MG_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, greedy_resolve_kernel, GREEDY_THREADS, 0));
+    // pass 1: each block's run, then its resolve (one cooperative launch), then the matrix cleared for the next block
+    auto resolve = [&](const DistArgs &a) -> int {
+        GreedyResolve p{bits.p, (uint32_t)pitch, a.q_count, a.q_begin, status.p, masks.p, masks.p + 2 * pitch, extent.p, extent.p + block, ctl.p,
+                        counters.p};
+        MG_CUDA(ctx, cudaMemsetAsync(ctl.p, 0, 3 * 4, st));
+        MG_CUDA(ctx, cudaMemsetAsync(ctl.p + 3, 0xFF, 3 * 4, st));
+        const uint64_t warps_needed = (a.q_count + 31) / 32;
+        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)per_sm * ctx->sm_count,
+                                                                                 (warps_needed * 32 + GREEDY_THREADS - 1) / GREEDY_THREADS));
+        void *args[] = {&p};
+        MG_CUDA(ctx, cudaLaunchCooperativeKernel((const void *)greedy_resolve_kernel, grid, GREEDY_THREADS, args, 0, st));
+        MG_CUDA(ctx, cudaMemsetAsync(bits.p, 0, (uint64_t)a.q_count * pitch * 4, st));
+        ctx->kernel_launches++;
+        return MASHGPU_OK;
+    };
+    MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) {
+        a.graph = GraphCapture{reinterpret_cast<uint32_t *>(runs.p + (a.q_begin - 1) / block), nullptr, nullptr};
+    }, block, resolve));
+    // pass 2: every member's nearest representative, at the default run size
+    MG_TRY(enqueue_lower_triangle(job, st, [&](DistArgs &a) { a.graph = GraphCapture{reinterpret_cast<uint32_t *>(runs.p + n_blocks), nullptr, nullptr}; }));
+    greedy_values_kernel<<<blocks_for(n), 256, 0, st>>>(dist_args(job, 0, n), status.p, slot.p, n, d_rep, d_numer, d_denom, d_distance, d_pvalue,
+                                                         counters.p);
+    MG_CUDA(ctx, cudaGetLastError());
+    ctx->kernel_launches++;
+    unsigned long long c[3] = {0, 0, 0};
+    MG_CUDA(ctx, cudaMemcpyAsync(c, counters.p, sizeof c, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));        // the state and the headers go out of scope
+    if (c[2] & 1) return fail(ctx, MASHGPU_ERR_CUDA, "internal error: a block of representatives not resolved in as many rounds as rows");
+    if (c[2] & 2) return fail(ctx, MASHGPU_ERR_CUDA, "internal error: a sketch with neither a representative status nor a representative");
+    *n_reps = c[1]; *n_rounds = c[0];
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_representatives(mashgpu_dist_job *job, uint32_t *rep, uint32_t *numer, uint32_t *denom, double *distance, double *pvalue,
+                                            uint64_t *n_reps, uint64_t *n_rounds)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "representatives of an encoded (sharded) job");
+    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "representatives need a self comparison (qry == NULL)");
+    if (!rep || !numer || !denom || !distance || !pvalue || !n_reps || !n_rounds) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    *n_reps = 0; *n_rounds = 0;
+    const uint64_t n = job->n_qry;
+    if (n == 0) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    DevBuf<uint32_t> d32; DevBuf<double> d64;
+    if (d32.alloc(3 * n) != cudaSuccess || d64.alloc(2 * n) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (representatives of %llu sketches)", (unsigned long long)n);
+    MG_TRY(mashgpu_dist_representatives_dev(job, d32.p, d32.p + n, d32.p + 2 * n, d64.p, d64.p + n, n_reps, n_rounds, ctx->stream));
+    cudaStream_t st = ctx->stream;
+    MG_CUDA(ctx, cudaMemcpyAsync(rep, d32.p, n * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(numer, d32.p + n, n * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(denom, d32.p + 2 * n, n * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(distance, d64.p, n * 8, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(pvalue, d64.p + n, n * 8, cudaMemcpyDeviceToHost, st));
     MG_CUDA(ctx, cudaStreamSynchronize(st));
     return MASHGPU_OK;
 }

@@ -3,9 +3,9 @@
 // The graph is the component graph of dist_cc.cuh: one vertex per sketch, an edge {i, j} (j < i) for every pair of the lower
 // triangle that passes (-d / -v) and shares a hash.  Edges are ordered by the strict total order (distance, j, i), so the forest is
 // unique.  It is built in Boruvka rounds without an edge list.  In a round every pair's capture offers its edge to the cheapest-edge
-// slot of both endpoints' components (dist_msf_offer, at the places where dist_cc_union is called); msf_hook_kernel then adds each
-// component's cheapest edge to the forest and joins the two components with dist_cc.cuh's union-find, and cc_flatten_kernel turns the
-// forest into the next round's labels.  The edge values are recomputed for the <= n - 1 forest edges after the last round.
+// slot of both endpoints' components (dist_graph_hit in dist_greedy.cuh, at the places where dist_cc_union is called); msf_hook_kernel
+// then adds each component's cheapest edge to the forest and joins the two components with dist_cc.cuh's union-find, and
+// cc_flatten_kernel turns the forest into the next round's labels.  The edge values are recomputed for the <= n - 1 forest edges after the last round.
 // The reference has no counterpart (its users build single linkage from the output of `mash triangle -E`).
 #pragma once
 #include <cstdint>
@@ -25,13 +25,14 @@ __device__ __forceinline__ bool msf_less(const MsfKey &x, const MsfKey &y)
     return x.hi < y.hi || (x.hi == y.hi && x.lo < y.lo);
 }
 
-// Capture target of the graph runs inside DistArgs; forest == nullptr outside them.  One struct for both kinds of run: the hit is
-// one not-inlined call with as few argument registers as possible (see dist_graph_hit).
+// Capture target of the graph runs inside DistArgs; forest == nullptr outside them.  One struct for every kind of run: the hit is
+// one not-inlined call with as few argument registers as possible (see dist_graph_hit, dist_greedy.cuh).  The kind follows from
+// which of edges and best are set: component runs set edges, spanning-forest rounds set best, greedy runs set neither.
 struct GraphCapture {
     uint32_t *forest;               // component runs: the union-find forest (dist_cc.cuh); spanning-forest rounds: the component
-                                    // (root) of every vertex, read-only during the round
-    unsigned long long *edges;      // component runs: the edge counter; nullptr in spanning-forest rounds
-    MsfKey *best;                   // spanning-forest rounds: per component root, the cheapest edge offered to it; nullptr in component runs
+                                    // (root) of every vertex, read-only during the round; greedy runs: their GreedyRun header
+    unsigned long long *edges;      // component runs: the edge counter; nullptr otherwise
+    MsfKey *best;                   // spanning-forest rounds: per component root, the cheapest edge offered to it; nullptr otherwise
 };
 
 __device__ __forceinline__ unsigned long long msf_load_u64(const unsigned long long *p)
@@ -58,24 +59,12 @@ __device__ __forceinline__ void msf_lower(MsfKey *slot, const MsfKey k)
     }
 }
 
-// Offers the edge {i, j} (j = r_global < i = q) at distance `dist` to the components of both endpoints.
-__device__ __forceinline__ void dist_msf_offer(const uint32_t *label, MsfKey *best, uint32_t i, uint32_t j, double dist)
+// The key of the edge {i, j}, j < i, at distance `dist`
+__device__ __forceinline__ MsfKey msf_key(uint32_t i, uint32_t j, double dist)
 {
-    const uint32_t a = __ldg(label + i), b = __ldg(label + j);
-    if (a == b) return;
-    const MsfKey k{((unsigned long long)j << 32) | i, dist == 0.0 ? 0ull : (unsigned long long)__double_as_longlong(dist)};
-    msf_lower(best + a, k);
-    msf_lower(best + b, k);
+    return MsfKey{((unsigned long long)j << 32) | i, dist == 0.0 ? 0ull : (unsigned long long)__double_as_longlong(dist)};
 }
 
-// A hit (pass, shared hash) of a component run or of a spanning-forest round.  Not inlined, like dist_best_append: the merge
-// kernels' epilogues keep their register allocation.  One call for both kinds of run: a second call site in dist_emit, or a second
-// capture among the arguments, costs dist_kernel registers beyond its allocation granule.
-__device__ __noinline__ void dist_graph_hit(const GraphCapture g, uint32_t q, uint32_t r_global, double dist)
-{
-    if (g.best) dist_msf_offer(g.forest, g.best, q, r_global, dist);
-    else dist_cc_union(g.forest, g.edges, q, r_global);
-}
 
 // One thread per vertex; the roots act.  A root's cheapest edge joins it to another component o.  When o picked the same edge (a
 // mutual pick) only the smaller of the two roots records it.  Under a strict order the picked edges form a forest, every one of them

@@ -6,7 +6,8 @@
 // help text, `bounds` and `find` are out of scope.  `triangle -G` (clusters) and `triangle -T` (the single-linkage tree as a minimum
 // spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.  Nor has `triangle -N` (the
 // neighbor-joining tree as a Newick line), which its users compute from the matrix with an NJ program, nor `triangle -L` (average
-// or complete linkage as a Newick line, or its flat clusters at `-d`), which its users compute from the matrix with scipy.
+// or complete linkage as a Newick line, or its flat clusters at `-d`), which its users compute from the matrix with scipy, nor
+// `triangle -R` (greedy representatives, the dereplication of CD-HIT and skDER), which its users run over the `-E` output.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -541,13 +542,23 @@ static void writeNewickLine(const Sketch &sketch, bool comment, const vector<uin
     fflush(stdout);
 }
 
-// the self job over every sketch, with the -d / -v thresholds
-static mashgpu_dist_job *openSelfJob(const Sketch &sketch, double distanceMax, double pValueMax)
+// the self job over every sketch, with the -d / -v thresholds; with `order`, job row t is sketch order[t]
+static mashgpu_dist_job *openSelfJob(const Sketch &sketch, double distanceMax, double pValueMax, const vector<uint32_t> *order = nullptr)
 {
     mashgpu_dist_params dp = {(uint64_t)sketch.getMinHashesPerWindow(), sketch.getKmerSize(), sketch.getKmerSpace(), distanceMax, pValueMax};
     mashgpu_sketch_set set;
     vector<uint64_t> h, l; vector<uint32_t> nn;
     sketch.toSketchSet(set, h, nn, l);
+    if (order) {
+        vector<uint64_t> ph(h.size()), pl(l.size()); vector<uint32_t> pn(nn.size());
+        for (uint64_t t = 0; t < order->size(); t++) {
+            const uint64_t i = (*order)[t];
+            std::copy(h.begin() + i * set.stride, h.begin() + (i + 1) * set.stride, ph.begin() + t * set.stride);
+            pn[t] = nn[i]; pl[t] = l[i];
+        }
+        h.swap(ph); nn.swap(pn); l.swap(pl);
+        set.hashes = h.data(); set.n_hashes = nn.data(); set.length = l.data();
+    }
     mashgpu_dist_job *job = 0;
     if (mashgpu_dist_open(gpuContext(), &set, 0, &dp, &job) != MASHGPU_OK) gpuFail();
     return job;
@@ -635,6 +646,33 @@ static void writeLinkage(mashgpu_dist_job *job, const Sketch &sketch, bool comme
     cerr << "Tree: " << n << " leaves, " << m << " merges, " << rows << " rows rescanned" << endl;
 }
 
+// `mash triangle -R length|input`: greedy dereplication (DESIGN.md 3.12) in priority order -- longest sketch first (ties by input
+// position), or input order.  A sketch is a representative unless a representative before it has a pair with it that passes -d / -v
+// and shares a hash; every other sketch goes to its nearest adjacent representative.  The job runs over the sketches in priority order;
+// the lines are in input order: name, its representative's name (itself for a representative) and the distance to it.
+static void writeRepresentatives(const Sketch &sketch, bool comment, bool byLength, double distanceMax, double pValueMax, int threads)
+{
+    const uint64_t n = sketch.getReferenceCount();
+    vector<uint32_t> order(n);
+    for (uint64_t i = 0; i < n; i++) order[i] = (uint32_t)i;
+    if (byLength)
+        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return sketch.getReference(a).length > sketch.getReference(b).length; });
+    mashgpu_dist_job *job = openSelfJob(sketch, distanceMax, pValueMax, &order);
+    vector<uint32_t> rep(n), numer(n), denom(n);
+    vector<double> distance(n), pValue(n);
+    uint64_t reps = 0, rounds = 0;
+    if (n && mashgpu_dist_representatives(job, rep.data(), numer.data(), denom.data(), distance.data(), pValue.data(), &reps, &rounds) != MASHGPU_OK)
+        gpuFail();
+    mashgpu_dist_close(job);
+    vector<uint32_t> repOf(n);              // in input order
+    vector<double> distOf(n);
+    for (uint64_t t = 0; t < n; t++) { repOf[order[t]] = order[rep[t]]; distOf[order[t]] = distance[t]; }
+    mashhost::writeRows(n, threads, 1, [&](uint64_t i, mashhost::OutBuf &o) {
+        o.str(sketchLabel(sketch, i, comment)); o.ch('\t'); o.str(sketchLabel(sketch, repOf[i], comment)); o.ch('\t'); o.dbl(distOf[i]); o.ch('\n');
+    });
+    cerr << "Representatives: " << reps << " of " << n << " sketches in " << rounds << " rounds" << endl;
+}
+
 int runTriangle(int argc, const char **argv)
 {
     Command c;
@@ -646,6 +684,7 @@ int runTriangle(int argc, const char **argv)
     c.add("tree", Option(Option::Boolean, "T", ""));          // not an option of the reference either
     c.add("nj", Option(Option::Boolean, "N", ""));            // nor is this one
     c.add("linkage", Option(Option::String, "L", ""));        // nor this one
+    c.add("representatives", Option(Option::String, "R", ""));        // nor this one
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
     c.add("distance", Option(Option::Number, "d", "1.0", 0., 1.));
     c.useSketchOptions();
@@ -656,7 +695,8 @@ int runTriangle(int argc, const char **argv)
              << "  -T        Single-linkage tree: the minimum spanning forest of the -G graph by distance, as -E lines in order of distance (not with" << endl
              << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl
              << "  -N        Neighbor-joining tree of every pair's distance, as one Newick line (not with -E, -G, -T, -d or -v)." << endl
-             << "  -L <m>    Average or complete linkage (m = average or complete) of every pair's distance as one Newick line; with -d t, per sketch its cluster at height <= t (not with -E, -G, -T, -N or -v)." << endl;
+             << "  -L <m>    Average or complete linkage (m = average or complete) of every pair's distance as one Newick line; with -d t, per sketch its cluster at height <= t (not with -E, -G, -T, -N or -v)." << endl
+             << "  -R <o>    Greedy representatives in order o (length: longest first, input: input order): a sketch is one unless an earlier one is within -d / -v; per sketch its representative, the nearest, and the distance (not with -E, -G, -T, -N or -L)." << endl;
         return 0;
     }
     bool comment = c.opt("comment").active, edge = c.opt("edge").active, cluster = c.opt("cluster").active, tree = c.opt("tree").active;
@@ -667,6 +707,12 @@ int runTriangle(int argc, const char **argv)
         linkMethod = m == "average" ? MASHGPU_LINKAGE_AVERAGE : m == "complete" ? MASHGPU_LINKAGE_COMPLETE : -1;
         if (linkMethod < 0) { cerr << "ERROR: The argument to -L must be average or complete (" << m << " given)." << endl; return 1; }
     }
+    const bool reps = c.opt("representatives").active;
+    const string &repOrder = c.opt("representatives").argument;
+    if (reps && repOrder != "length" && repOrder != "input") {
+        cerr << "ERROR: The argument to -R must be length or input (" << repOrder << " given)." << endl;
+        return 1;
+    }
     // the output modes that replace the matrix, and the options each refuses, in the order they are checked
     const struct { const char *mode, *refused[5], *why; } conflicts[] = {
         {"cluster", {"edge"}, "clusters replace the edge list"},
@@ -674,6 +720,7 @@ int runTriangle(int argc, const char **argv)
         {"tree", {"cluster"}, "cut the forest at the distance instead"},
         {"linkage", {"edge", "cluster", "tree", "nj", "pvalue"}, "the tree is built from every pair's distance; -d cuts it"},
         {"nj", {"edge", "cluster", "tree", "distance", "pvalue"}, "the tree is built from every pair's distance"},
+        {"representatives", {"edge", "cluster", "tree", "nj", "linkage"}, "the representatives replace the edge list, clusters and trees"},
     };
     for (const auto &t : conflicts)
         for (const char *o : t.refused)
@@ -682,7 +729,7 @@ int runTriangle(int argc, const char **argv)
                 return 1;
             }
     double pValueMax = c.opt("pvalue").number, distanceMax = c.opt("distance").number, pValuePeak = 0;
-    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree && !link) edge = true;
+    if ((c.opt("pvalue").active || c.opt("distance").active) && !cluster && !tree && !link && !reps) edge = true;
     Sketch::Parameters parameters;
     if (sketchParameterSetup(parameters, c)) return 1;
     if (c.arguments.size() == 1 && !c.opt("list").active) parameters.concatenated = false;
@@ -693,6 +740,11 @@ int runTriangle(int argc, const char **argv)
     KmerWarning w;
     w.scan(sketch, parameters);
     const uint64_t n = sketch.getReferenceCount();
+    if (reps) {
+        writeRepresentatives(sketch, comment, repOrder == "length", distanceMax, pValueMax, parameters.parallelism);
+        if (w.warningCount > 0 && !parameters.reads) warnKmerSize(parameters, w.lengthMax, w.lengthMaxName, w.randomChance, w.kMin, w.warningCount);
+        return 0;
+    }
     if (cluster || tree || nj || link) {
         mashgpu_dist_job *job = openSelfJob(sketch, distanceMax, pValueMax);
         // the cut is the -d argument read as a double, so that -d 0.1 cuts where fcluster(Z, 0.1, "distance") does (-d itself is a float)
