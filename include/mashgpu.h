@@ -412,6 +412,31 @@ int mashgpu_linkage_matrix(mashgpu_ctx *ctx, double *d_matrix, uint64_t n, uint6
  * MASHGPU_ERR_UNSUPPORTED.  8 n^2 bytes beyond the device's free memory: MASHGPU_ERR_NOMEM before anything is allocated. */
 int mashgpu_dist_linkage(mashgpu_dist_job *job, int method, uint32_t *id_lo, uint32_t *id_hi, double *height, uint32_t *size,
                          uint64_t *rows_rescanned);
+/* The flat clusters of mashgpu_dist_linkage's tree cut at height t (DESIGN.md 3.13), without the n x n matrix: memory and time scale
+ * with the largest component of the graph below, not with n.  labels[i] (n_qry entries) = the smallest index in sketch i's flat
+ * cluster, scipy's fcluster(Z, t, "distance") of the whole set's Z: a maximal subtree whose largest merge height is <= t.
+ * With T = t (1 + 8 n 2^-53) rounded up and T < 1, the set splits into the components of the pairs at distance <= T: those that share
+ * a hash (mashgpu_dist_components at max_distance T, no p-value test) and the pairs of empty sketches (distance 0); every other pair
+ * is at distance 1.  No merge at height <= t joins two of these components, so the cut of each
+ * component's own linkage (the same definition and arithmetic, over its members in index order) is the whole set's cut there, bit
+ * for bit, ties included.  With T >= 1 the whole set is one component.  A component of up to a few hundred members is linked inside
+ * one CTA; a larger one through an m x m device matrix and mashgpu_linkage_matrix, with the same merges.
+ * Optional merge forest (id_lo, id_hi, height, size: all NULL or all given, max(n_qry - 1, 0) entries each): each component's own
+ * linkage in scipy's Z layout, leaves = sketch indices, merge s = node n_qry + s; the first n_qry - *n_components entries are written,
+ * grouped by component in the order of its smallest member and in merge order within one.  Merges at height <= t are the whole
+ * set's merges (heights bit-identical); merges above t are the component's own linkage, not the whole set's.
+ * *n_clusters = number of flat clusters, *n_components = components (singletons included), *largest_component = its members.
+ * The job's max_distance, max_pvalue and mashgpu_dist_set_triangle are ignored and left unchanged.  0 or 1 sketches give the
+ * identity.  A job with a separate query set, NULL required outputs, a partial forest, an unknown method, or t NaN or negative:
+ * MASHGPU_ERR_INVALID; an encoded (sharded) job: MASHGPU_ERR_UNSUPPORTED; a component whose 8 m^2 bytes exceed the device's free
+ * memory: MASHGPU_ERR_NOMEM before its matrix is allocated.  Synchronises the stream. */
+int mashgpu_dist_linkage_cut(mashgpu_dist_job *job, int method, double t, uint32_t *labels, uint32_t *id_lo, uint32_t *id_hi, double *height,
+                             uint32_t *size, uint64_t *n_clusters, uint64_t *n_components, uint64_t *largest_component);
+/* The largest component mashgpu_dist_linkage_cut links inside one CTA (0 = default, the most that fits its shared memory, 238;
+ * larger values are cut to it; 1 sends every component to the matrix tier).  The result does not depend on it. */
+int mashgpu_dist_set_linkage_cut_cta_max(mashgpu_dist_job *job, uint64_t members);
+/* Device time in ms of the last mashgpu_dist_linkage_cut's phases: components, grouping, CTA tier, matrix tier (4 entries). */
+int mashgpu_dist_linkage_cut_stats(mashgpu_dist_job *job, double *phase_ms);
 
 /* ---- Sharded dictionary build (multi-GPU all-vs-all; DESIGN.md 5).  With the reference axis sharded over G ranks the
  * dictionary of mashgpu_dist_open would be rebuilt in full on every rank.  These entry points split it by HASH RANGE

@@ -135,6 +135,9 @@ def load_library():
     L.mashgpu_dist_neighbor_joining.argtypes = [C.c_void_p, u32p, f64p]
     L.mashgpu_neighbor_joining_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, u32p, f64p, C.c_void_p]
     L.mashgpu_dist_linkage.argtypes = [C.c_void_p, C.c_int, u32p, u32p, f64p, u32p, u64p]
+    L.mashgpu_dist_linkage_cut.argtypes = [C.c_void_p, C.c_int, C.c_double, u32p, u32p, u32p, f64p, u32p, u64p, u64p, u64p]
+    L.mashgpu_dist_set_linkage_cut_cta_max.argtypes = [C.c_void_p, C.c_uint64]
+    L.mashgpu_dist_linkage_cut_stats.argtypes = [C.c_void_p, f64p]
     L.mashgpu_linkage_matrix.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int, u32p, u32p, f64p, u32p, u64p, C.c_void_p]
     L.mashgpu_dist.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.POINTER(DistParams), u32p, u32p, f64p, f64p, u8p]
     L.mashgpu_within_open.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.POINTER(SketchSet), C.c_double, C.POINTER(C.c_void_p)]
@@ -629,6 +632,34 @@ class DistJob:
         self.eng._check(self.eng.lib.mashgpu_dist_linkage(self.h, _linkage_method(method), *_linkage_pointers(out), C.byref(rows)))
         out["rows_rescanned"] = rows.value
         return out
+
+    def linkage_cut(self, method, t, merges=False):
+        """The flat clusters of linkage(method) cut at height t (DESIGN.md 3.13), linked per component of the pairs within about t, so
+        the n x n matrix is never built: {"labels": uint32[n_qry], the smallest index of each sketch's cluster, "n_clusters",
+        "n_components", "largest_component"}.  With merges=True also "merges", each component's own linkage in Z layout (leaves =
+        sketch indices), n_qry - n_components entries grouped by component; those at height <= t are linkage()'s.  Self jobs only."""
+        n = self.n_qry
+        labels = np.zeros(n, np.uint32)
+        out = _linkage_outputs(n) if merges else None
+        ptrs = _linkage_pointers(out) if merges else (None, None, None, None)
+        clusters, comps, largest = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_dist_linkage_cut(self.h, _linkage_method(method), float(t), _p(labels, u32p), *ptrs, C.byref(clusters),
+                                                              C.byref(comps), C.byref(largest)))
+        res = {"labels": labels, "n_clusters": clusters.value, "n_components": comps.value, "largest_component": largest.value}
+        if merges:
+            res["merges"] = {k: v[:max(n - comps.value, 0)] for k, v in out.items()}
+        return res
+
+    def set_linkage_cut_cta_max(self, members):
+        """The largest component linkage_cut() links inside one CTA (0 = default, the most that fits; 1 = every component through the
+        matrix tier); the result does not depend on it."""
+        self.eng._check(self.eng.lib.mashgpu_dist_set_linkage_cut_cta_max(self.h, int(members)))
+
+    def linkage_cut_stats(self):
+        """Device time in ms of the last linkage_cut()'s phases: components, grouping, cta, matrix."""
+        ms = np.zeros(4, np.float64)
+        self.eng._check(self.eng.lib.mashgpu_dist_linkage_cut_stats(self.h, _p(ms, f64p)))
+        return dict(zip(("components", "grouping", "cta", "matrix"), ms.tolist()))
 
     def set_prefilter(self, mode):
         """-1 = auto (default), 0 = merge every pair, 1 = always probe the reference tiles first."""

@@ -1,6 +1,7 @@
 // dense.cuh -- pieces shared by the passes over a dense float64 distance matrix in device memory: neighbor joining (nj.cu,
-// DESIGN.md 3.10) and average / complete linkage (linkage.cu, DESIGN.md 3.11).  A strict total order on (value, key) with its
-// block minimum, the mirror of the lower triangle with its finiteness test, and what every pass does before its first step.
+// DESIGN.md 3.10) and average / complete linkage (linkage.cu, DESIGN.md 3.11, and its CTA tier linkage_cta.cuh, 3.13).  A strict
+// total order on (value, key) with its block minimum, the linkage update, the mirror of the lower triangle with its finiteness
+// test, and what every pass does before its first step.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -52,6 +53,27 @@ __device__ DenseMin dense_block_min(double q, unsigned long long k)
     }
     __syncthreads();
     return DenseMin{sq[0], sk[0]};
+}
+
+// Average / complete linkage (linkage.cu, and the CTA tier of the linkage cut, linkage_cta.cuh): merge s in scipy's Z layout, and the
+// two steps of a merge of (a, b) that every slot k does for itself.
+struct LkMerge { double height; uint32_t lo, hi, size; };   // node ids (smaller first), height, leaves
+
+// D(u, k) from D(a, k) and D(b, k): one IEEE double operation at a time, never fused
+template <bool AVERAGE>
+__device__ __forceinline__ double lk_value(uint32_t na, uint32_t nb, double dak, double dbk)
+{
+    if (AVERAGE) return __ddiv_rn(__dadd_rn(__dmul_rn((double)na, dak), __dmul_rn((double)nb, dbk)), (double)(na + nb));
+    return dbk > dak ? dbk : dak;
+}
+
+// What a merge of (a, b) does to the cache (c, j) of a row k > a, given v = D(u, k): a neighbour a or b becomes (v, a) when v <= c,
+// else the row is rescanned; any other neighbour is lowered to (v, a) when that is before it, else kept.
+enum { LK_KEEP, LK_TAKE, LK_RESCAN };
+__device__ __forceinline__ int lk_offer(double v, uint32_t a, uint32_t b, double c, uint32_t j)
+{
+    if (j == a || j == b) return v <= c ? LK_TAKE : LK_RESCAN;
+    return dense_before(v, a, c, j) ? LK_TAKE : LK_KEEP;
 }
 
 // the minimum of an argmin's n_partial per-CTA partials, reduced by a block of DENSE_THREADS threads and returned to every thread

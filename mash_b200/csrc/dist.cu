@@ -46,6 +46,7 @@
 #include "dist_cc.cuh"
 #include "dist_msf.cuh"
 #include "dist_greedy.cuh"
+#include "linkage_cta.cuh"
 
 namespace mashgpu {
 
@@ -677,6 +678,12 @@ __global__ void __launch_bounds__(256) dist_kernel_general(const DistArgs a)
     dist_emit(a, q, r, cd.x, cd.y, a.ref_len[r]);
 }
 
+// dist_emit's distance of a pair from its merge result
+__device__ __forceinline__ double dist_value(const DistArgs &a, uint32_t common, uint32_t denom)
+{
+    return (denom == a.S) ? a.dist_lut[common] : mash_distance(common, denom, a.kmer_size);
+}
+
 // The values of a graph edge (q, r) recomputed on its own: the sequential merge of dist_kernel_general and the arithmetic of dist_emit /
 // dist_fix_kernel, so every value is the one a dense run returns for (q, r).  Every edge shares a hash, so its p-value is the binomial
 // tail.
@@ -685,7 +692,7 @@ __device__ __forceinline__ void dist_edge_values(const DistArgs &a, uint32_t q, 
 {
     const uint2 cd = dist_merge_pair(a, q, r);
     *numer = cd.x; *denom = cd.y;
-    *distance = (cd.y == a.S) ? a.dist_lut[cd.x] : mash_distance(cd.x, cd.y, a.kmer_size);
+    *distance = dist_value(a, cd.x, cd.y);
     *pvalue = mash_pvalue(cd.x, a.ref_len[r], a.qry_len[q], a.kmer_space, cd.y, &a.binom);
 }
 
@@ -805,6 +812,74 @@ __global__ void iota_kernel(uint32_t *v, uint64_t n)
     if (t < n) v[t] = (uint32_t)t;
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Linkage cut (mashgpu_dist_linkage_cut, DESIGN.md 3.13): the CTA tier and the large tier's row gather
+// ---------------------------------------------------------------------------------------------------------
+struct CutComp { uint32_t first, m, merge0; };      // a component: members[first .. first + m), merges rec[merge0 .. merge0 + m - 2]
+
+// One CTA per component of a size class (m <= the class's bound, THREADS for it): the component's lower triangle of run()'s
+// distances into shared memory -- D(i, j), j < i, of the pair (q = members[i], r = members[j]) by the sequential merge and
+// dist_emit's arithmetic, as dist_edge_values computes it -- then its whole linkage there (linkage_cta.cuh).
+template <unsigned THREADS, bool AVERAGE>
+__global__ void __launch_bounds__(THREADS) cut_cta_kernel(const DistArgs a, const uint32_t *__restrict__ members, const CutComp *__restrict__ comps,
+                                                          LkMerge *rec, int *no_pair)
+{
+    extern __shared__ __align__(16) double cut_smem[];
+    const CutComp c = comps[blockIdx.x];
+    const uint32_t *mem = members + c.first;
+    const CtaLinkage L = cta_layout(cut_smem, c.m);
+    const uint32_t pairs = cta_tri(c.m);
+    for (uint32_t p = threadIdx.x; p < pairs; p += THREADS) {
+        uint32_t i = (uint32_t)((1.0f + sqrtf(1.0f + 8.0f * (float)p)) * 0.5f);     // the row: cta_tri(i) <= p < cta_tri(i + 1)
+        while (i > 1 && cta_tri(i) > p) i--;
+        while (cta_tri(i + 1) <= p) i++;
+        const uint2 cd = dist_merge_pair(a, mem[i], mem[p - cta_tri(i)]);
+        L.tri[p] = dist_value(a, cd.x, cd.y);
+    }
+    __syncthreads();
+    cta_linkage<THREADS, AVERAGE>(L, c.m, rec + c.merge0, no_pair);
+}
+
+// Empty sketches share no hash, yet are at distance 0 from one another (common = denom = 0): at any T they are one component, whose
+// label is the first of them.  (Every other pair without a shared hash is at distance 1.)
+__global__ void cut_empty_first_kernel(const uint32_t *n_eff, uint64_t n, uint32_t *first)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t < n && n_eff[t] == 0) atomicMin(first, (uint32_t)t);
+}
+
+__global__ void cut_empty_join_kernel(const uint32_t *n_eff, uint64_t n, const uint32_t *first, uint32_t *label)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t < n && n_eff[t] == 0) label[t] = *first;
+}
+
+// The components' first positions in the sorted keys: flag[t] = 1 where a run of equal keys starts, then (with scan = the inclusive sum of
+// the flags) first[scan[t] - 1] = t there
+__global__ void cut_start_kernel(const uint32_t *key, uint64_t n, uint32_t *flag)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t < n) flag[t] = (t == 0 || key[t] != key[t - 1]) ? 1u : 0u;
+}
+
+__global__ void cut_first_kernel(const uint32_t *key, const uint32_t *scan, uint64_t n, uint32_t *first)
+{
+    const uint64_t t = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (t < n && (t == 0 || key[t] != key[t - 1])) first[scan[t] - 1] = (uint32_t)t;
+}
+
+// The large tier's rows: row t := the self job's row members[t], with its hash count and length
+__global__ void cut_gather_kernel(const uint32_t *ranks, uint32_t P, const uint32_t *n_eff, const uint64_t *len, const uint32_t *members, uint64_t m,
+                                  uint32_t *o_ranks, uint32_t *o_n_eff, uint64_t *o_len)
+{
+    for (uint64_t x = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; x < m * P; x += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t t = x / P;
+        const uint32_t i = (uint32_t)(x % P), src = members[t];
+        o_ranks[x] = ranks[(uint64_t)src * P + i];
+        if (i == 0) { o_n_eff[t] = n_eff[src]; o_len[t] = len[src]; }
+    }
+}
+
 }  // namespace mashgpu
 
 using namespace mashgpu;
@@ -839,6 +914,8 @@ struct mashgpu_dist_job {
     std::vector<EventPair> best_events;
     DevBuf<unsigned long long> cc_edges;        // edge counter of mashgpu_dist_components_dev
     uint64_t greedy_block = 0;          // mashgpu_dist_set_representative_block; 0 = default
+    uint64_t cut_cta_max = 0;           // mashgpu_dist_set_linkage_cut_cta_max; 0 = default
+    double cut_ms[4] = {0, 0, 0, 0};    // device time of the last linkage cut's phases: components, grouping, CTA tier, large tier
     // prefilter (dist_probe_kernel): -1 = auto (on; switched off when most combinations turn out to share hashes), 0 = off, 1 = on
     int prefilter_mode = -1;
     bool triangle = false;
@@ -1946,6 +2023,294 @@ extern "C" int mashgpu_dist_linkage(mashgpu_dist_job *job, int method, uint32_t 
     MG_TRY(fill_distance_matrix(job, "linkage", 2, id_lo && id_hi && height && size, matrix));
     const uint64_t n = job->n_qry;
     return mashgpu_linkage_matrix(job->ctx, matrix.p, n, n, method, id_lo, id_hi, height, size, rows_rescanned, job->ctx->stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Flat clusters of average / complete linkage at a height, linked per component (DESIGN.md 3.13)
+// ---------------------------------------------------------------------------------------------------------
+// Upper member counts of the CTA tier's size classes below its largest one: a small component is not charged the shared memory of
+// the largest, so many of them are resident per SM.
+static const uint32_t CUT_CLASSES[] = {2, 4, 8, 16, 32, 64, 96, 128, 160};
+
+// The largest component whose triangle and linkage state fit one CTA's shared memory next to the static block minimum (238)
+static uint32_t cut_cta_limit()
+{
+    const size_t avail = 227 * 1024 - 256;
+    uint32_t m = 2;
+    while (cta_linkage_smem(m + 1) <= avail) m++;
+    return m;
+}
+
+// T = t (1 + 8 n 2^-53), rounded up.  A merge at a height <= t never joins two components of the graph whose edges are the pairs within
+// T that share a hash: between components every leaf pair is above T, and n nested averages lose less than a factor 1 - 3 n 2^-53.
+static double cut_threshold(double t, uint64_t n)
+{
+    return std::nextafter(t * (1.0 + 8.0 * (double)n * 0x1p-53), INFINITY);
+}
+
+template <unsigned THREADS>
+static cudaError_t cut_cta_launch(bool average, uint32_t n_comps, size_t smem, cudaStream_t st, const DistArgs &a, const uint32_t *members,
+                                  const CutComp *comps, LkMerge *rec, int *no_pair)
+{
+    void (*k)(const DistArgs, const uint32_t *, const CutComp *, LkMerge *, int *) =
+        average ? cut_cta_kernel<THREADS, true> : cut_cta_kernel<THREADS, false>;
+    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    k<<<n_comps, THREADS, smem, st>>>(a, members, comps, rec, no_pair);
+    return cudaGetLastError();
+}
+
+// The m x m matrix of the lower triangle of run()'s distances among `members` (device, ascending) of a self job, through the tiled merge
+// kernels: the job itself when the component is the whole set, else an encoded job over a gathered copy of the members' rows.
+static int cut_fill_matrix(mashgpu_dist_job *job, const uint32_t *d_members, uint64_t m, double *matrix, cudaStream_t st)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    auto target = [&](DistArgs &a) { a.distance = matrix + (uint64_t)a.q_begin * m; };
+    if (m == job->n_qry) return enqueue_lower_triangle(job, st, target);
+    DevBuf<uint32_t> rows, n_eff; DevBuf<uint64_t> len;
+    if (rows.alloc(m * job->P) != cudaSuccess || n_eff.alloc(m) != cudaSuccess || len.alloc(m) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (rows of a %llu-sketch component)", (unsigned long long)m);
+    cut_gather_kernel<<<ctx->sm_count * 8, 256, 0, st>>>(job->d_ranks, job->P, job->d_n_eff, job->d_lens, d_members, m, rows.p, n_eff.p, len.p);
+    MG_CUDA(ctx, cudaGetLastError());
+    ctx->kernel_launches++;
+    mashgpu_dist_job *sub = nullptr;
+    MG_TRY(mashgpu_dist_open_encoded(ctx, rows.p, n_eff.p, len.p, m, 0, m, &job->params, &sub));
+    const int rc = enqueue_lower_triangle(sub, st, target);
+    mashgpu_dist_close(sub);            // synchronises the stream before the rows are freed
+    return rc;
+}
+
+extern "C" int mashgpu_dist_set_linkage_cut_cta_max(mashgpu_dist_job *job, uint64_t members)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    job->cut_cta_max = members;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_linkage_cut_stats(mashgpu_dist_job *job, double *phase_ms)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    if (!phase_ms) return fail(job->ctx, MASHGPU_ERR_INVALID, "NULL output");
+    for (int i = 0; i < 4; i++) phase_ms[i] = job->cut_ms[i];
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_dist_linkage_cut(mashgpu_dist_job *job, int method, double t, uint32_t *labels, uint32_t *id_lo, uint32_t *id_hi,
+                                        double *height, uint32_t *size, uint64_t *n_clusters, uint64_t *n_components, uint64_t *largest_component)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (job->encoded) return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "linkage cut of an encoded (sharded) job");
+    if (!job->self) return fail(ctx, MASHGPU_ERR_INVALID, "linkage cut needs a self comparison (qry == NULL)");
+    if (method != MASHGPU_LINKAGE_AVERAGE && method != MASHGPU_LINKAGE_COMPLETE)
+        return fail(ctx, MASHGPU_ERR_INVALID, "unknown linkage method %d", method);
+    if (!(t >= 0)) return fail(ctx, MASHGPU_ERR_INVALID, "cut height %g is NaN or negative", t);
+    if (!labels || !n_clusters || !n_components || !largest_component) return fail(ctx, MASHGPU_ERR_INVALID, "NULL output");
+    const int forest = (id_lo != nullptr) + (id_hi != nullptr) + (height != nullptr) + (size != nullptr);
+    if (forest != 0 && forest != 4) return fail(ctx, MASHGPU_ERR_INVALID, "the merge forest needs all four outputs or none");
+    const uint64_t n = job->n_qry;
+    *n_clusters = *n_components = *largest_component = n;        // 0 or 1 sketch: the identity
+    for (double &ms : job->cut_ms) ms = 0;
+    if (n == 1) labels[0] = 0;
+    if (n < 2) return MASHGPU_OK;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    struct Events {
+        EventPair e[4] = {};
+        ~Events() { for (EventPair &p : e) { if (p.a) cudaEventDestroy(p.a); if (p.b) cudaEventDestroy(p.b); } }
+    } events;
+    EventPair *ev = events.e;
+    for (int i = 0; i < 4; i++) {
+        MG_CUDA(ctx, cudaEventCreate(&ev[i].a));
+        MG_CUDA(ctx, cudaEventCreate(&ev[i].b));
+    }
+
+    // 1. components of the pairs within T: those that share a hash (no p-value test: every p-value is <= 1), and the empty sketches
+    // joined; one component when T >= 1
+    const double T = cut_threshold(t, n);
+    DevBuf<uint32_t> d_label, d_key, d_idx, d_member, d_first;
+    if (d_label.alloc(n) != cudaSuccess || d_key.alloc(n) != cudaSuccess || d_idx.alloc(n) != cudaSuccess || d_member.alloc(n) != cudaSuccess ||
+        d_first.alloc(n) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (components of %llu sketches)", (unsigned long long)n);
+    MG_CUDA(ctx, cudaEventRecord(ev[0].a, st));
+    if (T < 1) {
+        const double md = job->params.max_distance, mp = job->params.max_pvalue;
+        job->params.max_distance = T;
+        job->params.max_pvalue = -1;
+        uint64_t edges = 0;
+        const int rc = mashgpu_dist_components_dev(job, d_label.p, &edges, st);
+        job->params.max_distance = md;
+        job->params.max_pvalue = mp;
+        MG_TRY(rc);
+        uint32_t *first_empty = d_key.p;                    // scratch until the sort
+        MG_CUDA(ctx, cudaMemsetAsync(first_empty, 0xFF, 4, st));
+        cut_empty_first_kernel<<<blocks_for(n), 256, 0, st>>>(job->d_n_eff, n, first_empty);
+        cut_empty_join_kernel<<<blocks_for(n), 256, 0, st>>>(job->d_n_eff, n, first_empty, d_label.p);
+        MG_CUDA(ctx, cudaGetLastError());
+        ctx->kernel_launches += 2;
+    } else {
+        MG_CUDA(ctx, cudaMemsetAsync(d_label.p, 0, n * 4, st));
+    }
+    MG_CUDA(ctx, cudaEventRecord(ev[0].b, st));
+
+    // 2. grouping: (label, index) sorted by label -- stable, so each component's members are ascending and the components come in the
+    // order of their smallest member, the label -- and where each component starts
+    MG_CUDA(ctx, cudaEventRecord(ev[1].a, st));
+    iota_kernel<<<blocks_for(n), 256, 0, st>>>(d_idx.p, n);
+    MG_CUDA(ctx, cudaGetLastError());
+    int bits = 1;
+    while (bits < 32 && (1ull << bits) < n) bits++;
+    size_t tb_sort = 0, tb_scan = 0;
+    DevBuf<uint8_t> tmp;
+    uint32_t *flag = d_idx.p, *scan = d_label.p;            // the sort's inputs are dead after it
+    MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, d_label.p, d_key.p, d_idx.p, d_member.p, (int)n, 0, bits, st));
+    MG_CUDA(ctx, cub::DeviceScan::InclusiveSum(nullptr, tb_scan, flag, scan, (int)n, st));
+    if (tmp.alloc(std::max(tb_sort, tb_scan)) != cudaSuccess) return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (sort scratch)");
+    MG_CUDA(ctx, cub::DeviceRadixSort::SortPairs(tmp.p, tb_sort, d_label.p, d_key.p, d_idx.p, d_member.p, (int)n, 0, bits, st));
+    cut_start_kernel<<<blocks_for(n), 256, 0, st>>>(d_key.p, n, flag);
+    MG_CUDA(ctx, cub::DeviceScan::InclusiveSum(tmp.p, tb_scan, flag, scan, (int)n, st));
+    cut_first_kernel<<<blocks_for(n), 256, 0, st>>>(d_key.p, scan, n, d_first.p);
+    MG_CUDA(ctx, cudaGetLastError());
+    uint32_t runs = 0;
+    std::vector<uint32_t> first, member(n);
+    MG_CUDA(ctx, cudaMemcpyAsync(&runs, scan + (n - 1), 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(member.data(), d_member.p, n * 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    ctx->kernel_launches += 8;
+    first.resize(runs + 1);
+    MG_CUDA(ctx, cudaMemcpy(first.data(), d_first.p, (size_t)runs * 4, cudaMemcpyDeviceToHost));
+    first[runs] = (uint32_t)n;
+    MG_CUDA(ctx, cudaEventRecord(ev[1].b, st));
+    // the components in order, each with its members' offset and its merges' offset; the CTA tier's components by size class, the
+    // large tier's in a list
+    const uint32_t limit = cut_cta_limit();
+    const uint32_t M = job->cut_cta_max ? (uint32_t)std::min<uint64_t>(job->cut_cta_max, limit) : limit;
+    std::vector<uint32_t> bound;
+    for (uint32_t b : CUT_CLASSES) if (b < M) bound.push_back(b);
+    if (M >= 2) bound.push_back(M);
+    std::vector<CutComp> comp(runs);
+    std::vector<std::vector<CutComp>> cls(bound.size());
+    std::vector<CutComp> large;
+    uint64_t merges = 0, largest = 0, largest_large = 0;
+    for (uint32_t c = 0; c < runs; c++) {
+        const uint32_t m = first[c + 1] - first[c];
+        comp[c] = CutComp{first[c], m, (uint32_t)merges};
+        merges += m - 1;
+        largest = std::max<uint64_t>(largest, m);
+        if (m < 2) continue;
+        if (m > M) { large.push_back(comp[c]); largest_large = std::max<uint64_t>(largest_large, m); continue; }
+        size_t k = 0;
+        while (bound[k] < m) k++;
+        cls[k].push_back(comp[c]);
+    }
+    size_t free_b = 0, total_b = 0;
+    MG_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+    if ((double)largest_large * (double)largest_large * 8.0 > (double)free_b)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "at t = %g the largest component has %llu sketches: its %llu x %llu distance matrix needs %.3g GB, the device has %.3g GB free",
+                    t, (unsigned long long)largest_large, (unsigned long long)largest_large, (unsigned long long)largest_large,
+                    (double)largest_large * (double)largest_large * 8e-9, (double)free_b * 1e-9);
+
+    // 3. the CTA tier: one launch per size class
+    std::vector<LkMerge> rec(merges);
+    DevBuf<LkMerge> d_rec; DevBuf<CutComp> d_comp; DevBuf<int> d_no_pair;
+    uint64_t in_cta = 0;
+    for (auto &v : cls) in_cta += v.size();
+    MG_CUDA(ctx, cudaEventRecord(ev[2].a, st));
+    if (in_cta) {
+        if (d_rec.alloc(merges) != cudaSuccess || d_comp.alloc(in_cta) != cudaSuccess || d_no_pair.alloc(1) != cudaSuccess)
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (merges of %llu components)", (unsigned long long)in_cta);
+        std::vector<CutComp> flat;
+        flat.reserve(in_cta);
+        for (auto &v : cls) flat.insert(flat.end(), v.begin(), v.end());
+        MG_CUDA(ctx, cudaMemcpyAsync(d_comp.p, flat.data(), in_cta * sizeof(CutComp), cudaMemcpyHostToDevice, st));
+        MG_CUDA(ctx, cudaMemsetAsync(d_no_pair.p, 0, sizeof(int), st));
+        const DistArgs a = dist_args(job, 0, n);
+        const bool average = method == MASHGPU_LINKAGE_AVERAGE;
+        uint64_t off = 0;
+        for (size_t k = 0; k < cls.size(); k++) {
+            const uint32_t nc = (uint32_t)cls[k].size();
+            if (!nc) continue;
+            const size_t smem = cta_linkage_smem(bound[k]);
+            const CutComp *dc = d_comp.p + off;
+            cudaError_t e;
+            if (bound[k] <= 32) e = cut_cta_launch<32>(average, nc, smem, st, a, d_member.p, dc, d_rec.p, d_no_pair.p);
+            else if (bound[k] <= 64) e = cut_cta_launch<64>(average, nc, smem, st, a, d_member.p, dc, d_rec.p, d_no_pair.p);
+            else if (bound[k] <= 128) e = cut_cta_launch<128>(average, nc, smem, st, a, d_member.p, dc, d_rec.p, d_no_pair.p);
+            else e = cut_cta_launch<256>(average, nc, smem, st, a, d_member.p, dc, d_rec.p, d_no_pair.p);
+            MG_CUDA(ctx, e);
+            ctx->kernel_launches++;
+            off += nc;
+        }
+        int no_pair = 0;
+        MG_CUDA(ctx, cudaMemcpyAsync(rec.data(), d_rec.p, merges * sizeof(LkMerge), cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaMemcpyAsync(&no_pair, d_no_pair.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        MG_CUDA(ctx, cudaStreamSynchronize(st));
+        if (no_pair) return fail(ctx, MASHGPU_ERR_INVALID, "linkage found no pair with a comparable distance (an update overflowed)");
+    }
+    MG_CUDA(ctx, cudaEventRecord(ev[2].b, st));
+
+    // 4. the large tier: per component an m x m matrix through the tiled merge kernels, then mashgpu_linkage_matrix
+    MG_CUDA(ctx, cudaEventRecord(ev[3].a, st));
+    for (const CutComp &c : large) {
+        const uint64_t m = c.m;
+        DevBuf<double> matrix;
+        if (matrix.alloc(m * m) != cudaSuccess)
+            return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (%llu x %llu distance matrix of a component at t = %g)", (unsigned long long)m,
+                        (unsigned long long)m, t);
+        MG_TRY(cut_fill_matrix(job, d_member.p + c.first, m, matrix.p, st));
+        std::vector<uint32_t> lo(m - 1), hi(m - 1), sz(m - 1);
+        std::vector<double> h(m - 1);
+        MG_TRY(mashgpu_linkage_matrix(ctx, matrix.p, m, m, method, lo.data(), hi.data(), h.data(), sz.data(), nullptr, st));
+        for (uint64_t s = 0; s + 1 < m; s++) rec[c.merge0 + s] = LkMerge{h[s], lo[s], hi[s], sz[s]};
+    }
+    MG_CUDA(ctx, cudaEventRecord(ev[3].b, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    for (int i = 0; i < 4; i++) {
+        float ms = 0;
+        MG_CUDA(ctx, cudaEventElapsedTime(&ms, ev[i].a, ev[i].b));
+        job->cut_ms[i] = ms;
+    }
+
+    // 5. per component the cut (writeLinkage's: a maximal subtree whose largest merge height is <= t), labelled by its smallest member,
+    // and the merges with the set's ids: leaf j -> members[first + j], node m + s -> n + merge0 + s
+    std::vector<double> worst;
+    std::vector<uint32_t> top, low;
+    for (const CutComp &c : comp) {
+        const uint32_t m = c.m, *mem = member.data() + c.first;
+        if (m == 1) { labels[mem[0]] = mem[0]; continue; }
+        const LkMerge *r = rec.data() + c.merge0;
+        const uint32_t nodes = 2 * m - 1;
+        worst.assign(nodes, 0.0);
+        low.resize(nodes);
+        top.resize(nodes);
+        for (uint32_t j = 0; j < m; j++) low[j] = j;
+        for (uint32_t s = 0; s + 1 < m; s++) {
+            worst[m + s] = std::max(r[s].height, std::max(worst[r[s].lo], worst[r[s].hi]));
+            low[m + s] = std::min(low[r[s].lo], low[r[s].hi]);
+        }
+        top[nodes - 1] = nodes - 1;
+        for (uint32_t s = m - 1; s-- > 0;) {
+            const uint32_t u = m + s;
+            top[r[s].lo] = worst[u] <= t ? top[u] : r[s].lo;
+            top[r[s].hi] = worst[u] <= t ? top[u] : r[s].hi;
+        }
+        for (uint32_t j = 0; j < m; j++) labels[mem[j]] = mem[low[top[j]]];
+        if (forest) {
+            auto global = [&](uint32_t x) { return x < m ? mem[x] : (uint32_t)(n + c.merge0 + (x - m)); };
+            for (uint32_t s = 0; s + 1 < m; s++) {
+                id_lo[c.merge0 + s] = global(r[s].lo);
+                id_hi[c.merge0 + s] = global(r[s].hi);
+                height[c.merge0 + s] = r[s].height;
+                size[c.merge0 + s] = r[s].size;
+            }
+        }
+    }
+    uint64_t clusters = 0;
+    for (uint64_t i = 0; i < n; i++) clusters += labels[i] == i;
+    *n_clusters = clusters;
+    *n_components = runs;
+    *largest_component = largest;
+    return MASHGPU_OK;
 }
 
 extern "C" int mashgpu_dist_close(mashgpu_dist_job *job)

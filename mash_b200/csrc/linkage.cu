@@ -23,7 +23,6 @@ namespace {
 
 constexpr unsigned LK_RESCAN_THREADS = 1024;    // one CTA per rescanned row: a row of n doubles in a few round trips
 
-struct LkMerge { double height; uint32_t lo, hi, size; };   // merge s, Z layout: node ids (smaller first), height, leaves
 struct LkStep { uint32_t a, b; };                           // the slots of the merge in flight
 
 // slot i: a leaf of size 1, no cached neighbour, and on the rescan list (which therefore holds every row)
@@ -98,20 +97,13 @@ __global__ void __launch_bounds__(DENSE_THREADS) lk_update_kernel(double *D, uin
     }
     double *row_a = D + (uint64_t)a * ld;
     const double dak = row_a[k], dbk = D[(uint64_t)b * ld + k];
-    double v;
-    if (AVERAGE) v = __ddiv_rn(__dadd_rn(__dmul_rn((double)na, dak), __dmul_rn((double)nb, dbk)), (double)(na + nb));
-    else v = dbk > dak ? dbk : dak;
+    const double v = lk_value<AVERAGE>(na, nb, dak, dbk);
     row_a[k] = v;
     D[(uint64_t)k * ld + a] = v;
     if (k < a) return;
-    const double c = cv[k];
-    const uint32_t j = cj[k];
-    if (j == a || j == b) {
-        if (v <= c) { cv[k] = v; cj[k] = a; }
-        else list[atomicAdd(count, 1u)] = k;
-    } else if (dense_before(v, a, c, j)) {
-        cv[k] = v; cj[k] = a;
-    }
+    const int o = lk_offer(v, a, b, cv[k], cj[k]);
+    if (o == LK_TAKE) { cv[k] = v; cj[k] = a; }
+    else if (o == LK_RESCAN) list[atomicAdd(count, 1u)] = k;
 }
 
 // Grid-stride CTAs over the rescan list (its length read here): row i's cache := the least (D(i, j), j) over j < i, NaN (dead)

@@ -615,28 +615,24 @@ static void writeNeighborJoining(mashgpu_dist_job *job, const Sketch &sketch, bo
 // device.  Without -d, the rooted tree as one Newick line: a merge's node sits at half its height, leaves at 0, and a branch is the
 // parent's height minus the child's.  With -d t, per sketch its flat cluster at t in -G's format: scipy's fcluster(Z, t, "distance"),
 // a maximal subtree whose every merge has height <= t (the largest height in it, since rounding in the average can make a later
-// merge lower by an ulp).  One sketch has no merge: its name, or cluster 0.
+// merge lower by an ulp).  The cut is linked per component of the pairs within about t (DESIGN.md 3.13), so it needs memory for the
+// largest component's matrix, not for all n sketches.  One sketch has no merge: its name, or cluster 0.
 static void writeLinkage(mashgpu_dist_job *job, const Sketch &sketch, bool comment, int method, bool cutting, double t, int threads)
 {
     const uint64_t n = sketch.getReferenceCount(), m = n ? n - 1 : 0, nodes = n + m;
+    if (cutting) {
+        vector<uint32_t> label(n);
+        uint64_t flat = 0, components = 0, largest = 0;
+        if (n && mashgpu_dist_linkage_cut(job, method, t, label.data(), 0, 0, 0, 0, &flat, &components, &largest) != MASHGPU_OK) gpuFail();
+        const uint32_t clusters = writeClusterLines(sketch, comment, threads, label, n);
+        cerr << "Clusters: " << clusters << " at height <= " << t << endl;
+        cerr << "Components: " << components << " linked, the largest of " << largest << " sketches" << endl;
+        return;
+    }
     vector<uint32_t> lo(m), hi(m), size(m);
     vector<double> height(m);
     uint64_t rows = 0;
     if (n > 1 && mashgpu_dist_linkage(job, method, lo.data(), hi.data(), height.data(), size.data(), &rows) != MASHGPU_OK) gpuFail();
-    if (cutting) {
-        vector<double> worst(nodes, 0.0);                  // the largest merge height in each node's subtree
-        for (uint64_t s = 0; s < m; s++) worst[n + s] = std::max(height[s], std::max(worst[lo[s]], worst[hi[s]]));
-        vector<uint32_t> top(nodes);                       // the root of each node's flat cluster, assigned from the root down
-        if (nodes) top[nodes - 1] = (uint32_t)(nodes - 1);
-        for (uint64_t s = m; s-- > 0;) {
-            const uint32_t u = (uint32_t)(n + s);
-            top[lo[s]] = worst[u] <= t ? top[u] : lo[s];
-            top[hi[s]] = worst[u] <= t ? top[u] : hi[s];
-        }
-        const uint32_t clusters = writeClusterLines(sketch, comment, threads, top, nodes);
-        cerr << "Clusters: " << clusters << " at height <= " << t << endl;
-        return;
-    }
     vector<uint32_t> parent(nodes, UINT32_MAX);
     vector<double> length(nodes, 0.0);
     auto nodeHeight = [&](uint64_t v) { return v < n ? 0.0 : height[v - n] * 0.5; };
@@ -696,6 +692,7 @@ int runTriangle(int argc, const char **argv)
              << "            -E or -G).  The lines up to distance t are the -G clusters at -d t." << endl
              << "  -N        Neighbor-joining tree of every pair's distance, as one Newick line (not with -E, -G, -T, -d or -v)." << endl
              << "  -L <m>    Average or complete linkage (m = average or complete) of every pair's distance as one Newick line; with -d t, per sketch its cluster at height <= t (not with -E, -G, -T, -N or -v)." << endl
+             << "            The tree needs an n x n matrix on the device; with -d the limit is the largest component of the pairs within t, not n." << endl
              << "  -R <o>    Greedy representatives in order o (length: longest first, input: input order): a sketch is one unless an earlier one is within -d / -v; per sketch its representative, the nearest, and the distance (not with -E, -G, -T, -N or -L)." << endl;
         return 0;
     }
