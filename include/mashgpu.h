@@ -549,6 +549,29 @@ int mashgpu_screen_finish(mashgpu_screen_job *job, uint64_t *shared, uint64_t *m
  * (ties: the longer genome, refs->length at mashgpu_screen_open; a tie in both goes to the lowest index -- the reference
  * leaves it to the iteration order of a hash set) before shared / median / identity / p-value are computed. */
 int mashgpu_screen_set_winner(mashgpu_screen_job *job, int on);
+/* Screening samples one after another against one resident table (`mash screen -I`).  After mashgpu_screen_reset, every
+ * finish of the job returns, bit for bit, what a fresh job over the same sketches fed only the chunks fed since would return.
+ *
+ * mashgpu_screen_finish_hits: the values of mashgpu_screen_finish at exactly the sketches with shared >= 1 (under -w: after
+ * the reallocation), in ascending sketch index: ref[i], shared[i], median[i], identity[i], pvalue[i] for i < *n_rows.  Every
+ * other sketch has shared 0, median 0, p-value 1.0 and identity 0 (1.0 for a sketch of 0 hashes).  Host buffers of n_ref
+ * entries each (any of ref .. pvalue and set_size may be NULL); honours mashgpu_screen_set_winner; leaves the job unchanged,
+ * like mashgpu_screen_finish.  The work follows the sample's hits through an inverted index (distinct hash -> sketches)
+ * built at the first call and kept until close: 4 B per (sketch, hash) pair plus 4 B per distinct hash, with scratch of
+ * another 4 B per pair so that no later call allocates.  MASHGPU_ERR_UNSUPPORTED for 2^32 or more pairs (32-bit segment
+ * offsets), MASHGPU_ERR_NOMEM when the index does not fit on the device.
+ *
+ * mashgpu_screen_reset: starts a new sample and keeps the table, the bitmap and the -w setting.  Feeds the small chunks still
+ * joined in the library and collects the chunk in flight (their counts are then dropped), zeroes the hit counters (only those
+ * hit, when no chunk was fed since a mashgpu_screen_finish_hits) and empties the mixture's bottom-s list.  Allocates nothing.
+ *
+ * mashgpu_screen_hits_stats: for the last mashgpu_screen_finish_hits, the distinct reference hashes the sample hit, the
+ * (hash, sketch) pairs expanded from them, the device time of the one-off index build and of the call's own device work
+ * (CUDA events, ms).  Any pointer may be NULL. */
+int mashgpu_screen_finish_hits(mashgpu_screen_job *job, uint32_t *ref, uint64_t *shared, uint64_t *median, double *identity,
+                               double *pvalue, uint64_t *n_rows, uint64_t *set_size);
+int mashgpu_screen_reset(mashgpu_screen_job *job);
+int mashgpu_screen_hits_stats(mashgpu_screen_job *job, uint64_t *hit_hashes, uint64_t *hit_pairs, double *index_ms, double *finish_ms);
 /* Multi-GPU screening (reads sharded over ranks, table replicated): the hit counters live in device memory as one
  * uint32 per distinct reference hash, in ascending hash order, so counter i means the same hash on every rank that
  * opened the job with the same sketches.  *d_counters / *n_counters expose that array for an all-reduce(sum) (NCCL via torch.distributed); the

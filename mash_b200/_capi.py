@@ -154,6 +154,9 @@ def load_library():
     L.mashgpu_screen_close.argtypes = [C.c_void_p]
     L.mashgpu_screen_mixture_dev.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
     L.mashgpu_screen_merge_mixtures_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64]
+    L.mashgpu_screen_finish_hits.argtypes = [C.c_void_p, u32p, u64p, u64p, f64p, f64p, u64p, u64p]
+    L.mashgpu_screen_reset.argtypes = [C.c_void_p]
+    L.mashgpu_screen_hits_stats.argtypes = [C.c_void_p, u64p, u64p, f64p, f64p]
     L.mashgpu_dict_local_sort.argtypes = [C.c_void_p, C.POINTER(SketchSet), C.c_uint64, C.c_void_p, C.c_void_p, u64p, C.c_void_p]
     L.mashgpu_dict_split.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, u64p, C.c_uint32, u64p, C.c_void_p]
     L.mashgpu_dict_rank.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, u64p, C.c_void_p]
@@ -828,6 +831,30 @@ class ScreenJob:
         self.eng._check(self.eng.lib.mashgpu_screen_finish(self.h, _p(shared, u64p), _p(median, u64p), _p(ident, f64p), _p(pv, f64p),
                                                            C.byref(set_size), _p(mix, u64p), C.byref(mix_n)))
         return dict(shared=shared, median=median, identity=ident, pvalue=pv, set_size=set_size.value, mixture=mix[:mix_n.value].copy())
+
+    def finish_hits(self):
+        """The sparse finish: finish()'s values at the references with shared >= 1 only, in ascending reference index.
+        Returns dict(ref, shared, median, identity, pvalue (arrays of the rows), set_size)."""
+        n = self.n_ref
+        ref = np.zeros(max(1, n), np.uint32)
+        shared = np.zeros(max(1, n), np.uint64); median = np.zeros(max(1, n), np.uint64)
+        ident = np.zeros(max(1, n), np.float64); pv = np.zeros(max(1, n), np.float64)
+        n_rows = C.c_uint64(0); set_size = C.c_uint64(0)
+        self.eng._check(self.eng.lib.mashgpu_screen_finish_hits(self.h, _p(ref, u32p), _p(shared, u64p), _p(median, u64p), _p(ident, f64p),
+                                                                _p(pv, f64p), C.byref(n_rows), C.byref(set_size)))
+        m = n_rows.value
+        return dict(ref=ref[:m].copy(), shared=shared[:m].copy(), median=median[:m].copy(), identity=ident[:m].copy(),
+                    pvalue=pv[:m].copy(), set_size=set_size.value)
+
+    def reset(self):
+        """Start a new sample: hit counters and the mixture list emptied, the table kept."""
+        self.eng._check(self.eng.lib.mashgpu_screen_reset(self.h))
+
+    def hits_stats(self):
+        """Of the last finish_hits(): dict(hit_hashes, hit_pairs, index_ms (the one-off index build), finish_ms)."""
+        hh = C.c_uint64(0); hp = C.c_uint64(0); ims = C.c_double(0); fms = C.c_double(0)
+        self.eng._check(self.eng.lib.mashgpu_screen_hits_stats(self.h, C.byref(hh), C.byref(hp), C.byref(ims), C.byref(fms)))
+        return dict(hit_hashes=hh.value, hit_pairs=hp.value, index_ms=ims.value, finish_ms=fms.value)
 
     def taxonomy(self, tax, ref_code, unknown_taxid=(), hash_taxid=False):
         """`mash taxscreen` after the last feed: LCA taxon of every distinct hash, per-taxon counts and their roll-up.

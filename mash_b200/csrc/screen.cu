@@ -17,7 +17,10 @@
 #include <cmath>
 #include <cstring>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_merge_sort.cuh>
+#include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
+#include <thrust/iterator/counting_iterator.h>
 
 #include <chrono>
 #include <vector>
@@ -130,6 +133,20 @@ __global__ void __launch_bounds__(SCR_THREADS) merge_bottom_s_kernel(uint64_t *m
     }
 }
 
+// identity and p-value of a sketch of n hashes with `shared` of them seen; the dense and the sparse reduce both call this, so
+// their values are the same bits
+__device__ __forceinline__ void screen_estimates(uint32_t shared, uint32_t n, uint64_t set_size, int kmer_size, double kmer_space,
+                                                 double *identity_out, double *pvalue_out)
+{
+    double identity;                                                             // estimateIdentity, :463-482
+    if (shared == n) identity = 1.;
+    else if (shared == 0) identity = 0.;
+    else identity = pow((double)shared / (double)n, 1. / kmer_size);
+    *identity_out = identity;
+    // pValueWithin, :601-615
+    *pvalue_out = shared == 0 ? 1.0 : binomial_upper_tail(shared, (double)set_size / kmer_space, n);
+}
+
 // One CTA per reference sketch: shared count, sorted depths -> median, identity, p-value.
 __global__ void __launch_bounds__(SCR_THREADS) screen_reduce_kernel(
     const uint64_t *hashes, uint64_t stride, const uint32_t *n_hashes, const uint64_t *keys, const uint32_t *slot_idx, const uint32_t *cnt, uint32_t log2cap,
@@ -179,13 +196,7 @@ __global__ void __launch_bounds__(SCR_THREADS) screen_reduce_kernel(
     if (threadIdx.x == 0) {
         shared_out[r] = shared;
         median_out[r] = shared > 0 ? depths[shared / 2] : 0;                      // :436
-        double identity;                                                         // estimateIdentity, :463-482
-        if (shared == n) identity = 1.;
-        else if (shared == 0) identity = 0.;
-        else identity = pow((double)shared / (double)n, 1. / kmer_size);
-        identity_out[r] = identity;
-        // pValueWithin, :601-615
-        pvalue_out[r] = shared == 0 ? 1.0 : binomial_upper_tail(shared, (double)set_size / kmer_space, n);
+        screen_estimates(shared, n, set_size, kmer_size, kmer_space, &identity_out[r], &pvalue_out[r]);
     }
 }
 
@@ -218,6 +229,8 @@ __global__ void __launch_bounds__(SCR_THREADS) screen_winner_kernel(
 
 }  // namespace mashgpu
 
+#include "screen_hits.cuh"
+
 using namespace mashgpu;
 
 struct mashgpu_screen_job {
@@ -244,7 +257,11 @@ struct mashgpu_screen_job {
     bool pending = false;            // a chunk's kernels are in flight (ticket + mixture read-back not yet collected)
     DevBuf<uint64_t> d_mix_top; PinnedBuf<uint64_t> h_mix_top2;      // {n, top} of the mixture after the chunk in flight
     PinnedBuf<uint8_t> acc; uint64_t acc_len = 0;                    // small host chunks are joined here before they are fed
-    ~mashgpu_screen_job() { for (int b = 0; b < 2; b++) if (copied[b]) cudaEventDestroy(copied[b]); }
+    ~mashgpu_screen_job()
+    {
+        for (int b = 0; b < 2; b++) if (copied[b]) cudaEventDestroy(copied[b]);
+        for (int b = 0; b < 2; b++) if (hit_ev[b]) cudaEventDestroy(hit_ev[b]);
+    }
     bool winner = false;     // -w
     std::vector<uint64_t> h_len;      // Reference::length per sketch (tie break of -w), zeros when the caller gave none
     std::vector<uint32_t> h_n;        // hashes per sketch
@@ -253,6 +270,23 @@ struct mashgpu_screen_job {
     // scanned; a slot's buffer stays untouched until its chunk is collected (the exact re-run reads it again)
     bool translate = false;
     DevBuf<uint8_t> pep[2];
+    // sparse finish (screen_hits.cuh): the inverted index distinct hash -> sketches, built at the first finish_hits, and scratch
+    // sized then for a sample that hits every pair
+    bool index_built = false;
+    uint64_t n_pairs = 0;
+    DevBuf<uint32_t> seg_start, seg_ref;                 // index: seg_ref[seg_start[d] .. seg_start[d + 1]) = sketches holding d
+    DevBuf<uint32_t> hit_d, long_list, best;             // per hit (n_distinct)
+    DevBuf<uint32_t> ref_cnt, ref_start, rows_ref, order, prio;      // per sketch (n_ref + 1)
+    DevBuf<uint32_t> depths;                             // per pair
+    DevBuf<uint32_t> hit_n;                              // {hits, long segments, rows}
+    DevBuf<uint64_t> d_len, out_shared, out_median;
+    DevBuf<double> out_ident, out_pv;
+    DevBuf<uint8_t> hit_tmp; size_t hit_tmp_bytes = 0;
+    PinnedBuf<uint32_t> h_hit;                           // read-backs: n_hit, rows, pairs
+    cudaEvent_t hit_ev[2] = {nullptr, nullptr};
+    double index_ms = 0, finish_ms = 0;
+    uint64_t last_hits = 0, last_pairs = 0;
+    bool hits_valid = false;         // hit_d[0 .. last_hits) lists every nonzero counter (no feed since the last finish_hits)
 };
 
 namespace {
@@ -410,6 +444,7 @@ int screen_enqueue(mashgpu_screen_job *job, int slot, const void *d_chunk, uint6
     S.d_stream = d_chunk; S.d_codes = d_codes; S.d_inval = d_inval; S.unit_start = unit_start; S.n_units = 1; S.data_ready = data_ready;
     if (job->h_mix_n == s) { S.t_cap = true; S.t_cap_value = job->h_mix_top; }   // nothing above the running s-th smallest can matter
     ScreenProbe probe{job->keys.p, job->slot_idx.p, job->cnt.p, job->log2cap, job->hmax, job->bitmap.p, job->bitmap_shift};
+    job->hits_valid = false;
     MG_CUDA(ctx, cudaMemsetAsync(job->chunk_n.p, 0, 4, st));      // an overflowing chunk leaves an empty list until its exact re-run
     MG_TRY(sketch_stream_enqueue(ctx, &job->params, S, job->chunk_hashes.p, nullptr, job->chunk_n.p, st, &probe, job->ticket));
     uint32_t N = 2;
@@ -685,6 +720,7 @@ extern "C" int mashgpu_screen_counters(mashgpu_screen_job *job, uint32_t **d_cou
     MG_TRY(screen_flush_acc(job));
     MG_TRY(screen_collect(job));
     cudaStreamSynchronize(job->ctx->stream);
+    job->hits_valid = false;         // the caller may write the counters
     *d_counters = job->cnt.p;
     *n_slots = job->n_distinct;
     return MASHGPU_OK;
@@ -770,6 +806,219 @@ int mashgpu::screen_table_view(mashgpu_screen_job *job, ScreenTableView *v)
     MG_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *v = ScreenTableView{ctx, job->n_ref, job->stride, job->ref_hashes, job->ref_n, job->h_n.data(), job->keys.p, job->slot_idx.p, job->cnt.p,
                          job->log2cap, job->n_distinct};
+    return MASHGPU_OK;
+}
+
+namespace {
+
+// The inverted index and the per-sample scratch of the sparse finish, once per job.  The counting sort runs over every (sketch,
+// hash) pair; seg_start is 32-bit, so a job of 2^32 or more pairs is refused.  Device memory: 4 B per pair for the index and 4 B per
+// pair for the depth runs, 4 B per distinct hash for seg_start plus 12 B for the hit lists, about 60 B per sketch, and 8 B per pair
+// of build temporaries.
+int screen_build_index(mashgpu_screen_job *job)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint64_t n = job->n_ref, nd = job->n_distinct;
+    uint64_t n_pairs = 0;
+    std::vector<uint64_t> off(n);
+    std::vector<uint32_t> iota(n);
+    for (uint64_t r = 0; r < n; r++) { off[r] = n_pairs; iota[r] = (uint32_t)r; n_pairs += job->h_n[r]; }
+    if (n_pairs >= 0xFFFFFFFFull || n >= 0x7FFFFFFFull)
+        return fail(ctx, MASHGPU_ERR_UNSUPPORTED, "sparse screen finish: 2^32 or more (sketch, hash) pairs");
+    size_t tb[4] = {0, 0, 0, 0};
+    thrust::counting_iterator<uint32_t> it(0);
+    MG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(nullptr, tb[0], job->seg_start.p, job->seg_start.p, (int)std::max<uint64_t>(nd, n) + 1, st));
+    MG_CUDA(ctx, cub::DeviceSelect::If(nullptr, tb[1], it, job->hit_d.p, job->hit_n.p, (int)nd, HitPred{job->cnt.p}, st));
+    MG_CUDA(ctx, cub::DeviceSelect::If(nullptr, tb[2], it, job->rows_ref.p, job->hit_n.p, (int)n, RefPred{job->ref_cnt.p}, st));
+    MG_CUDA(ctx, cub::DeviceMergeSort::SortKeys(nullptr, tb[3], job->order.p, (int)n, WinnerOrder{nullptr, nullptr, nullptr}, st));
+    job->hit_tmp_bytes = *std::max_element(tb, tb + 4);
+    DevBuf<uint32_t> d_iota, pair_d, seg_n; DevBuf<uint64_t> d_off;
+    if (job->seg_start.alloc(nd + 1) != cudaSuccess || job->seg_ref.alloc(n_pairs) != cudaSuccess || job->hit_d.alloc(nd) != cudaSuccess ||
+        job->long_list.alloc(nd) != cudaSuccess || job->best.alloc(nd) != cudaSuccess || job->ref_cnt.alloc(n + 1) != cudaSuccess ||
+        job->ref_start.alloc(n + 1) != cudaSuccess || job->rows_ref.alloc(n) != cudaSuccess || job->order.alloc(n) != cudaSuccess ||
+        job->prio.alloc(n) != cudaSuccess || job->depths.alloc(n_pairs) != cudaSuccess || job->hit_n.alloc(3) != cudaSuccess ||
+        job->d_len.alloc(n) != cudaSuccess || job->out_shared.alloc(n) != cudaSuccess || job->out_median.alloc(n) != cudaSuccess ||
+        job->out_ident.alloc(n) != cudaSuccess || job->out_pv.alloc(n) != cudaSuccess || job->hit_tmp.alloc(job->hit_tmp_bytes) != cudaSuccess ||
+        job->h_hit.alloc(4) != cudaSuccess ||
+        d_iota.alloc(n) != cudaSuccess || d_off.alloc(n) != cudaSuccess || pair_d.alloc(n_pairs) != cudaSuccess || seg_n.alloc(nd + 1) != cudaSuccess)
+        return fail(ctx, MASHGPU_ERR_NOMEM, "out of device memory (sparse screen index: %llu pairs, %llu hashes)", (unsigned long long)n_pairs, (unsigned long long)nd);
+    for (int b = 0; b < 2; b++)
+        if (!job->hit_ev[b]) MG_CUDA(ctx, cudaEventCreate(&job->hit_ev[b]));
+    MG_CUDA(ctx, cudaEventRecord(job->hit_ev[0], st));
+    MG_CUDA(ctx, cudaMemcpyAsync(d_iota.p, iota.data(), n * 4, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(d_off.p, off.data(), n * 8, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->d_len.p, job->h_len.data(), n * 8, cudaMemcpyHostToDevice, st));
+    MG_CUDA(ctx, cudaMemsetAsync(seg_n.p, 0, (nd + 1) * 4, st));
+    MG_CUDA(ctx, cudaMemsetAsync(job->ref_cnt.p, 0, (n + 1) * 4, st));       // kept at zero from here on (screen_hits.cuh)
+    if (n_pairs) {
+        tax_pairs_kernel<<<(unsigned)n, SCR_THREADS, 0, st>>>(job->ref_hashes, job->stride, job->ref_n, d_iota.p, d_off.p, job->keys.p, job->slot_idx.p,
+                                                            job->log2cap, pair_d.p, seg_n.p);
+        MG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(job->hit_tmp.p, job->hit_tmp_bytes, seg_n.p, job->seg_start.p, (int)(nd + 1), st));
+        tax_scatter_kernel<<<(unsigned)n, SCR_THREADS, 0, st>>>(job->ref_n, d_iota.p, d_iota.p, d_off.p, pair_d.p, job->seg_start.p, seg_n.p, job->seg_ref.p);
+        ctx->kernel_launches += 3;
+    }
+    MG_CUDA(ctx, cudaGetLastError());
+    MG_CUDA(ctx, cudaEventRecord(job->hit_ev[1], st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));                 // the temporaries go out of scope
+    float ms = 0;
+    MG_CUDA(ctx, cudaEventElapsedTime(&ms, job->hit_ev[0], job->hit_ev[1]));
+    job->index_ms = ms;
+    job->n_pairs = n_pairs;
+    job->index_built = true;
+    return MASHGPU_OK;
+}
+
+// ExclusiveSum of ref_cnt[0 .. n] -> ref_start, then the sketches with ref_cnt > 0 -> rows_ref (ascending) and their number and the
+// pair total to the host
+int screen_hits_runs(mashgpu_screen_job *job, uint32_t *n_rows, uint32_t *n_pairs)
+{
+    mashgpu_ctx *ctx = job->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint64_t n = job->n_ref;
+    thrust::counting_iterator<uint32_t> it(0);
+    size_t tb = job->hit_tmp_bytes;
+    MG_CUDA(ctx, cub::DeviceScan::ExclusiveSum(job->hit_tmp.p, tb, job->ref_cnt.p, job->ref_start.p, (int)(n + 1), st));
+    tb = job->hit_tmp_bytes;
+    MG_CUDA(ctx, cub::DeviceSelect::If(job->hit_tmp.p, tb, it, job->rows_ref.p, job->hit_n.p + 2, (int)n, RefPred{job->ref_cnt.p}, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->h_hit.p, job->hit_n.p + 2, 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->h_hit.p + 1, job->ref_start.p + n, 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    *n_rows = job->h_hit.p[0];
+    *n_pairs = job->h_hit.p[1];
+    return MASHGPU_OK;
+}
+
+}  // namespace
+
+extern "C" int mashgpu_screen_finish_hits(mashgpu_screen_job *job, uint32_t *ref, uint64_t *shared, uint64_t *median, double *identity,
+                                          double *pvalue, uint64_t *n_rows, uint64_t *set_size_out)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    if (!n_rows) return fail(ctx, MASHGPU_ERR_INVALID, "n_rows is NULL");
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    MG_TRY(screen_flush_acc(job));
+    MG_TRY(screen_collect(job));
+    cudaStream_t st = ctx->stream;
+    const int k = job->params.kmer_size;
+    int asize = 0;
+    for (int i = 0; i < 256; i++) asize += job->params.alphabet[i] != 0;
+    const double kmer_space = std::pow((double)asize, (double)k);
+    uint64_t set_size = 0;             // as mashgpu_screen_finish
+    if (job->h_mix_n)
+        set_size = (uint64_t)(std::pow(2.0, job->params.use64 ? 64.0 : 32.0) * (double)job->h_mix_n / (double)job->h_mix_top);
+    if (set_size_out) *set_size_out = set_size;
+    *n_rows = 0;
+    job->last_hits = job->last_pairs = 0;
+    job->finish_ms = 0;
+    const uint64_t n = job->n_ref, nd = job->n_distinct;
+    if (n == 0 || nd == 0) { job->hits_valid = true; return MASHGPU_OK; }
+    if (!job->index_built) MG_TRY(screen_build_index(job));
+    MG_CUDA(ctx, cudaEventRecord(job->hit_ev[0], st));
+    // hits: every distinct index with cnt >= 1, ascending
+    thrust::counting_iterator<uint32_t> it(0);
+    size_t tb = job->hit_tmp_bytes;
+    MG_CUDA(ctx, cub::DeviceSelect::If(job->hit_tmp.p, tb, it, job->hit_d.p, job->hit_n.p, (int)nd, HitPred{job->cnt.p}, st));
+    MG_CUDA(ctx, cudaMemsetAsync(job->hit_n.p + 1, 0, 4, st));
+    MG_CUDA(ctx, cudaMemcpyAsync(job->h_hit.p, job->hit_n.p, 4, cudaMemcpyDeviceToHost, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    const uint32_t n_hit = job->h_hit.p[0];
+    uint32_t rows = 0, pairs = 0;
+    if (n_hit) {
+        const unsigned blocks = (n_hit + SCR_THREADS - 1) / SCR_THREADS, long_blocks = (unsigned)ctx->sm_count * 8;
+        const uint32_t *hit_d = job->hit_d.p, *seg_start = job->seg_start.p, *seg_ref = job->seg_ref.p, *cnt = job->cnt.p;
+        uint32_t *ref_cnt = job->ref_cnt.p, *ref_start = job->ref_start.p, *depths = job->depths.p, *long_list = job->long_list.p, *n_long = job->hit_n.p + 1;
+        // per-sketch counts over the hit segments (queueing the long ones), runs, and the depths scattered into them
+        hits_pairs_kernel<false><<<blocks, SCR_THREADS, 0, st>>>(hit_d, n_hit, seg_start, seg_ref, cnt, ref_start, ref_cnt, depths, long_list, n_long, true);
+        hits_pairs_long_kernel<false><<<long_blocks, SCR_THREADS, 0, st>>>(hit_d, seg_start, seg_ref, cnt, ref_start, ref_cnt, depths, long_list, n_long);
+        ctx->kernel_launches += 2;
+        MG_CUDA(ctx, cudaGetLastError());
+        MG_TRY(screen_hits_runs(job, &rows, &pairs));
+        job->last_pairs = pairs;
+        if (job->winner) {
+            // rank the hit sketches by their plain counts, give each hit to the best-ranked sketch holding it, and count again
+            MG_CUDA(ctx, cudaMemcpyAsync(job->order.p, job->rows_ref.p, rows * 4ull, cudaMemcpyDeviceToDevice, st));
+            tb = job->hit_tmp_bytes;
+            MG_CUDA(ctx, cub::DeviceMergeSort::SortKeys(job->hit_tmp.p, tb, job->order.p, (int)rows, WinnerOrder{ref_start, job->ref_n, job->d_len.p}, st));
+            hits_rank_kernel<<<(rows + SCR_THREADS - 1) / SCR_THREADS, SCR_THREADS, 0, st>>>(job->order.p, rows, job->prio.p);
+            hits_best_kernel<<<blocks, SCR_THREADS, 0, st>>>(hit_d, n_hit, seg_start, seg_ref, job->prio.p, job->best.p);
+            hits_best_long_kernel<<<long_blocks, SCR_THREADS, 0, st>>>(hit_d, seg_start, seg_ref, job->prio.p, long_list, n_long, job->best.p);
+            // the plain runs are not needed: their counters go back to 0, then the winners are counted
+            clear_listed_kernel<<<(rows + SCR_THREADS - 1) / SCR_THREADS, SCR_THREADS, 0, st>>>(job->rows_ref.p, rows, ref_cnt);
+            hits_winner_kernel<false><<<blocks, SCR_THREADS, 0, st>>>(hit_d, n_hit, job->best.p, job->order.p, cnt, ref_start, ref_cnt, depths);
+            ctx->kernel_launches += 6;
+            MG_CUDA(ctx, cudaGetLastError());
+            uint32_t winner_pairs = 0;
+            MG_TRY(screen_hits_runs(job, &rows, &winner_pairs));
+            hits_winner_kernel<true><<<blocks, SCR_THREADS, 0, st>>>(hit_d, n_hit, job->best.p, job->order.p, cnt, ref_start, ref_cnt, depths);
+        } else {
+            hits_pairs_kernel<true><<<blocks, SCR_THREADS, 0, st>>>(hit_d, n_hit, seg_start, seg_ref, cnt, ref_start, ref_cnt, depths, long_list, n_long, false);
+            hits_pairs_long_kernel<true><<<long_blocks, SCR_THREADS, 0, st>>>(hit_d, seg_start, seg_ref, cnt, ref_start, ref_cnt, depths, long_list, n_long);
+            ctx->kernel_launches++;
+        }
+        ctx->kernel_launches++;
+        uint32_t N = 2;
+        while (N < job->max_n) N <<= 1;         // <= SCREEN_MAX_REF_HASHES (refused at open): 128 KB
+        if ((size_t)N * 4 > 48 * 1024)
+            MG_CUDA(ctx, cudaFuncSetAttribute(hits_reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)((size_t)N * 4)));
+        if (rows) {
+            hits_reduce_kernel<<<rows, SCR_THREADS, (size_t)N * 4, st>>>(job->rows_ref.p, ref_start, depths, job->ref_n, set_size, k, kmer_space,
+                                                                        job->out_shared.p, job->out_median.p, job->out_ident.p, job->out_pv.p);
+            ctx->kernel_launches++;
+        }
+        MG_CUDA(ctx, cudaGetLastError());
+    }
+    MG_CUDA(ctx, cudaEventRecord(job->hit_ev[1], st));
+    if (rows) {
+        if (ref) MG_CUDA(ctx, cudaMemcpyAsync(ref, job->rows_ref.p, rows * 4ull, cudaMemcpyDeviceToHost, st));
+        if (shared) MG_CUDA(ctx, cudaMemcpyAsync(shared, job->out_shared.p, rows * 8ull, cudaMemcpyDeviceToHost, st));
+        if (median) MG_CUDA(ctx, cudaMemcpyAsync(median, job->out_median.p, rows * 8ull, cudaMemcpyDeviceToHost, st));
+        if (identity) MG_CUDA(ctx, cudaMemcpyAsync(identity, job->out_ident.p, rows * 8ull, cudaMemcpyDeviceToHost, st));
+        if (pvalue) MG_CUDA(ctx, cudaMemcpyAsync(pvalue, job->out_pv.p, rows * 8ull, cudaMemcpyDeviceToHost, st));
+    }
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    float ms = 0;
+    MG_CUDA(ctx, cudaEventElapsedTime(&ms, job->hit_ev[0], job->hit_ev[1]));
+    job->finish_ms = ms;
+    job->last_hits = n_hit;
+    job->hits_valid = true;
+    *n_rows = rows;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_screen_hits_stats(mashgpu_screen_job *job, uint64_t *hit_hashes, uint64_t *hit_pairs, double *index_ms, double *finish_ms)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    if (hit_hashes) *hit_hashes = job->last_hits;
+    if (hit_pairs) *hit_pairs = job->last_pairs;
+    if (index_ms) *index_ms = job->index_ms;
+    if (finish_ms) *finish_ms = job->finish_ms;
+    return MASHGPU_OK;
+}
+
+extern "C" int mashgpu_screen_reset(mashgpu_screen_job *job)
+{
+    if (!job) return MASHGPU_ERR_INVALID;
+    mashgpu_ctx *ctx = job->ctx;
+    MG_CUDA(ctx, cudaSetDevice(ctx->device));
+    MG_TRY(screen_flush_acc(job));               // the joined small chunks belong to the sample being closed
+    MG_TRY(screen_collect(job));
+    cudaStream_t st = ctx->stream;
+    if (job->hits_valid) {
+        if (job->last_hits) {
+            clear_listed_kernel<<<(unsigned)((job->last_hits + SCR_THREADS - 1) / SCR_THREADS), SCR_THREADS, 0, st>>>(job->hit_d.p, (uint32_t)job->last_hits, job->cnt.p);
+            ctx->kernel_launches++;
+            MG_CUDA(ctx, cudaGetLastError());
+        }
+    } else if (job->n_distinct) {
+        MG_CUDA(ctx, cudaMemsetAsync(job->cnt.p, 0, job->n_distinct * 4, st));
+    }
+    MG_CUDA(ctx, cudaMemsetAsync(job->mix_n.p, 0, 4, st));
+    MG_CUDA(ctx, cudaStreamSynchronize(st));
+    job->h_mix_n = 0;
+    job->h_mix_top = 0;
+    job->hits_valid = false;
     return MASHGPU_OK;
 }
 

@@ -7,7 +7,9 @@
 // spanning forest) have no counterpart in the reference: its users compute both from the `-E` output.  Nor has `triangle -N` (the
 // neighbor-joining tree as a Newick line), which its users compute from the matrix with an NJ program, nor `triangle -L` (average
 // or complete linkage as a Newick line, or its flat clusters at `-d`), which its users compute from the matrix with scipy, nor
-// `triangle -R` (greedy representatives, the dereplication of CD-HIT and skDER), which its users run over the `-E` output.
+// `triangle -R` (greedy representatives, the dereplication of CD-HIT and skDER), which its users run over the `-E` output, nor
+// `screen -I` (each mixture argument screened as its own sample against one table kept on the GPU), which its users get from
+// one `mash screen` process per sample.
 #include <chrono>
 #include <algorithm>
 #include <cmath>
@@ -792,20 +794,17 @@ int runTriangle(int argc, const char **argv)
 
 // ---------------------------------------------------------------------------------------------------- screen
 // The stream of `mash screen` and `mash taxscreen` (CommandScreen.cpp:156-270, CommandTaxScreen.cpp:212-384): round robin over
-// the input files arguments[1..], '*'-joined chunks of 64 MiB instead of 1 MiB (any split gives the same counts) fed to the
-// job.  Exits with the reference's messages on a bad input.
-void streamInputs(mashgpu_screen_job *job, const vector<string> &arguments, int kmerSize, bool trans)
+// the input files, '*'-joined chunks of 64 MiB instead of 1 MiB (any split gives the same counts) fed to the job.  Returns the
+// number of sequence records; exits with the reference's messages on a file it cannot open or read.
+uint64_t feedInputs(mashgpu_screen_job *job, const vector<string> &files, int kmerSize)
 {
-    int queryCount = (int)arguments.size() - 1;
-    cerr << (trans ? "Translating from " : "Streaming from ");
-    if (queryCount == 1) cerr << arguments[1]; else cerr << queryCount << " inputs";
-    cerr << "..." << endl;
     vector<gzFile> fps;
     std::vector<mashhost::FastxReader *> readers;
-    for (size_t f = 1; f < arguments.size(); f++) {
-        if (arguments[f] == "-" && f > 1) { cerr << "ERROR: '-' for stdin must be first query" << endl; exit(1); }
-        gzFile fp = mashhost::FastxReader::openPath(arguments[f]);
-        if (fp == 0) { cerr << "ERROR: could not open " << arguments[f] << endl; exit(1); }
+    for (size_t f = 0; f < files.size(); f++) {
+        const string &file = files[f];
+        if (file == "-" && f > 0) { cerr << "ERROR: '-' for stdin must be first query" << endl; exit(1); }
+        gzFile fp = mashhost::FastxReader::openPath(file);
+        if (fp == 0) { cerr << "ERROR: could not open " << file << endl; exit(1); }
         fps.push_back(fp);
         readers.push_back(new mashhost::FastxReader(fp));
     }
@@ -842,7 +841,59 @@ void streamInputs(mashgpu_screen_job *job, const vector<string> &arguments, int 
     flush();
     if (lstate != -1) { cerr << "\nERROR: reading inputs" << endl; exit(1); }
     for (gzFile fp : fps) gzclose(fp);
+    return count;
+}
+
+// all inputs arguments[1..] pooled into one mixture
+void streamInputs(mashgpu_screen_job *job, const vector<string> &arguments, int kmerSize, bool trans)
+{
+    int queryCount = (int)arguments.size() - 1;
+    cerr << (trans ? "Translating from " : "Streaming from ");
+    if (queryCount == 1) cerr << arguments[1]; else cerr << queryCount << " inputs";
+    cerr << "..." << endl;
+    const uint64_t count = feedInputs(job, vector<string>(arguments.begin() + 1, arguments.end()), kmerSize);
     if (count == 0) { cerr << "\nERROR: Did not find sequence records in inputs" << endl; exit(1); }
+}
+
+// `mash screen -I`: every input arguments[1..] is a sample of its own, screened against the one table the job holds.  Per sample:
+// stream the file, take the rows of the references it hit (mashgpu_screen_finish_hits) and print them after a column naming the
+// sample, then reset the job for the next one.  A sample without records gets a warning and no rows.
+void screenSamples(mashgpu_screen_job *job, const vector<string> &arguments, const Sketch &sketch, int kmerSize, bool trans,
+                   double identityMin, double pValueMax)
+{
+    for (size_t f = 2; f < arguments.size(); f++)
+        if (arguments[f] == "-") { cerr << "ERROR: '-' for stdin must be first query" << endl; exit(1); }
+    const uint64_t n = sketch.getReferenceCount();
+    vector<uint32_t> ref(n); vector<uint64_t> shared(n), median(n); vector<double> identity(n), pValue(n);
+    for (size_t f = 1; f < arguments.size(); f++) {
+        const string &sample = arguments[f];
+        cerr << (trans ? "Translating from " : "Streaming from ") << sample << "..." << endl;
+        if (feedInputs(job, vector<string>(1, sample), kmerSize) == 0) {
+            cerr << "WARNING: Did not find sequence records in " << sample << endl;
+            if (mashgpu_screen_reset(job) != MASHGPU_OK) gpuFail();
+            continue;
+        }
+        uint64_t rows = 0, setSize = 0;
+        if (mashgpu_screen_finish_hits(job, ref.data(), shared.data(), median.data(), identity.data(), pValue.data(), &rows, &setSize) != MASHGPU_OK)
+            gpuFail();
+        cerr << "   Estimated distinct" << (trans ? " (translated)" : "") << " k-mers in " << sample << ": " << setSize << endl;
+        if (setSize == 0) cerr << "WARNING: no valid k-mers in " << sample << "." << endl;
+        // rows of every reference under -i < 0; the ones the sample did not hit take the values of a reference with shared 0
+        uint64_t row = 0;
+        for (uint64_t i = 0; i < n; i++) {                   // reference CommandScreen.cpp:418-455
+            const bool hit = row < rows && ref[row] == i;
+            if (!hit && identityMin >= 0.0) continue;
+            const size_t size = sketch.getReference(i).hashesSorted.size();
+            const uint64_t sh = hit ? shared[row] : 0, med = hit ? median[row] : 0;
+            const double id = hit ? identity[row] : (size == 0 ? 1. : 0.), pv = hit ? pValue[row] : 1.0;
+            if (hit) row++;
+            if (id < identityMin) continue;
+            if (pv > pValueMax) continue;
+            cout << sample << '\t' << id << '\t' << sh << '/' << size << '\t' << med << '\t' << pv
+                 << '\t' << sketch.getReference(i).name << '\t' << sketch.getReference(i).comment << endl;
+        }
+        if (mashgpu_screen_reset(job) != MASHGPU_OK) gpuFail();
+    }
 }
 
 int runScreen(int argc, const char **argv)
@@ -853,8 +904,13 @@ int runScreen(int argc, const char **argv)
     c.add("winning!", Option(Option::Boolean, "w", ""));
     c.add("identity", Option(Option::Number, "i", "0", -1., 1.));
     c.add("pvalue", Option(Option::Number, "v", "1.0", 0., 1.));
+    c.add("samples", Option(Option::Boolean, "I", ""));     // not an option of the reference: its users run one screen per sample
     if (c.parse(argc, argv)) return 1;
-    if (c.arguments.size() < 2 || c.opt("help").active) { cerr << "usage: mash screen [options] <queries>.msh <mixture> [<mixture>] ..." << endl; return 0; }
+    if (c.arguments.size() < 2 || c.opt("help").active) {
+        cerr << "usage: mash screen [options] <queries>.msh <mixture> [<mixture>] ...\n"
+                "       mash screen -I [options] <queries>.msh <sample> [<sample>] ...   (each sample screened on its own; rows prefixed by the sample)" << endl;
+        return 0;
+    }
     if (!hasSuffix(c.arguments[0], suffixSketch)) {
         cerr << "ERROR: " << c.arguments[0] << " does not look like a sketch (.msh)" << endl;
         exit(1);
@@ -877,6 +933,11 @@ int runScreen(int argc, const char **argv)
     mashgpu_screen_job *job = 0;
     if (mashgpu_screen_open(gpuContext(), &p, &set, &job) != MASHGPU_OK) gpuFail();
     if (c.opt("winning!").active && mashgpu_screen_set_winner(job, 1) != MASHGPU_OK) gpuFail();     // -w, CommandScreen.cpp:357-407
+    if (c.opt("samples").active) {
+        screenSamples(job, c.arguments, sketch, parameters.kmerSize, trans, identityMin, pValueMax);
+        mashgpu_screen_close(job);
+        return 0;
+    }
     streamInputs(job, c.arguments, parameters.kmerSize, trans);
     const uint64_t n = sketch.getReferenceCount();
     vector<uint64_t> shared(n), median(n); vector<double> identity(n), pValue(n);
